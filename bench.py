@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — headline benchmark of the B200 LSM compaction / read engine (BASELINE.json metric:
+"""bench.py — headline benchmark of the H100 LSM compaction / read engine (BASELINE.json metric:
 compaction merged-GB/s + scan keys/s, next to the CPU path).
 
 One "step" = one L0->L1 compaction of one hash partition (BASELINE.json configs[1]: 4 sorted runs x
@@ -13,8 +13,7 @@ collective on the data path (hash partitions are independent, SURVEY.md §8e).
              (pinned host memory -> HBM, device index + Bloom build) + compaction + result struct back.
   roofline = the merge kernels (k_walk + k_emit, back to back on one stream): algorithmic bytes (B_in + B_out,
              key+value only) / their CUDA-event duration, against the measured HBM copy bandwidth in
-             MEASURED_PEAKS.json; `traffic` is the DRAM byte count of an ncu capture of the same launch
-             (profiles/traffic_r02.json), labelled with its source, or null.
+             MEASURED_PEAKS.json (else the H100 data-sheet figure, labelled as such).
   cpu_baseline = the oracle's block-level CPU compaction (heap merging iterator -> filter -> block builder,
              all host threads) on the SAME full workload (independent of the core count); its statistics are
              compared with the device's (`parity_checked`).  It is the oracle port, not RocksDB itself (RocksDB
@@ -27,12 +26,21 @@ collective on the data path (hash partitions are independent, SURVEY.md §8e).
              sizes 8..256 MB, bottommost forced, roofline fraction per size.
   ycsb_a   = BASELINE.json configs[4] at small scale (N=1): 50/50 put+get through the rrdb surface.
 
-Usage: python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+--steps K is the number of timed repetitions of every leg.  --dump-outputs DIR writes what the timed path computed as
+DIR/<name>.npy (float32 or float64, about 10 MB whatever the sizes): the records of the last timed compaction (record
+statistics, a SHA-256 of the whole decoded record stream, the records at a seeded sample of record indices; nothing
+that depends on where the output is cut into blocks) and, per request of a seeded sample, the answers of the last
+timed get and prefix-scan batches including a hash of the returned bytes.  With --impl reference it writes the
+compaction arrays of the CPU path under the same names.  The inputs are generated from fixed seeds, so two builds
+can be compared output for output.
+
+Usage: python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
 """
 from __future__ import annotations
 
 import argparse
 import ctypes as C
+import hashlib
 import json
 import os
 import subprocess
@@ -44,6 +52,7 @@ from concurrent.futures import ThreadPoolExecutor
 import numpy as np
 
 ROOT = os.path.dirname(os.path.abspath(__file__))
+sys.dont_write_bytecode = True  # the benchmark leaves the tree as it found it (it may be read-only)
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "oracle"))
 
@@ -60,19 +69,7 @@ def load_peaks():
         with open(p) as f:
             j = json.load(f)
         return float(j["hbm_gbs"]), "measured (MEASURED_PEAKS.json, torch copy)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
-
-
-def load_traffic():
-    """DRAM bytes per launch from the committed ncu captures (tools/summarize_profiles.py writes the file)"""
-    p = os.path.join(ROOT, "profiles", "traffic_r02.json")
-    if os.path.exists(p):
-        try:
-            with open(p) as f:
-                return json.load(f)
-        except Exception:
-            return {}
-    return {}
+    return 3350.0, "H100 SXM data sheet HBM3 bandwidth (not measured)"
 
 
 def workload_config(records_per_run: int) -> dict:
@@ -113,6 +110,16 @@ class ClockSampler(threading.Thread):
                 "samples": len(sm)}
 
 
+def power_limit(index: int):
+    """the card's power limit in W (numbers measured on it are only comparable at the same limit), None if unknown"""
+    try:
+        out = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader,nounits", "-i", str(index)],
+                             capture_output=True, text=True, timeout=5).stdout.strip()
+        return float(out)
+    except Exception:
+        return None
+
+
 def gen_runs(records_per_run: int, seed: int):
     from incubator_pegasus_b200 import synth
     return synth.compaction_runs(k=RUNS, n_per_run=records_per_run, hk_len=HK, sk_len=SK, user_len=VAL, now=NOW,
@@ -126,11 +133,11 @@ def cpu_block_runs(runs):
 
 
 def cpu_compaction(bruns, threads: int):
-    """oracle block-level compaction on host cores; returns (merged GB/s, seconds, stats)."""
+    """oracle block-level compaction on host cores; returns (merged GB/s, seconds, stats, merged block run)."""
     import oracle_py as orc
     fp = orc.filter_params(enabled=True)
-    _out, st, secs = orc.compact_blocks(bruns, True, fp, NOW, threads)
-    return st.in_bytes / secs / 1e9, secs, st
+    out, st, secs = orc.compact_blocks(bruns, True, fp, NOW, threads)
+    return st.in_bytes / secs / 1e9, secs, st, out
 
 
 def zipf_ids(rng, n_items: int, n: int, theta: float = 0.99):
@@ -167,8 +174,10 @@ def reference_arm(args, rank: int, world: int):
     bruns = cpu_block_runs(gen_runs(n, 1000))
     vals = []
     for _ in range(args.warmup + args.steps):
-        gbs, secs, st = cpu_compaction(bruns, threads)
+        gbs, secs, st, out = cpu_compaction(bruns, threads)
         vals.append((gbs, secs))
+    if args.dump_outputs:
+        write_outputs(args.dump_outputs, compaction_outputs(st, out.decode().records()))
     in_bytes = int(st.in_bytes)
     timed = vals[args.warmup:]
     ms = 1e3 * sum(s for _, s in timed) / len(timed)
@@ -273,7 +282,7 @@ def sharded_read_leg(pgs, torch, dist, eng, rank, world, args, barrier, check_cp
     list(pool.map(serve, work))  # warm-up pass (also the answer that is checked below)
     first = dict(tot)
     verify[0] = False
-    reps = max(3, args.steps)
+    reps = args.steps
     walls = []
     for _ in range(reps):
         tot.update(found=0, returned=0, kernel_ms=0.0, calls=0)
@@ -353,6 +362,7 @@ def sharded_read_leg(pgs, torch, dist, eng, rank, world, args, barrier, check_cp
 # BASELINE.json configs[3]: manual compaction sweep, 30 % expired, run sizes 8..256 MB, bottommost forced
 # ---------------------------------------------------------------------------------------------------------------------
 def sweep_leg(pgs, eng, args, peak):
+    warm = 2
     from incubator_pegasus_b200 import synth
     out = []
     rec_bytes = 2 + HK + SK + 12 + VAL
@@ -370,9 +380,9 @@ def sweep_leg(pgs, eng, args, peak):
         part = eng.partition(app_id=3, pidx=mb)
         ids = part.upload_many([pgs.build_run(r) for r in runs], levels=[4, 3, 2, 1, 0])
         ms = []
-        for i in range(2 + 3):
+        for i in range(warm + args.steps):
             res = part.compact(ids, out_level=4, bottommost=1, now=NOW, enabled=True, flags=3)
-            if i >= 2:
+            if i >= warm:
                 ms.append(res.merge_kernel_ms)
         k_ms = sum(ms) / len(ms)
         algo = int(res.in_bytes + res.out_bytes)
@@ -382,7 +392,7 @@ def sweep_leg(pgs, eng, args, peak):
                     "roofline_frac": algo / (k_ms / 1e3) / 1e9 / peak})
         part.close()
     return {"workload": "manual_compact sweep: 5 runs (L0..L4) of equal size, 30 % of the values expired, TTL filter on, bottommost forced "
-                        "(BASELINE.json configs[3]); merge kernels timed with CUDA events, mean of 3 after 2 warm-ups",
+                        "(BASELINE.json configs[3]); merge kernels timed with CUDA events, mean of --steps launches after 2 warm-ups",
             "sizes": out}
 
 
@@ -417,6 +427,73 @@ def ycsb_a_leg(pgs, eng, args):
             "note": "single-key calls are launch-latency bound; the batched read legs above are the throughput path"}
 
 
+# ---------------------------------------------------------------------------------------------------------------------
+# --dump-outputs: what the timed path computed, as float arrays that two builds can compare element by element
+# ---------------------------------------------------------------------------------------------------------------------
+# Every array has a size fixed by these constants (a seeded sample of a larger output), so a dump stays far below 64 MB
+# whatever --records-per-run, --n-get or --n-scan are.
+DUMP_SAMPLE_RECORDS = 4096   # merged records dumped in full
+DUMP_MAX_REQUESTS = 65536    # get / scan requests whose answers are dumped
+
+
+def seeded_sample(n: int, k: int, seed: int) -> np.ndarray:
+    return np.arange(n) if n <= k else np.sort(np.random.default_rng(seed).choice(n, k, replace=False))
+
+
+def hash48(*parts: bytes) -> float:
+    """48-bit BLAKE2b of the parts, exact in a float64"""
+    h = hashlib.blake2b(digest_size=6)
+    for b in parts:
+        h.update(len(b).to_bytes(4, "little"))
+        h.update(b)
+    return float(int.from_bytes(h.digest(), "little"))
+
+
+def compaction_outputs(stats, rec) -> dict:
+    """The merged run as the records a caller decodes from it: record-level statistics, a SHA-256 of the whole record stream
+    (keys, values, sequence numbers, types) and the records at a seeded sample of record indices.  Nothing here depends on
+    where the run is cut into blocks, which follows the launch geometry of the device."""
+    h = hashlib.sha256()
+    for a in (rec.key_off, rec.keys, rec.val_off, rec.vals, rec.seq, rec.type):
+        h.update(np.ascontiguousarray(a).view(np.uint8).data)
+    pick = seeded_sample(rec.n, DUMP_SAMPLE_RECORDS, 12345)
+    keys = [rec.key(int(i)) for i in pick]
+    vals = [rec.value(int(i)) for i in pick]
+    return {"compaction_stats": np.array([float(getattr(stats, f)) for f in STAT_FIELDS], np.float64),
+            "compaction_sha256": np.frombuffer(h.digest(), np.uint8).astype(np.float32),
+            "compaction_sample_index": pick.astype(np.float64),
+            "compaction_sample_keys": np.frombuffer(b"".join(keys), np.uint8).astype(np.float32),
+            "compaction_sample_key_len": np.array([len(k) for k in keys], np.float64),
+            "compaction_sample_values": np.frombuffer(b"".join(vals), np.uint8).astype(np.float32),
+            "compaction_sample_value_len": np.array([len(v) for v in vals], np.float64),
+            "compaction_sample_seq": rec.seq[pick].astype(np.float64),
+            "compaction_sample_type": rec.type[pick].astype(np.float32)}
+
+
+def read_outputs(gres, garena, n_get: int, sb, n_scan: int) -> dict:
+    """Per request of a seeded sample: what a get / prefix scan returned, with a hash of the returned bytes (value offsets
+    depend on arena placement and are left out)."""
+    gi = seeded_sample(n_get, DUMP_MAX_REQUESTS, 4242)
+    get = np.zeros((gi.size, 5), np.float64)
+    for j, i in enumerate(gi):
+        r = gres[int(i)]
+        value = garena[r.value_off:r.value_off + r.value_len].tobytes() if r.status == 0 else b""
+        get[j] = (r.status, r.expired, r.expire_ts, r.value_len, hash48(value))
+    si = seeded_sample(n_scan, DUMP_MAX_REQUESTS, 4343)
+    scan = np.zeros((si.size, 6), np.float64)
+    for j, i in enumerate(si):
+        r = sb.results[int(i)]
+        scan[j] = (r.status, r.n_kvs, r.count, r.iter_count, r.size, hash48(*(b for kv in sb.records(int(i)) for b in kv)))
+    return {"get_index": gi.astype(np.float64), "get_results": get, "scan_index": si.astype(np.float64), "scan_results": scan}
+
+
+def write_outputs(dirpath: str, arrays: dict):
+    os.makedirs(dirpath, exist_ok=True)
+    for name, a in arrays.items():
+        assert a.dtype in (np.float32, np.float64), name
+        np.save(os.path.join(dirpath, name + ".npy"), a)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -438,7 +515,10 @@ def main():
     ap.add_argument("--sweep-mb", type=int, nargs="*", default=[8, 16, 32, 64, 128, 256])
     ap.add_argument("--ycsb-keys", type=int, default=20000)
     ap.add_argument("--ycsb-ops", type=int, default=20000)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None)
     args = ap.parse_args()
+    if args.steps < 1 or args.warmup < 0:
+        ap.error("--steps must be >= 1 and --warmup >= 0")
 
     rank = int(os.environ.get("RANK", "0"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
@@ -490,9 +570,10 @@ def main():
     stream = torch.cuda.ExternalStream(eng.stream, device=torch.device("cuda", local_rank))
     KEEP = 1 | 2  # PGS_COMPACT_KEEP_INPUTS | PGS_COMPACT_DISCARD_OUTPUT: repeat the same job
 
-    def step():
-        return part.compact(ids, out_level=1, bottommost=1, now=NOW, enabled=True, flags=KEEP)
+    def step(flags=KEEP):
+        return part.compact(ids, out_level=1, bottommost=1, now=NOW, enabled=True, flags=flags)
 
+    dump = bool(args.dump_outputs) and rank == 0  # ranks > 0 merge differently seeded inputs
     for _ in range(args.warmup):
         res = step()
     sampler = ClockSampler(local_rank)
@@ -504,8 +585,9 @@ def main():
     w0 = time.perf_counter()
     with torch.cuda.stream(stream):
         ev0.record(stream)
-        for _ in range(args.steps):
-            res = step()
+        for i in range(args.steps):
+            # with --dump-outputs the last step installs its merged run (inputs kept) so that it can be read back
+            res = step(1 if dump and i == args.steps - 1 else KEEP)
             merge_ms.append(res.merge_kernel_ms)
             plan_ms.append(res.device_ms - res.merge_kernel_ms)
             walk_ms.append(res.walk_ms)
@@ -522,6 +604,9 @@ def main():
     max_ms = float(t.item())
     ms_per_step = max_ms / args.steps
     value = world * in_bytes / (ms_per_step / 1e3) / 1e9
+    if dump:
+        write_outputs(args.dump_outputs, compaction_outputs(res, pgs.decode_blocks(part.download(res.new_run_id))))
+        part.drop(res.new_run_id)  # the read legs below see the four input runs only
 
     # ---- end to end through the C ABI from host buffers ------------------------------------------
     e2e = None
@@ -545,7 +630,7 @@ def main():
         barrier()
         split.update(upload=0.0, compact=0.0, drop=0.0)
         e0 = time.perf_counter()
-        n_e2e = max(1, min(args.steps, 3))
+        n_e2e = args.steps
         for _ in range(n_e2e):
             e2e_step()
         barrier()
@@ -575,7 +660,6 @@ def main():
 
     # ---- read path on the same partition (4 overlapping runs resident): YCSB-C shaped, zipfian hash keys ----------
     reads = None
-    traffic = load_traffic()
     peak, peak_src = load_peaks()
     if not args.skip_reads:
         pins = []
@@ -594,7 +678,7 @@ def main():
         garena_cap = args.n_get * (VAL + 8)
         garena_buf = pinned_alloc(garena_cap, np.uint8)
         gres_buf = (pgs.GetResult * args.n_get)()
-        reps = max(3, args.steps)
+        reps = args.steps
         # gets
         part.get_batch(gkeys, goff, NOW, arena_cap=garena_cap, arena=garena_buf, results=gres_buf)
         g_ms, g_wall, found, probes = [], [], 0, 0
@@ -622,6 +706,8 @@ def main():
         returned = int(kbase[-1])
         iterated = int(sum(sres[i].iter_count for i in range(args.n_scan)))
         scan_bytes = int(abase[-1])
+        if dump:
+            write_outputs(args.dump_outputs, read_outputs(gres, garena, args.n_get, sb, args.n_scan))
         mean = lambda xs: sum(xs) / len(xs)
         gm, sm, gw, sw = mean(g_ms), mean(s_ms), mean(g_wall), mean(s_wall)
         nb_log = 18
@@ -633,18 +719,10 @@ def main():
             dist.all_reduce(vals, op=dist.ReduceOp.SUM)  # partitions are independent: whole-job keys/s = sum over ranks
 
         def roof(kernel, algo, ms):
-            tr = traffic.get(kernel)
-            r = {"bound": "hbm", "kernel": kernel, "achieved": algo / (ms / 1e3) / 1e9, "peak": peak, "unit": "GB/s",
+            return {"bound": "hbm", "kernel": kernel, "achieved": algo / (ms / 1e3) / 1e9, "peak": peak, "unit": "GB/s",
                  "frac": algo / (ms / 1e3) / 1e9 / peak, "algorithmic_bytes_per_launch": algo,
                  "formula": "SURVEY.md §8(d): blocks probed x (4 KB block + index path) + keys + values returned" if kernel == "k_get"
                             else "SURVEY.md §8(d): records iterated x record bytes + records returned x record bytes"}
-            if tr:  # DRAM bytes of the same launch shape under ncu (time from this run's CUDA events)
-                r["traffic"] = tr["dram_bytes_per_launch"]
-                r["traffic_source"] = tr.get("source")
-                r["dram_frac"] = tr["dram_bytes_per_launch"] / (ms / 1e3) / 1e9 / peak
-            else:
-                r["traffic"] = None
-            return r
 
         reads = {
             "statistic": "mean over the repetitions, for the device (kernel CUDA events) and the e2e (host wall clock) numbers alike",
@@ -689,19 +767,16 @@ def main():
     k_ms = sum(merge_ms) / len(merge_ms)
     algo_bytes = int(res.in_bytes + res.out_bytes)
     achieved = algo_bytes / (k_ms / 1e3) / 1e9
-    tr_w, tr_e = traffic.get("k_walk"), traffic.get("k_emit")
     roofline = {"bound": "hbm", "kernel": "k_walk+k_emit", "achieved": achieved, "peak": peak, "unit": "GB/s",
                 "frac": achieved / peak, "peak_source": peak_src, "algorithmic_bytes_per_launch": algo_bytes, "kernel_ms": k_ms,
                 "kernels_ms": {"k_walk": sum(walk_ms) / len(walk_ms), "k_emit": sum(emit_ms) / len(emit_ms),
-                               "plan (k_plan+k_seg_bounds+k_seg_layout)": sum(plan_ms) / len(plan_ms)},
-                "traffic": (tr_w["dram_bytes_per_launch"] + tr_e["dram_bytes_per_launch"]) if tr_w and tr_e else None,
-                "traffic_source": tr_w.get("source") if tr_w and tr_e else None}
+                               "plan (k_plan+k_seg_bounds+k_seg_layout)": sum(plan_ms) / len(plan_ms)}}
 
     # ---- CPU baseline on the same full workload + parity of the statistics (rank 0, N=1 only) -----------
     cpu, parity = None, None
     if rank == 0 and world == 1 and not args.skip_cpu:
         threads = os.cpu_count() or 1
-        gbs, secs, st = cpu_compaction(cpu_block_runs(runs), threads)
+        gbs, secs, st, _ = cpu_compaction(cpu_block_runs(runs), threads)
         cpu = {"value": gbs, "unit": "GB/s", "cores": threads, "kind": "port",
                "what": "oracle-CPU block-level compaction (a restatement of the reference's RocksDB path, not RocksDB)",
                "sample": f"{RUNS} runs x {args.records_per_run} records ({st.in_bytes / 1e9:.2f} GB merged): the full workload, {secs:.2f} s"}
@@ -720,10 +795,12 @@ def main():
         ycsb = ycsb_a_leg(pgs, eng, args)
 
     if rank == 0:
+        props = torch.cuda.get_device_properties(local_rank)
         cfg = workload_config(args.records_per_run)
         cfg.update({"records_per_step_per_gpu": n_records, "merged_bytes_per_step_per_gpu": in_bytes,
                     "survivors": int(res.out_records), "segments": int(res.n_tiles),
-                    "l2": "inputs (2.9 GB of blocks) larger than the 126 MB L2", "input_gen_s": round(gen_s, 1)})
+                    "l2": f"inputs ({h2d_bytes / 1e9:.1f} GB of blocks) vs the {props.L2_cache_size >> 20} MB L2",
+                    "input_gen_s": round(gen_s, 1)})
         line = {
             "metric": "compaction_merged_GBps", "value": value, "unit": "GB/s", "n_gpus": world, "steps": args.steps,
             "warmup": args.warmup, "ms_per_step": ms_per_step, "higher_is_better": True, "scaling": "weak",
@@ -731,6 +808,7 @@ def main():
             "roofline": roofline, "cpu_baseline": cpu, "parity_checked": parity, "e2e": e2e, "reads": reads,
             "sharded_reads": sharded, "sweep": sweep, "ycsb_a": ycsb, "nccl": nccl, "gpu_launches": int(launches),
             "clocks": sampler.summary(), "wall_ms_per_step": wall_ms / args.steps,
+            "device": {"name": props.name, "sm_count": props.multi_processor_count, "power_limit_w": power_limit(local_rank)},
         }
         print(json.dumps(line), flush=True)
     part.close()

@@ -1,5 +1,5 @@
 /*
- * pegasus_b200.h — C ABI of the B200-native LSM read/compaction engine for the Pegasus replica
+ * pegasus_b200.h — C ABI of the GPU-native (H100) LSM read/compaction engine for the Pegasus replica
  * server.  This is the drop-in boundary: everything a reference-side binding (the C++ class
  * that takes RocksDB's place behind `replication_app_base`, or a cgo/JNI stub) needs is declared
  * here with plain pointers and sizes.  No torch / CUDA / C++ types cross it, no exception does.

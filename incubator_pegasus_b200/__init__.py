@@ -26,7 +26,7 @@ u64p = C.POINTER(C.c_uint64)
 
 
 def build(force: bool = False) -> str:
-    """Compile the library in-tree with nvcc for sm_100a (no GPU needed)."""
+    """Compile the library in-tree with nvcc for sm_90a (no GPU needed)."""
     env = dict(os.environ)
     if force:
         env["FORCE"] = "1"
@@ -152,7 +152,7 @@ def lib() -> C.CDLL:
     if _lib is not None:
         return _lib
     if not os.path.exists(LIB_PATH):
-        raise RuntimeError(f"{LIB_PATH} is missing: run incubator_pegasus_b200/build.sh (nvcc, sm_100a)")
+        raise RuntimeError(f"{LIB_PATH} is missing: run incubator_pegasus_b200/build.sh (nvcc, sm_90a)")
     L = C.CDLL(LIB_PATH)
     vp = C.c_void_p
     L.pgs_last_error.restype = C.c_char_p

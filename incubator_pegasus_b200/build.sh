@@ -1,13 +1,14 @@
 #!/bin/bash
-# Builds libpegasus_b200.so (CUDA kernels for sm_100a + host code + C ABI) in-tree.
+# Builds libpegasus_b200.so (CUDA kernels for sm_90a + host code + C ABI) in-tree.
 set -e
 HERE="$(cd "$(dirname "$0")" && pwd)"
 NVCC=${NVCC:-/usr/local/cuda/bin/nvcc}
 OUT="$HERE/libpegasus_b200.so"
 SRCS=("$HERE"/csrc/*.cu "$HERE"/host/*.cpp)
-newest=$(ls -t "${SRCS[@]}" "$HERE"/csrc/*.h "$HERE"/csrc/*.cuh "$HERE"/host/*.h "$HERE"/../include/*.h 2>/dev/null | head -1)
+newest=$(ls -t "${SRCS[@]}" "$HERE"/csrc/*.h "$HERE"/csrc/*.cuh "$HERE"/host/*.h "$HERE"/../include/*.h "$0" 2>/dev/null | head -1)
 if [ -f "$OUT" ] && [ "$OUT" -nt "$newest" ] && [ -z "$FORCE" ]; then echo "up to date: $OUT"; exit 0; fi
-FLAGS=(-gencode arch=compute_100a,code=sm_100a -lineinfo -O3 -std=c++17 -Xcompiler -fPIC,-fvisibility=hidden,-Wall,-Wno-unused-function -Xptxas -v --expt-relaxed-constexpr -cudart static)
+ARCH=(-gencode arch=compute_90a,code=sm_90a)
+FLAGS=("${ARCH[@]}" -lineinfo -O3 -std=c++17 -Xcompiler -fPIC,-fvisibility=hidden,-Wall,-Wno-unused-function -Xptxas -v --expt-relaxed-constexpr -cudart static)
 OBJS=()
 mkdir -p "$HERE/build"
 for s in "${SRCS[@]}"; do
@@ -19,5 +20,5 @@ for s in "${SRCS[@]}"; do
   fi
   OBJS+=("$o")
 done
-"$NVCC" -gencode arch=compute_100a,code=sm_100a -shared -cudart static -o "$OUT" "${OBJS[@]}" -lpthread
+"$NVCC" "${ARCH[@]}" -shared -cudart static -o "$OUT" "${OBJS[@]}" -lpthread
 echo "built $OUT"

@@ -9,7 +9,7 @@
 //   compaction_operation / compaction_filter_rule ....... src/server/compaction_operation.cpp:33-113,
 //                                                         src/server/compaction_filter_rule.cpp:31-90
 //
-// Shape of the computation (B200-first; byte/integer work bound by HBM, no tensor cores):
+// Shape of the computation (byte/integer work bound by HBM, no tensor cores):
 //   k_plan        one thread per input block ranks the block's last user key against every run's block index
 //                 => cumulative weight of everything <= that key.  Keys where the weight crosses a multiple of the
 //                 segment budget become segment boundaries: segment q = user keys in (U_q, U_q+1], a contiguous
@@ -175,9 +175,8 @@ inline bool compact_geometry(MergeParams &P, const CompactTotals &T, uint32_t ma
         // A group walks its segments one after the other and a segment is a sequential job: the walk takes (waves of
         // segments) x (time of a segment), and a last, partly filled wave costs as much as a full one.  Size the segments
         // so that they fill a whole number of waves -- one wave whenever a segment stays under kSegWeightMax: every segment
-        // pays for opening its cursors and skipping into its range, so fewer and longer ones are cheaper (measured at
-        // config #2: 3.46 -> 3.22 ms for one wave of 283 KB segments instead of two of 141 KB).  Small inputs get one
-        // wave of short segments.
+        // pays for opening its cursors and skipping into its range, so fewer and longer ones are cheaper.  Small inputs
+        // get one wave of short segments.
         const uint64_t waves = (W_total + kSegWeightMax * walk_groups - 1) / (kSegWeightMax * walk_groups);
         const uint64_t slots = (waves ? waves : 1) * walk_groups;
         uint64_t w = (W_total + slots - 1) / slots;

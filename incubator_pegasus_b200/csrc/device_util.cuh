@@ -1,4 +1,4 @@
-// device_util.cuh — device-side primitives shared by the sm_100a kernels: TMA bulk copies and
+// device_util.cuh — device-side primitives shared by the sm_90a kernels: TMA bulk copies and
 // mbarriers (inline PTX), varint decode, byte-string compares, warp/block scans, misaligned
 // warp copies.
 #pragma once

@@ -39,7 +39,7 @@ static bool engine_alive(Engine *e)
 
 constexpr uint64_t kSpareMin = 64ull << 20; // only buffers this large are worth keeping
 constexpr size_t kSpareMax = 8;
-constexpr uint64_t kSpareBytesMax = 24ull << 30;
+constexpr uint64_t kSpareMemDivisor = 8; // spare buffers hold at most 1/8 of the device memory (10 GB on an 80 GB H100)
 
 uint8_t *Engine::take_data(uint64_t need, uint64_t *cap)
 {
@@ -83,7 +83,7 @@ void Engine::give_data(uint8_t *p, uint64_t cap)
     spares.push_back(Spare{p, cap});
     uint64_t total = 0;
     for (auto &s : spares) total += s.cap;
-    while (spares.size() > kSpareMax || total > kSpareBytesMax) { // give the smallest ones back to the pool
+    while (spares.size() > kSpareMax || total > spare_bytes_max) { // give the smallest ones back to the pool
         size_t m = 0;
         for (size_t i = 1; i < spares.size(); i++) if (spares[i].cap < spares[m].cap) m = i;
         total -= spares[m].cap;
@@ -516,6 +516,11 @@ int32_t pgs_engine_open(const pgs_engine_config *cfg, pgs_engine **out)
     if (err == cudaSuccess) err = cudaStreamCreateWithFlags(&e.stream, cudaStreamNonBlocking);
     if (err == cudaSuccess) err = cudaDeviceGetAttribute(&e.sm_count, cudaDevAttrMultiProcessorCount, dev);
     if (err == cudaSuccess) err = cudaDeviceGetAttribute(&e.max_smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
+    if (err == cudaSuccess) {
+        size_t free_b = 0, total_b = 0;
+        err = cudaMemGetInfo(&free_b, &total_b);
+        e.spare_bytes_max = total_b / kSpareMemDivisor;
+    }
     for (auto &s : e.rd_streams) if (err == cudaSuccess) err = cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking);
     if (err == cudaSuccess) err = cudaStreamCreateWithFlags(&e.up_copy, cudaStreamNonBlocking);
     if (err == cudaSuccess && (lookup_init_kernels(e.max_smem_optin) != PGS_OK || compact_init_kernels(e.max_smem_optin) != PGS_OK ||

@@ -59,11 +59,12 @@ struct Engine {
     size_t h_pinned_cap = 0;
     void *pinned(size_t bytes);
     // Spare list of large block buffers.  A compaction frees a few ~GB buffers and asks for one of a different size; what
-    // the stream-ordered pool does with that depends on its placement choices, and growing the pool costs ~100 ms.
+    // the stream-ordered pool does with that depends on its placement choices, and growing the pool is slow.
     // Buffers of dropped runs are therefore kept here (all uses are ordered on `stream`) and handed to the next taker.
     struct Spare { uint8_t *p; uint64_t cap; };
     std::mutex spare_mu;
     std::vector<Spare> spares;
+    uint64_t spare_bytes_max = 0; // set at open from the device's memory size
     uint8_t *take_data(uint64_t need, uint64_t *cap); // nullptr when nothing suitable is kept
     void give_data(uint8_t *p, uint64_t cap);
     // pinned host staging for the small arrays of an upload (block handles in, per-block counts out): with pageable memory a

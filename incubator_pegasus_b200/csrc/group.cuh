@@ -6,10 +6,10 @@
 // one ballot.  The 32/G groups of a warp run in LOCK STEP on different data: control flow around every collective is
 // warp-uniform (loops run while any group still needs them, per-group work is switched on and off with an `en`
 // predicate), so all shuffles / ballots use the constant full mask -- a collective with a run-time lane mask costs a
-// MATCH.ANY + REDUX convergence check per call and lets the groups drift apart; measured 4x slower.
+// MATCH.ANY + REDUX convergence check per call and lets the groups drift apart.
 // G = 1 is the degenerate case: one thread per iterator, no collectives at all, so its control flow may diverge freely (the
 // hardware serialises the paths); the same source serves both shapes.
-// This is the B200 shape of RocksDB's DataBlockIter / MergingIterator (v8.5.3, not in the reference tree; SURVEY.md
+// This is the GPU shape of RocksDB's DataBlockIter / MergingIterator (v8.5.3, not in the reference tree; SURVEY.md
 // Appendix A): the per-record decode chain stays sequential, the parallelism comes from thousands of independent groups.
 #pragma once
 #include "../../include/pegasus_b200.h"

@@ -199,7 +199,7 @@ def test_bench_size_digest(pgs, oracle, engine):
             for a in (r.key_off, r.keys, r.val_off, r.vals, r.seq, r.type):
                 h.update(np.ascontiguousarray(a).view(np.uint8).data)
             return h.hexdigest()
-        assert got.n == want.n == res.out_records == 8_240_347  # the survivor count of this seed (BENCH_r01.json)
+        assert got.n == want.n == res.out_records == 8_240_347  # the survivor count of this seed (bench.py's compaction step)
         assert digest(got) == digest(want)
     finally:
         part.close()

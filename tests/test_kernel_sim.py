@@ -1,4 +1,4 @@
-"""CPU check of the compaction KERNELS' logic: the same sources nvcc compiles for sm_100a
+"""CPU check of the compaction KERNELS' logic: the same sources nvcc compiles for sm_90a
 (incubator_pegasus_b200/csrc/compact_kernels.cuh, group.cuh) are compiled by g++ against tools/simt/simt.h, a host-side SIMT
 interpreter (every CUDA thread a fiber, shuffles / ballots / barriers as rendezvous), and their output is compared with the
 oracle.  This says nothing about timing or the memory model -- the `-m gpu` tests do -- but it runs the merge, filter,

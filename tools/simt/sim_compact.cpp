@@ -1,5 +1,5 @@
 // sim_compact.cpp — runs the compaction kernels (incubator_pegasus_b200/csrc/compact_kernels.cuh, the same source nvcc compiles
-// for sm_100a) inside the host SIMT interpreter of simt.h.  Test / development tool: lets the CPU test-suite execute the kernels'
+// for sm_90a) inside the host SIMT interpreter of simt.h.  Test / development tool: lets the CPU test-suite execute the kernels'
 // logic against the oracle without a GPU.  NOT part of the product library and never a fallback for it.
 #include "simt.h"
 
