@@ -36,6 +36,7 @@ int32_t scan_many(Partition &part, const pgs_scan_request *reqs, uint32_t n, uin
                   uint32_t kv_stride, uint8_t *arena, uint64_t arena_cap, pgs_kv *kvs, uint64_t kv_cap, uint8_t *resume,
                   uint32_t resume_stride, pgs_scan_result *results, uint64_t *arena_base, uint32_t *kv_base,
                   const std::vector<std::shared_ptr<Run>> *pinned);
+bool scan_stages_every_run(Partition &part);
 
 constexpr size_t kReadMaxRuns = 12; // a read-triggered flush compacts L0 once the run list grows past this
 
@@ -169,13 +170,15 @@ struct Server {
         for (auto &r : runs()) l0 += r->level == 0;
         return l0 >= trigger ? compact_l0(now) : PGS_OK;
     }
-    // range reads: the memtable becomes an L0 run (and L0 is folded once the run list grows past kReadMaxRuns)
-    bool range_read_needs_prepare() { return !mem.empty() || runs().size() > kReadMaxRuns; }
-    int32_t prepare_read(uint32_t now)
+    // range reads: the memtable becomes an L0 run, and L0 is folded once the run list grows past kReadMaxRuns, or when the
+    // reverse-scan kernel could not stage one block of every run (many L0 runs of small records, such as tombstones)
+    bool needs_fold(bool reverse) { return runs().size() > kReadMaxRuns || (reverse && !scan_stages_every_run(part->p)); }
+    bool range_read_needs_prepare(bool reverse) { return !mem.empty() || needs_fold(reverse); }
+    int32_t prepare_read(uint32_t now, bool reverse)
     {
         int32_t st = flush_mem();
         if (st != PGS_OK) return st;
-        if (runs().size() > kReadMaxRuns) st = compact_l0(now);
+        if (needs_fold(reverse)) st = compact_l0(now);
         return st;
     }
     // point reads: newest version in the memtable, if any.  0 = not there, 1 = value, 2 = tombstone
@@ -286,14 +289,14 @@ static int32_t read_fail(Resp &r, int32_t st)
 using RLock = std::shared_lock<std::shared_mutex>;
 // A range read runs on HBM runs only: when the memtable holds anything (or L0 has piled up) the shared lock is traded for
 // the exclusive one for the duration of the flush.  Writes that land between the two locks are concurrent with this read.
-static int32_t ensure_range_ready(Server &s, RLock &lk, uint32_t now)
+static int32_t ensure_range_ready(Server &s, RLock &lk, uint32_t now, bool reverse = false)
 {
-    if (!s.range_read_needs_prepare()) return PGS_OK;
+    if (!s.range_read_needs_prepare(reverse)) return PGS_OK;
     lk.unlock();
     int32_t st;
     {
         std::unique_lock<std::shared_mutex> w(s.mu);
-        st = s.prepare_read(now);
+        st = s.prepare_read(now, reverse);
     }
     lk.lock();
     return st;
@@ -370,7 +373,7 @@ static int32_t do_multi_get(Server &s, RLock &lk, const pgs_multi_get_request &q
 {
     r.reset(s.app_id, s.pidx);
     if (!filter_type_supported(q.sort_key_filter_type)) return r.seal(PGS_INVALID_ARGUMENT);
-    int32_t st = q.n_sort_keys == 0 ? ensure_range_ready(s, lk, now) : PGS_OK;
+    int32_t st = q.n_sort_keys == 0 ? ensure_range_ready(s, lk, now, q.reverse != 0) : PGS_OK;
     if (st != PGS_OK) return read_fail(r, st);
     uint32_t max_kv_count = s.cfg_mget_count(), max_iteration_count = s.cfg_mget_count();
     if (q.max_kv_count > 0 && (uint32_t)q.max_kv_count < max_kv_count) max_kv_count = q.max_kv_count;

@@ -104,6 +104,27 @@ def test_reads_over_many_runs_and_big_values(engine):
         o.close()
 
 
+def test_reverse_reads_over_many_runs_of_tombstones(engine):
+    """11 L0 runs of ~2,000 short tombstones each (multi_remove + flush): a 4 KB block holds ~320 records, so k_scan could
+    not stage one block of every run, and 11 runs stay under the read-triggered fold at 12.  Reverse reads must still
+    answer (the server folds L0 for them first); forward reads and counts as well."""
+    g, o = Backend("gpu", engine, opts={"l0_compaction_trigger": 100}), Backend("oracle", opts={"l0_compaction_trigger": 100})
+    try:
+        for round_ in range(11):
+            for be in (g, o):
+                be.decree = round_ * 1000
+                be.multi_put(b"t", {b"%d" % (round_ * 37 + j): b"v%d" % round_ for j in range(5)})
+                assert be.multi_remove(b"t", [b"%d" % (i * 11 + round_) for i in range(2000)])[0] == 0
+                be.flush(NOW)
+        for kw in [dict(reverse=True), dict(), dict(reverse=True, max_kv_count=3), dict(start=b"200", stop=b"300", reverse=True)]:
+            rg, ro = g.multi_get(b"t", now=NOW, **kw), o.multi_get(b"t", now=NOW, **kw)
+            assert rg["error"] == ro["error"] and same_response(rg, ro)[0], (kw, rg["error"], ro["error"])
+        assert same_response(g.sortkey_count(b"t", now=NOW), o.sortkey_count(b"t", now=NOW))[0]
+    finally:
+        g.close()
+        o.close()
+
+
 def test_corrupt_and_unsupported_uploads(pgs, engine):
     run = pgs.build_run(synth.compaction_runs(k=1, n_per_run=500, seed=5)[0])
     part = engine.partition()

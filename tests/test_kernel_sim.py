@@ -20,7 +20,8 @@ SIM_DIR = os.path.join(ROOT, "tools", "simt")
 def sim():
     so = os.path.join(SIM_DIR, "libpgs_sim.so")
     srcs = [os.path.join(SIM_DIR, f) for f in ("sim_compact.cpp", "simt.h")]
-    srcs += [os.path.join(ROOT, "incubator_pegasus_b200", "csrc", f) for f in ("compact_kernels.cuh", "group.cuh", "device_util.cuh", "format.h")]
+    srcs += [os.path.join(ROOT, "incubator_pegasus_b200", "csrc", f)
+             for f in ("compact_kernels.cuh", "read_kernels.cuh", "scan_kernel.cuh", "group.cuh", "device_util.cuh", "format.h")]
     if not os.path.exists(so) or any(os.path.getmtime(s) > os.path.getmtime(so) for s in srcs):
         subprocess.check_call(["g++", "-std=c++17", "-O1", "-g", "-fPIC", "-shared", "-Wno-unknown-pragmas",
                                os.path.join(SIM_DIR, "sim_compact.cpp"), "-o", so])
@@ -68,6 +69,27 @@ def sim_compact(pgs, sim, runs, *, bottommost, now=synth.NOW, default_ttl=0, val
     return out, dict(stats=list(stats), blk_rec=blk_rec, ikey_off=ikey_off, ikeys=ikeys, rec_off=rec_off, end=end, nseg=nseg.value)
 
 
+def entry_offsets(data, off, size):
+    """offsets of the entries of the block at data[off:off + size], from its headers (shared, non_shared, value length)"""
+    nr = int.from_bytes(data[off + size - 4:off + size].tobytes(), "little")
+    limit, p, out = size - 4 - 4 * nr, 0, []
+    while p < limit:
+        out.append(p)
+        h, lens = 0, []
+        for _ in range(3):
+            v = sh = 0
+            while True:
+                c = int(data[off + p + h])
+                h += 1
+                v |= (c & 127) << sh
+                sh += 7
+                if c < 128:
+                    break
+            lens.append(v)
+        p += h + lens[1] + lens[2]
+    return out
+
+
 def crc_table():
     poly = 0x9a6c9329ac4bc9b5
     tab = []
@@ -112,9 +134,10 @@ def check(pgs, oracle, sim, runs, *, bottommost, ops_json=None, **kw):
     for b in range(n):
         last = int(x["blk_rec"][b + 1]) - 1
         assert x["ikeys"][int(x["ikey_off"][b]):int(x["ikey_off"][b + 1])].tobytes() == want.key(last)
-    # entry offsets: decoding each block entry by entry must land on rec_off
-    one = pgs.decode_blocks(pgs.BlockRun(got_run.data, got_run.blk_off[:1], got_run.blk_size[:1]))
-    assert int(x["rec_off"][0]) == 0 and one.n == int(x["blk_rec"][1])
+    # entry offsets: walking each block entry by entry must land on its rec_off entries
+    for b in range(n):
+        walk = entry_offsets(got_run.data, int(got_run.blk_off[b]), int(got_run.blk_size[b]))
+        assert walk == [int(v) for v in x["rec_off"][int(x["blk_rec"][b]):int(x["blk_rec"][b + 1])]], b
     assert x["stats"][10] == int(np.sum(want.type == 0))
     assert x["stats"][11] == want.keys.shape[0] and x["stats"][12] == want.vals.shape[0]
     return x

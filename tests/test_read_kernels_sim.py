@@ -9,56 +9,10 @@ import numpy as np
 import pytest
 
 from incubator_pegasus_b200 import synth
+from scan_model import answer, diff, make_db, mirror, model_scan, next_key, raw_key, scan_list, scan_requests, visible
 from test_kernel_sim import sim, sim_compact  # noqa: F401  (fixture + helper)
 
 NOW = synth.NOW
-
-
-def be(n, w):
-    return int(n).to_bytes(w, "big")
-
-
-def raw_key(hk, sk):
-    return be(len(hk), 2) + hk + sk
-
-
-def value(ets, data):
-    return be(ets, 4) + be((1 << 8) | 2, 8) + data
-
-
-def make_db(pgs, rng, n_runs, hashkeys, sort_per_hk, big=False):
-    """n_runs runs, NEWEST FIRST (as Partition.runs): each write gets a global seq; a run holds a random subset of keys."""
-    seq = 0
-    runs_items = []
-    for r in range(n_runs):  # oldest run first while generating
-        items = {}
-        for hk in hashkeys:
-            for s in range(sort_per_hk):
-                if rng.random() < 0.45:
-                    continue
-                sk = b"s%04d" % s
-                for _ in range(int(rng.integers(1, 3))):
-                    seq += 1
-                    u = rng.random()
-                    if u < 0.12:
-                        items[(raw_key(hk, sk), -seq)] = (raw_key(hk, sk), seq, 0, b"")
-                    else:
-                        ets = 0 if u < 0.6 else (NOW + int(rng.integers(1, 1000)) if u < 0.85 else NOW - int(rng.integers(0, 1000)))
-                        dl = int(rng.integers(0, 30)) if not big or rng.random() < 0.9 else int(rng.integers(600, 1500))
-                        items[(raw_key(hk, sk), -seq)] = (raw_key(hk, sk), seq, 1, value(ets, bytes(rng.integers(0, 256, dl, dtype=np.uint8))))
-        runs_items.append([items[k] for k in sorted(items)])
-    runs_items.reverse()  # newest first
-    return [pgs.Records.from_list(it) for it in runs_items if it], runs_items
-
-
-def visible(runs_items):
-    """newest version of every user key; tombstones hide the key.  -> sorted [(key, value)]"""
-    best = {}
-    for items in runs_items:
-        for k, s, t, v in items:
-            if k not in best or s > best[k][0]:
-                best[k] = (s, t, v)
-    return [(k, v) for k, (s, t, v) in sorted(best.items()) if t == 1], best
 
 
 def run_args(pgs, runs, block_size=4096, ri=16):
@@ -150,146 +104,65 @@ def test_sim_get_multi_partition(pgs, sim):
     assert hits > 30
 
 
-def model_scan(vis, q, now):
-    """the reference loop over the visible records; returns dict like pgs_scan_result + kvs"""
-    start, stop = q["start"], q["stop"]
-    pos = 0
-    while pos < len(vis) and vis[pos][0] < start:
-        pos += 1
-    prefix = None
-    if q.get("prefix") and len(start) >= 2:
-        hl = int.from_bytes(start[:2], "big")
-        if 2 + hl <= len(start):
-            prefix = start[:2 + hl]
-
-    def valid(p):
-        if p >= len(vis):
-            return False
-        k = vis[p][0]
-        if prefix is not None and k[:len(prefix)] != prefix:
-            return False
-        if q.get("has_upper") and k >= stop:
-            return False
-        return True
-    count = it = exp = fil = 0
-    size = 0
-    kvs = []
-    complete = False
-    first_excl = not q["start_inclusive"]
-    while count < q["max_count"] and it < q["max_iter_count"] and not (q["max_iter_size"] > 0 and size >= q["max_iter_size"]) and valid(pos):
-        k, v = vis[pos]
-        if k > stop or (k == stop and not q["stop_inclusive"]):
-            complete = True
-            break
-        if first_excl:
-            first_excl = False
-            if k == start:
-                pos += 1
-                continue
-        it += 1
-        ets = int.from_bytes(v[:4], "big")
-        hl = int.from_bytes(k[:2], "big")
-        hk, sk = k[2:2 + hl], k[2 + hl:]
-
-        def match(ft, pat, s):
-            if ft == 0 or not pat:
-                return True
-            return {1: pat in s, 2: s.startswith(pat), 3: s.endswith(pat)}[ft]
-        if 0 < ets <= now:
-            exp += 1
-        elif not match(q.get("hft", 0), q.get("hpat", b""), hk) or not match(q.get("sft", 0), q.get("spat", b""), sk):
-            fil += 1
-        else:
-            ko = sk if q["key_mode"] == 1 else k
-            vo = b"" if q.get("no_value") else v[12:]
-            count += 1
-            size += len(ko) + len(vo)
-            if not q.get("count_only"):
-                kvs.append((ko, vo, ets if q.get("return_expire_ts") else 0))
-        if k == stop:
-            complete = True
-            break
-        pos += 1
-    iv = valid(pos)
-    return dict(count=count, iter_count=it, expire_count=exp, filter_count=fil, size=size, complete=complete, iter_valid=iv,
-                resume=vis[pos][0] if iv and not complete else None, kvs=kvs)
-
-
-def do_scans(pgs, sim, args, reqs, lanes=0):
+def do_scans(pgs, sim, args, reqs, lanes=0, pool=0):
     n = len(reqs)
     keep = []
-
-    def blob(b):
-        buf = (C.c_uint8 * max(1, len(b))).from_buffer_copy(b if b else b"\0")
-        keep.append(buf)
-        return pgs.Blob(C.cast(buf, C.POINTER(C.c_uint8)), len(b))
-    arr = (pgs.ScanRequest * n)()
-    for i, q in enumerate(reqs):
-        r = arr[i]
-        r.start, r.stop = blob(q["start"]), blob(q["stop"])
-        r.start_inclusive, r.stop_inclusive = int(q["start_inclusive"]), int(q["stop_inclusive"])
-        r.no_value, r.key_mode, r.return_expire_ts = int(q.get("no_value", 0)), q["key_mode"], int(q.get("return_expire_ts", 0))
-        r.count_only, r.prefix_same_as_start = int(q.get("count_only", 0)), int(q.get("prefix", 0))
-        r.reserved[0] = int(q.get("has_upper", 0))
-        r.hash_filter_type, r.sort_filter_type = q.get("hft", 0), q.get("sft", 0)
-        r.hash_filter, r.sort_filter = blob(q.get("hpat", b"")), blob(q.get("spat", b""))
-        r.max_count, r.max_iter_count, r.max_iter_size = q["max_count"], q["max_iter_count"], q["max_iter_size"]
+    arr = scan_requests(pgs, reqs, keep)
     astride, kstride, rstride = 1 << 16, 512, 512
     arena = np.zeros(astride * n, np.uint8)
     kvs = (pgs.KV * (kstride * n))()
     resume = np.zeros(rstride * n, np.uint8)
     res = (pgs.ScanResult * n)()
     st = sim.sim_scan(*args, arr, n, NOW, C.c_uint64(astride), kstride, arena.ctypes.data_as(C.c_void_p), kvs,
-                      resume.ctypes.data_as(C.c_void_p), rstride, res, lanes)
+                      resume.ctypes.data_as(C.c_void_p), rstride, res, lanes, pool)
     assert st == 0, st
-    out = []
-    for i in range(n):
-        r = res[i]
-        a = arena[i * astride:(i + 1) * astride]
-        recs = [(a[kv.key_off:kv.key_off + kv.key_len].tobytes(), a[kv.value_off:kv.value_off + kv.value_len].tobytes(), kv.expire_ts)
-                for kv in kvs[i * kstride:i * kstride + r.n_kvs]]
-        out.append(dict(count=r.count, iter_count=r.iter_count, expire_count=r.expire_count, filter_count=r.filter_count, size=r.size,
-                        complete=bool(r.complete), iter_valid=bool(r.iter_valid),
-                        resume=resume[i * rstride:i * rstride + r.resume_len].tobytes() if r.iter_valid and not r.complete else None, kvs=recs))
-    return out
+    return [answer(res[i], arena[i * astride:(i + 1) * astride], kvs[i * kstride:i * kstride + res[i].n_kvs],
+                   resume[i * rstride:(i + 1) * rstride]) for i in range(n)]
+
+
+def check_scans(vis, reqs, got):
+    for i, (q, g_) in enumerate(zip(reqs, got)):
+        want = model_scan(vis, q, NOW)
+        assert g_ == want, (i, q, diff(g_, want))
+
+
+SCAN_HKS = [b"h%d" % i for i in range(7)] + [b"", b"h1x", bytes([0xff, 0xff])]
 
 
 @pytest.mark.parametrize("n_runs,lanes", [(4, 0), (1, 0), (6, 16), (3, 32)])
 def test_sim_scan_forward(pgs, sim, n_runs, lanes):
     rng = np.random.default_rng(100 + n_runs)
-    hks = [b"h%d" % i for i in range(7)] + [b"", b"h1x", bytes([0xff, 0xff])]
-    runs, items = make_db(pgs, rng, n_runs, hks, 30)
+    runs, items = make_db(pgs, rng, n_runs, SCAN_HKS, 30)
     vis, best = visible(items)
     args, keep = run_args(pgs, runs, block_size=512, ri=4)
-    reqs = []
-    for hk in hks + [b"nope"]:
-        lo, hi = raw_key(hk, b""), raw_key(hk, b"\xff" * 8)
-        nxt = bytearray(raw_key(hk, b""))
-        while nxt and nxt[-1] == 0xff:
-            nxt.pop()
-        nxt[-1] += 1
-        nxt = bytes(nxt)
-        base = dict(start=lo, stop=nxt, start_inclusive=True, stop_inclusive=False, key_mode=1, prefix=1,
-                    max_count=3000, max_iter_count=3000, max_iter_size=0)
-        reqs.append(base)                                                               # multi_get: whole hash key
-        reqs.append(dict(base, max_count=7))                                            # count limit
-        reqs.append(dict(base, max_iter_count=9))                                       # iteration limit
-        reqs.append(dict(base, max_iter_size=100))                                      # size limit
-        reqs.append(dict(base, start=raw_key(hk, b"s0010"), stop=raw_key(hk, b"s0020"), stop_inclusive=True))
-        reqs.append(dict(base, start=raw_key(hk, b"s0010"), start_inclusive=False, stop=raw_key(hk, b"s0010"), stop_inclusive=True))
-        reqs.append(dict(base, start=raw_key(hk, b"s0005"), start_inclusive=False, no_value=1))
-        reqs.append(dict(base, sft=3, spat=b"7"))                                       # sort-key postfix filter
-        reqs.append(dict(base, sft=1, spat=b"01", count_only=1))
-        reqs.append(dict(base, has_upper=1, count_only=1, max_count=2**32 - 1, max_iter_count=2**32 - 1))  # sortkey_count
-        reqs.append(dict(base, key_mode=0, prefix=0, stop=hi, hft=2, hpat=hk[:1], return_expire_ts=1, max_count=11))  # scanner batch
-    reqs.append(dict(start=b"", stop=b"\xff\xff\xff", start_inclusive=True, stop_inclusive=True, key_mode=0, prefix=0,
-                     max_count=100000, max_iter_count=100000, max_iter_size=0))         # full table
-    reqs.append(dict(start=b"\x00\x02h", stop=b"\x00\x02h5", start_inclusive=True, stop_inclusive=False, key_mode=0, prefix=0,
-                     max_count=40, max_iter_count=1000, max_iter_size=0))
-    got = do_scans(pgs, sim, args, reqs, lanes)
-    for i, (q, g_) in enumerate(zip(reqs, got)):
-        want = model_scan(vis, q, NOW)
-        assert g_ == want, (i, q, {k: (g_[k], want[k]) for k in want if g_[k] != want[k]})
+    reqs = scan_list(SCAN_HKS)
+    check_scans(vis, reqs, do_scans(pgs, sim, args, reqs, lanes))
+
+
+@pytest.mark.parametrize("pool", ["product", "minimal"])
+@pytest.mark.parametrize("n_runs", [1, 4, 9])
+def test_sim_scan_reverse_and_mixed(pgs, sim, n_runs, pool):
+    """k_scan: the forward list mirrored (all reverse), then forward and reverse requests interleaved in one batch, which
+    sends the forward ones through k_scan too.  The minimal pool holds one block of every run, so chunks end after about
+    one block and the far bound, the cursors and the look-ahead state cross a chunk boundary every few records."""
+    rng = np.random.default_rng(200 + n_runs)
+    hks = SCAN_HKS[:3] + SCAN_HKS[-3:] + [b"hlong0123"]  # its keys are 16 bytes long: the kernel's key slot
+    runs, items = make_db(pgs, rng, n_runs, hks, 24, big=True)
+    vis, best = visible(items)
+    args, keep = run_args(pgs, runs, block_size=512, ri=4)
+    fwd = scan_list(hks)
+    full = dict(start=b"", stop=b"\xff" * 4, start_inclusive=True, stop_inclusive=True, key_mode=0, max_count=1000, max_iter_count=1000,
+                max_iter_size=0)
+    for k in [k for k, _ in vis if len(k) == 16][::5]:  # bounds one byte longer than the slot, equal to a stored key in it
+        for si in (True, False):
+            for ti in (True, False):
+                fwd += [dict(full, start=k + b"\x00", start_inclusive=si, stop_inclusive=ti),
+                        dict(full, stop=k + b"\x00", start_inclusive=si, stop_inclusive=ti)]
+    rev = [mirror(q) for q in fwd]
+    p = 0 if pool == "product" else 1
+    check_scans(vis, rev, do_scans(pgs, sim, args, rev, pool=p))
+    mixed = [q for pair in zip(fwd[0::2], rev[1::2]) for q in pair]
+    check_scans(vis, mixed, do_scans(pgs, sim, args, mixed, pool=p))
 
 
 @pytest.mark.parametrize("n_runs,lanes", [(4, 0), (5, 16)])
@@ -304,11 +177,7 @@ def test_sim_scan_multi_partition(pgs, sim, n_runs, lanes):
     args, keep = run_args(pgs, runs, block_size=512, ri=4)
     reqs = []
     for hk in hks + [b"nope"]:
-        nxt = bytearray(raw_key(hk, b""))
-        while nxt and nxt[-1] == 0xff:
-            nxt.pop()
-        nxt[-1] += 1
-        base = dict(start=raw_key(hk, b""), stop=bytes(nxt), start_inclusive=True, stop_inclusive=False, key_mode=1, prefix=1,
+        base = dict(start=raw_key(hk, b""), stop=next_key(raw_key(hk, b"")), start_inclusive=True, stop_inclusive=False, key_mode=1, prefix=1,
                     max_count=3000, max_iter_count=3000, max_iter_size=0)
         for q in (base, dict(base, max_count=7), dict(base, start=raw_key(hk, b"s0010"), stop=raw_key(hk, b"s0020"), stop_inclusive=True),
                   dict(base, sft=1, spat=b"01", count_only=1),
@@ -319,7 +188,7 @@ def test_sim_scan_multi_partition(pgs, sim, n_runs, lanes):
     for i, (q, g_) in enumerate(zip(reqs, got)):
         want = model_scan(vis_of[i % 3], q, NOW)
         nonempty += want["count"] > 0
-        assert g_ == want, (i, i % 3, q, {k: (g_[k], want[k]) for k in want if g_[k] != want[k]})
+        assert g_ == want, (i, i % 3, q, diff(g_, want))
     assert nonempty > 20
 
 

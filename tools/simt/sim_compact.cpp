@@ -6,6 +6,7 @@
 #define PGS_SIM 1
 #include "../../incubator_pegasus_b200/csrc/compact_kernels.cuh"
 #include "../../incubator_pegasus_b200/csrc/read_kernels.cuh"
+#include "../../incubator_pegasus_b200/csrc/scan_kernel.cuh"
 
 #include <string>
 #include <vector>
@@ -350,10 +351,14 @@ int32_t sim_get(uint32_t k, const uint8_t **data, const uint64_t *data_bytes, co
     return err[0] ? (int32_t)err[0] : PGS_OK;
 }
 
-// k_scan_fwd over k runs; outputs as the device side of scan_many (request i uses arena + i*arena_stride, kvs + i*kv_stride)
+// range scans over k runs; outputs as the device side of scan_many (request i uses arena + i*arena_stride, kvs + i*kv_stride).
+// As scan_launch: a batch without reverse requests runs k_scan_fwd, any other batch k_scan (here without TMA).  pool_bytes
+// (k_scan only): 0 = the pool scan_launch gives a batch of n requests; otherwise at most pool_bytes, but never below the
+// smallest pool scan_launch accepts (one block of every run), so that a small value forces chunks of about one block.
 int32_t sim_scan(uint32_t k, const uint8_t **data, const uint64_t *data_bytes, const uint64_t **blk_off, const uint32_t **blk_size,
                  const uint32_t *n_blocks, const pgs_scan_request *reqs, uint32_t n, uint32_t now, uint64_t arena_stride, uint32_t kv_stride,
-                 uint8_t *arena, pgs_kv *kvs, uint8_t *resume, uint32_t resume_stride, pgs_scan_result *results, uint32_t lanes)
+                 uint8_t *arena, pgs_kv *kvs, uint8_t *resume, uint32_t resume_stride, pgs_scan_result *results, uint32_t lanes,
+                 uint32_t pool_bytes)
 {
     std::vector<HostRun> runs;
     ScanParams P{};
@@ -361,7 +366,7 @@ int32_t sim_scan(uint32_t k, const uint8_t **data, const uint64_t *data_bytes, c
     if (!load_runs(k, data, data_bytes, blk_off, blk_size, n_blocks, runs, P.rr, mk)) return PGS_CORRUPTION;
     std::vector<ScanReqDev> dev(n);
     std::string blob;
-    bool need_crc = false;
+    bool need_crc = false, any_reverse = false;
     for (uint32_t i = 0; i < n; i++) {
         const pgs_scan_request &q = reqs[i];
         ScanReqDev &d = dev[i];
@@ -377,7 +382,7 @@ int32_t sim_scan(uint32_t k, const uint8_t **data, const uint64_t *data_bytes, c
         d.max_count = q.max_count; d.max_iter_count = q.max_iter_count; d.max_iter_size = q.max_iter_size;
         d.pidx = q.pidx; d.partition_version = q.partition_version;
         need_crc |= q.validate_hash != 0;
-        if (q.reverse) return PGS_NOT_SUPPORTED;
+        any_reverse |= q.reverse != 0;
     }
     blob.append(16, '\0'); // as lookup.cu
     uint32_t err[16] = {0};
@@ -385,6 +390,26 @@ int32_t sim_scan(uint32_t k, const uint8_t **data, const uint64_t *data_bytes, c
     P.results = results; P.kvs = kvs; P.kv_stride = kv_stride; P.arena = arena; P.arena_stride = arena_stride;
     P.resume = resume; P.resume_stride = resume_stride; P.error = err; P.ticket = err + 8;
     if (need_crc) { make_crc(); P.crc_table = (const unsigned long long *)crc_tab; }
+    if (any_reverse) {
+        if (lanes) return PGS_INVALID_ARGUMENT; // k_scan has no lane groups and no multi-partition shape
+        uint32_t max_blk = 0, max_rec = 0;
+        for (auto &r : runs) { max_blk = std::max(max_blk, r.info.max_block_size); max_rec = std::max(max_rec, r.info.max_block_records); }
+        P.KS = std::max(8u, (mk + 7) & ~7u); // as snapshot_runs
+        P.use_tma = 0;
+        if (resume_stride < P.KS) resume_stride = 0; // as scan_launch
+        P.resume_stride = resume_stride ? resume_stride : P.KS;
+        const uint64_t max_dyn = 227 * 1024 - sizeof(ScanShared) - 256;
+        uint64_t dyn = scan_dyn_bytes(k, P.KS, max_blk, max_rec, n, max_dyn, &P.pool_bytes);
+        if (!dyn) return PGS_NOT_SUPPORTED;
+        if (pool_bytes) {
+            const uint32_t fixed_dyn = (uint32_t)dyn - P.pool_bytes;
+            const uint32_t one = ((max_blk + 15) & ~15u) + 32 + max_rec * (P.KS + kScanRecExtra);
+            P.pool_bytes = std::max(std::min(P.pool_bytes, pool_bytes), one * std::max(1u, k) + 64 + scan_carve_slack(P.KS));
+            dyn = fixed_dyn + P.pool_bytes;
+        }
+        PGS_LAUNCH(k_scan, std::min(n, 3u), kScanThreads, dyn, 0, P);
+        return err[0] ? (int32_t)err[0] : PGS_OK;
+    }
     // lanes & 0x100: the multi-partition shape of pgs_range_scan_many_multi -- slot 0 owns the runs [0, k/2), slot 1 the rest,
     // slot 2 is an empty partition; request i belongs to slot i % 3
     const bool multi = (lanes & 0x100) != 0;
