@@ -233,7 +233,8 @@ typedef struct {
 
 /* keys: n raw Pegasus keys back to back, key i = keys[key_off[i] .. key_off[i+1]).
  * Values of found, unexpired records are written to `arena` (host memory).  A record whose
- * value does not fit gets PGS_INCOMPLETE and *arena_used is the total need. */
+ * value does not fit gets PGS_INCOMPLETE and *arena_used is the total need.  value_off is 32-bit:
+ * only the first 4 GiB - 1 bytes of the arena are used, whatever arena_cap says. */
 PGS_API int32_t pgs_get_batch(pgs_partition *p, const uint8_t *keys, const uint32_t *key_off,
                               uint32_t n, uint32_t now, uint8_t *arena, uint64_t arena_cap,
                               pgs_get_result *results, uint64_t *arena_used);

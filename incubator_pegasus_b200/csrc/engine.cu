@@ -8,6 +8,7 @@
 #include <cstring>
 
 #include "engine.h"
+#include "index_kernel.cuh"
 #include "read_kernels.cuh"
 
 namespace pgs {
@@ -166,116 +167,6 @@ void Partition::insert(std::shared_ptr<Run> r)
     runs.insert(runs.begin() + pos, std::move(r));
 }
 
-// ------------------------------------------------------------------------------------------------
-// index build: one warp walks one block (entries are sequential inside a restart interval and
-// the last key needs every delta before it), the running internal key lives in a per-warp
-// shared-memory scratch.
-// ------------------------------------------------------------------------------------------------
-struct IndexStats {
-    unsigned long long n_records, n_tomb, raw_key, raw_val, min_seq, max_seq, n_prefix;
-    uint32_t max_ukey, max_vlen, max_blk_rec, error;
-};
-constexpr uint32_t kIdxWarps = 8;
-constexpr uint32_t kIdxScratch = kMaxUkeyLen + 16;
-
-template <bool kEmitKey>
-__global__ void __launch_bounds__(kIdxWarps * 32)
-k_index_walk(const uint8_t *__restrict__ data, const uint64_t *__restrict__ blk_off,
-             const uint32_t *__restrict__ blk_size, uint32_t nb, uint32_t *__restrict__ nrec_out,
-             uint32_t *__restrict__ lastlen_out, const uint32_t *__restrict__ ikey_off,
-             uint8_t *__restrict__ ikeys, const uint32_t *__restrict__ blk_rec, uint32_t *__restrict__ rec_off,
-             uint32_t *__restrict__ bloom, uint32_t bloom_lines, IndexStats *__restrict__ stats, uint32_t b_begin)
-{
-    const Grp<32> g;
-    extern __shared__ __align__(16) uint8_t smem[];
-    uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    uint32_t b = b_begin + blockIdx.x * kIdxWarps + warp; // blocks [b_begin, nb)
-    if (b >= nb) return;
-    uint8_t *scr = smem + warp * kIdxScratch;
-    const uint8_t *base = data + blk_off[b];
-    uint32_t size = blk_size[b];
-    uint32_t err = 0;
-    uint32_t nr = 0;
-    if (size < 8) err = PGS_CORRUPTION;
-    if (!err) {
-        const uint8_t *t = base + size - 4;
-        nr = t[0] | (t[1] << 8) | (t[2] << 16) | ((uint32_t)t[3] << 24);
-        if (nr == 0 || (uint64_t)nr * 4 + 4 > size) err = PGS_CORRUPTION;
-    }
-    uint32_t limit = err ? 0 : size - 4 - 4 * nr;
-    uint32_t p = 0, prev_klen = 0, nrec = 0;
-    unsigned long long raw_key = 0, raw_val = 0, n_tomb = 0, min_seq = ~0ull, max_seq = 0;
-    uint32_t max_ukey = 0, max_vlen = 0, n_prefix = 0, prev_pl = 0xFFFFFFFFu;
-    while (!err && p < limit) {
-        uint32_t shared, non_shared, vlen, h = 0, c;
-        c = get_varint32(base + p, limit - p, shared);
-        h += c;
-        if (c) { c = get_varint32(base + p + h, limit - p - h, non_shared); h += c; }
-        if (c) { c = get_varint32(base + p + h, limit - p - h, vlen); h += c; }
-        if (!c) { err = PGS_CORRUPTION; break; }
-        uint32_t klen = shared + non_shared;
-        if (shared > prev_klen || klen < 8 || (uint64_t)p + h + non_shared + vlen > limit) { err = PGS_CORRUPTION; break; }
-        if (klen > kMaxUkeyLen + 8) { err = PGS_NOT_SUPPORTED; break; }
-        for (uint32_t i = lane; i < non_shared; i += 32) scr[shared + i] = base[p + h + i];
-        if (kEmitKey && lane == 0) rec_off[blk_rec[b] + nrec] = p;
-        __syncwarp();
-        { // Bloom entries: the whole user key, and its hash-key prefix whenever that differs from the previous entry's
-            const uint32_t ulen = klen - 8;
-            const uint32_t pl = hashkey_prefix_len(scr, ulen);
-            const bool new_prefix = pl != 0 && (pl != prev_pl || shared < pl);
-            prev_pl = pl;
-            if (kEmitKey) {
-                if (bloom_lines) {
-                    const unsigned long long hk = bloom_hash_row(g, (const uint32_t *)scr, ulen);
-                    if (lane < 6) bloom_add_bit(bloom, bloom_lines, hk, lane);
-                    if (new_prefix) {
-                        const unsigned long long hp = bloom_hash_row(g, (const uint32_t *)scr, pl);
-                        if (lane < 6) bloom_add_bit(bloom, bloom_lines, hp, lane);
-                    }
-                }
-            } else if (new_prefix) n_prefix++;
-        }
-        if (!kEmitKey && lane == 0) {
-            unsigned long long tr = 0;
-            for (int i = 7; i >= 0; i--) tr = (tr << 8) | scr[klen - 8 + i];
-            unsigned long long seq = tr >> 8;
-            n_tomb += ((uint8_t)tr == PGS_TYPE_DELETION);
-            min_seq = seq < min_seq ? seq : min_seq;
-            max_seq = seq > max_seq ? seq : max_seq;
-            raw_key += klen - 8;
-            raw_val += vlen;
-            max_ukey = max(max_ukey, klen - 8);
-            max_vlen = max(max_vlen, vlen);
-        }
-        __syncwarp();
-        nrec++;
-        prev_klen = klen;
-        p += h + non_shared + vlen;
-    }
-    if (!err && nrec == 0) err = PGS_CORRUPTION;
-    if (kEmitKey) {
-        if (!err) {
-            uint32_t ulen = prev_klen - 8;
-            uint8_t *dst = ikeys + ikey_off[b];
-            for (uint32_t i = lane; i < ulen; i += 32) dst[i] = scr[i];
-        }
-    } else if (lane == 0) {
-        nrec_out[b] = nrec;
-        lastlen_out[b] = err ? 0 : prev_klen - 8;
-        atomicAdd(&stats->n_records, (unsigned long long)nrec);
-        atomicAdd(&stats->n_tomb, n_tomb);
-        atomicAdd(&stats->raw_key, raw_key);
-        atomicAdd(&stats->raw_val, raw_val);
-        atomicAdd(&stats->n_prefix, (unsigned long long)n_prefix);
-        atomicMin(&stats->min_seq, min_seq);
-        atomicMax(&stats->max_seq, max_seq);
-        atomicMax(&stats->max_ukey, max_ukey);
-        atomicMax(&stats->max_vlen, max_vlen);
-        atomicMax(&stats->max_blk_rec, nrec);
-    }
-    if (err && lane == 0) atomicMax(&stats->error, err);
-}
-
 int32_t index_init_kernels()
 {
     const int smem = (int)(kIdxWarps * kIdxScratch);
@@ -417,19 +308,11 @@ static int32_t upload_stage_b(Engine *e, UploadJob &j)
         set_error("run upload: block scan failed with status %u", j.hs.error);
         return (int32_t)j.hs.error;
     }
-    uint64_t rc = 0, kc = 0;
-    for (uint32_t b = 0; b < nb; b++) {
-        j.rec_cum[b] = (uint32_t)rc;
-        j.key_cum[b] = (uint32_t)kc;
-        rc += j.nrec[b];
-        kc += j.lastlen[b];
-    }
-    if (rc > 0xFFFFFFF0ull || kc > 0xFFFFFFF0ull) {
+    if (!index_layout(j.nrec, j.lastlen, nb, j.rec_cum, j.key_cum)) {
         set_error("run too large for 32-bit record / index-key offsets");
         return PGS_NOT_SUPPORTED;
     }
-    j.rec_cum[nb] = (uint32_t)rc;
-    j.key_cum[nb] = (uint32_t)kc;
+    const uint32_t rc = j.rec_cum[nb], kc = j.key_cum[nb];
     PGS_CUDA(cudaMallocAsync(&r->d_blk_rec, sizeof(uint32_t) * (nb + 1), st));
     PGS_CUDA(cudaMallocAsync(&r->d_ikey_off, sizeof(uint32_t) * (nb + 1), st));
     PGS_CUDA(cudaMallocAsync(&r->d_ikeys, kc + 16, st));

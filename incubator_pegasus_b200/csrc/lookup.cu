@@ -409,6 +409,9 @@ static int32_t get_batch_impl(pgs_partition *const *parts, uint32_t n_parts, con
     Engine *e = part.eng;
     if (arena_used) *arena_used = 0;
     if (n == 0) return PGS_OK;
+    // pgs_get_result::value_off is 32-bit: a call uses at most the first 4 GiB - 1 of the arena.  A value that would end
+    // beyond that gets PGS_INCOMPLETE like any value that does not fit, and *arena_used still reports the whole need.
+    arena_cap = std::min<uint64_t>(arena_cap, UINT32_MAX);
     std::vector<std::shared_ptr<Run>> runs; // every run a key may touch stays alive until the launch is done
     GetParams P{};
     std::vector<RunDev> packed;

@@ -81,6 +81,12 @@ def crc64(data):
     return c ^ ((1 << 64) - 1)
 
 
+def expire_ts(v):
+    """BE32 of the value's first four bytes; a value shorter than that (which the reference never writes) has none, as
+    the kernels read it"""
+    return int.from_bytes(v[:4], "big") if len(v) >= 4 else 0
+
+
 def _match(ft, pat, s):
     """validate_filter of the read path (pegasus_server_impl.cpp:2350-2380): an empty pattern matches"""
     if ft == 0 or not pat:
@@ -90,7 +96,7 @@ def _match(ft, pat, s):
 
 def _state(k, v, q, now):
     """validate_key_value_for_scan (:2382-2430): 'normal', 'expired', 'hash' (kHashInvalid) or 'filtered'"""
-    ets = int.from_bytes(v[:4], "big")
+    ets = expire_ts(v)
     if 0 < ets <= now:
         return "expired"
     hl = int.from_bytes(k[:2], "big") if len(k) >= 2 else 0
@@ -169,7 +175,7 @@ def model_scan(vis, q, now=NOW):
             count += 1
             size += len(ko) + len(vo)
             if not q.get("count_only"):
-                kvs.append((ko, vo, int.from_bytes(v[:4], "big") if q.get("return_expire_ts") else 0))
+                kvs.append((ko, vo, expire_ts(v) if q.get("return_expire_ts") else 0))
         if k == end_key:
             complete = True
             break

@@ -21,7 +21,8 @@ def sim():
     so = os.path.join(SIM_DIR, "libpgs_sim.so")
     srcs = [os.path.join(SIM_DIR, f) for f in ("sim_compact.cpp", "simt.h")]
     srcs += [os.path.join(ROOT, "incubator_pegasus_b200", "csrc", f)
-             for f in ("compact_kernels.cuh", "read_kernels.cuh", "scan_kernel.cuh", "group.cuh", "device_util.cuh", "format.h")]
+             for f in ("compact_kernels.cuh", "index_kernel.cuh", "read_kernels.cuh", "scan_kernel.cuh", "group.cuh", "device_util.cuh",
+                       "format.h")]
     if not os.path.exists(so) or any(os.path.getmtime(s) > os.path.getmtime(so) for s in srcs):
         subprocess.check_call(["g++", "-std=c++17", "-O1", "-g", "-fPIC", "-shared", "-Wno-unknown-pragmas",
                                os.path.join(SIM_DIR, "sim_compact.cpp"), "-o", so])

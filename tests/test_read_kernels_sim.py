@@ -8,6 +8,8 @@ import ctypes as C
 import numpy as np
 import pytest
 
+from get_model import (check_results, compacted_run, flat_keys, key_slot, model_get, model_stats, query_keys, sweep_items, sweep_keys,
+                       uploaded_run)
 from incubator_pegasus_b200 import synth
 from scan_model import answer, diff, make_db, mirror, model_scan, next_key, raw_key, scan_list, scan_requests, visible
 from test_kernel_sim import sim, sim_compact  # noqa: F401  (fixture + helper)
@@ -206,4 +208,90 @@ def test_sim_bloom_no_false_negatives(pgs, sim):
     for _ in range(2000):
         k = bytes(rng.integers(0, 256, 50, dtype=np.uint8))
         miss += sim.sim_result_bloom_check(k, len(k))
-    assert miss < 200  # ~1 % expected at 10 bits per entry (the filter is sized for twice the entries here)
+    assert miss < 200  # ~1 % expected at 10 bits per entry
+
+
+# ---- k_get against tests/get_model.py: every result field and the exact probe / skip counts ---------------------------------
+def sim_lookup(pgs, sim, args, keys, use_bloom=1):
+    flat, off = flat_keys(keys)
+    res = (pgs.GetResult * len(keys))()
+    arena = np.zeros(1 << 22, np.uint8)
+    stats = (C.c_uint64 * 3)()
+    st = sim.sim_get(*args, flat.ctypes.data_as(C.c_void_p), off.ctypes.data_as(C.c_void_p), len(keys), NOW,
+                     arena.ctypes.data_as(C.c_void_p), C.c_uint64(arena.shape[0]), res, stats, use_bloom)
+    assert st == 0, st
+    return res, arena, list(stats)
+
+
+def sim_filter(sim, br):
+    """the filter words the upload's k_index_walk builds for one run, in the simulator"""
+    out = np.zeros(1 << 20, np.uint32)
+    lines = sim.sim_run_bloom(br.data.ctypes.data_as(C.c_void_p), C.c_uint64(br.data.shape[0]), br.blk_off.ctypes.data_as(C.c_void_p),
+                              br.blk_size.ctypes.data_as(C.c_void_p), br.n_blocks, out.ctypes.data_as(C.c_void_p), C.c_uint64(out.shape[0]))
+    return out[:16 * lines]
+
+
+def check_lookup(pgs, sim, args, runs, keys, use_bloom=1):
+    res, arena, stats = sim_lookup(pgs, sim, args, keys, use_bloom)
+    want = [model_get(runs, k, NOW) for k in keys]
+    n_ok = check_results(res, arena, keys, want)
+    assert stats[0] == sum((len(w["value"]) + 3) & ~3 for w in want if w["status"] == pgs.OK)
+    assert stats[1:] == list(model_stats(runs, keys)), (stats, model_stats(runs, keys))
+    return n_ok
+
+
+def sample(rng, keys, n):
+    return [keys[i] for i in sorted(rng.permutation(len(keys))[:n])] if len(keys) > n else keys
+
+
+@pytest.mark.parametrize("n_runs,block_size,ri", [(1, 4096, 16), (4, 256, 1), (9, 512, 4)])
+def test_sim_get_against_model(pgs, sim, n_runs, block_size, ri):
+    """user keys of 0..300 bytes, hash keys of 0..140 bytes, 4 KB keys, values shorter than the header, expire_ts == now, and
+    (256 B blocks) a hot key whose 300 versions span many blocks.  The filters the simulated upload builds equal the model's
+    bit for bit, and the probe / skip counters equal model_stats."""
+    rng = np.random.default_rng(40 + n_runs)
+    items = sweep_items(rng, n_runs, sweep_keys(rng, long_keys=n_runs < 9), NOW, hot=300 if block_size == 256 else 0)
+    args, brs = run_args(pgs, [pgs.Records.from_list(it) for it in items], block_size, ri)
+    runs = [uploaded_run(b) for b in brs]
+    for b, r in zip(brs, runs):
+        assert np.array_equal(sim_filter(sim, b), r.bloom.words())
+    keys = sample(rng, query_keys(runs), 1500)
+    assert check_lookup(pgs, sim, args, runs, keys) > 100
+    if n_runs > 1:  # without filters: no run is skipped, the answers stay the same
+        res, arena, stats = sim_lookup(pgs, sim, args, keys[:300], use_bloom=0)
+        check_results(res, arena, keys[:300], [model_get(runs, k, NOW) for k in keys[:300]])
+        assert stats[2] == 0
+
+
+def test_sim_get_multi_partition_against_model(pgs, sim):
+    """pgs_get_batch_multi's kernel shape: slot 0 = the newest 3 runs, slot 1 = the other 3, slot 2 = an empty partition;
+    one key slot for the whole launch, the counters summed over the slots"""
+    rng = np.random.default_rng(77)
+    items = sweep_items(rng, 6, sweep_keys(rng), NOW, hot=200)
+    args, brs = run_args(pgs, [pgs.Records.from_list(it) for it in items], 256, 1)
+    runs = [uploaded_run(b) for b in brs]
+    slots = [runs[:3], runs[3:], []]
+    ks = key_slot([runs])
+    keys = sample(rng, query_keys(runs), 1200)
+    res, arena, stats = sim_lookup(pgs, sim, args, keys, use_bloom=3)
+    want = [model_get(slots[i % 3], k, NOW, ks=ks) for i, k in enumerate(keys)]
+    assert check_results(res, arena, keys, want) > 100
+    per_slot = [model_stats(slots[s], keys[s::3], ks) for s in range(3)]
+    assert stats[1:] == [sum(p[0] for p in per_slot), sum(p[1] for p in per_slot)]
+
+
+def test_sim_get_on_a_compacted_run(pgs, sim):
+    """the oldest three of five runs merged by the simulated compaction: its filter (k_emit's builder, sized as compact.cu
+    sizes it) equals the model's bit for bit, and lookups through it and the two newer uploaded runs match the model"""
+    rng = np.random.default_rng(91)
+    items = sweep_items(rng, 5, sweep_keys(rng, long_keys=False), NOW, hot=250)
+    recs = [pgs.Records.from_list(it) for it in items]
+    out, _ = sim_compact(pgs, sim, recs[2:], bottommost=False, enabled=False, block_size=512, restart_interval=4, seg_weight=16 * 1024)
+    merged = compacted_run(out, [uploaded_run(pgs.build_run(r, 512, 4)) for r in recs[2:]])
+    words = np.zeros(16 * merged.bloom.n_lines, np.uint32)
+    assert sim.sim_result_bloom(words.ctypes.data_as(C.c_void_p), C.c_uint64(words.shape[0])) == merged.bloom.n_lines
+    assert np.array_equal(words, merged.bloom.words())
+    args, brs = run_args(pgs, recs[:2], 512, 4)
+    runs = [uploaded_run(b) for b in brs] + [merged]
+    keys = sample(rng, query_keys(runs), 1500)
+    assert check_lookup(pgs, sim, args, runs, keys, use_bloom=5) > 100

@@ -5,6 +5,7 @@
 
 #define PGS_SIM 1
 #include "../../incubator_pegasus_b200/csrc/compact_kernels.cuh"
+#include "../../incubator_pegasus_b200/csrc/index_kernel.cuh"
 #include "../../incubator_pegasus_b200/csrc/read_kernels.cuh"
 #include "../../incubator_pegasus_b200/csrc/scan_kernel.cuh"
 
@@ -21,6 +22,7 @@ struct HostRun {
     std::vector<uint32_t> blk_size, blk_rec, ikey_off, rec_off;
     std::vector<uint8_t> ikeys;
     std::vector<uint32_t> bloom;
+    uint64_t n_bloom_entries = 0;
     pgs_run_info info{};
     RunDev dev() const
     {
@@ -39,69 +41,44 @@ uint32_t varint(const uint8_t *p, uint32_t &v)
     return 0;
 }
 
-// what k_index_walk builds on the device (engine.cu): record counts, last user keys, entry offsets, run info
+// the run's index and Bloom filter as pgs_run_upload builds them (engine.cu): the two passes of k_index_walk with the host
+// layout between them
 bool build_index(HostRun &r)
 {
     const uint32_t nb = (uint32_t)r.blk_size.size();
+    std::vector<uint32_t> nrec(nb + 1), lastlen(nb + 1);
+    IndexStats st{};
+    st.min_seq = ~0ull;
+    const uint32_t grid = (nb + kIdxWarps - 1) / kIdxWarps, smem = kIdxWarps * kIdxScratch;
+    if (nb)
+        PGS_LAUNCH(k_index_walk<false>, grid, kIdxWarps * 32, smem, 0, (const uint8_t *)r.data.data(), (const uint64_t *)r.blk_off.data(),
+                   (const uint32_t *)r.blk_size.data(), nb, nrec.data(), lastlen.data(), (const uint32_t *)nullptr, (uint8_t *)nullptr,
+                   (const uint32_t *)nullptr, (uint32_t *)nullptr, (uint32_t *)nullptr, 0u, &st, 0u);
+    if (st.error) return false;
     r.blk_rec.assign(nb + 1, 0);
     r.ikey_off.assign(nb + 1, 0);
-    r.info.n_blocks = nb;
-    r.info.smallest_seq = ~0ull;
-    std::string key;
-    std::vector<std::string> all_keys;
-    for (uint32_t b = 0; b < nb; b++) {
-        const uint8_t *base = r.data.data() + r.blk_off[b];
-        const uint32_t size = r.blk_size[b];
-        if (size < 8) return false;
-        uint32_t nr;
-        memcpy(&nr, base + size - 4, 4);
-        const uint32_t limit = size - 4 - 4 * nr;
-        uint32_t p = 0, n = 0;
-        key.clear();
-        while (p < limit) {
-            uint32_t sh, ns, vl, h = 0, c;
-            c = varint(base + p, sh); h += c;
-            c = varint(base + p + h, ns); h += c;
-            c = varint(base + p + h, vl); h += c;
-            if (!c || sh > key.size()) return false;
-            key.resize(sh);
-            key.append((const char *)base + p + h, ns);
-            r.rec_off.push_back(p);
-            all_keys.emplace_back(key.data(), key.size() - 8);
-            unsigned long long tr;
-            memcpy(&tr, key.data() + key.size() - 8, 8);
-            r.info.n_tombstones += (uint8_t)tr == PGS_TYPE_DELETION;
-            r.info.smallest_seq = std::min<uint64_t>(r.info.smallest_seq, tr >> 8);
-            r.info.largest_seq = std::max<uint64_t>(r.info.largest_seq, tr >> 8);
-            r.info.raw_key_bytes += key.size() - 8;
-            r.info.raw_value_bytes += vl;
-            r.info.max_ukey_len = std::max<uint32_t>(r.info.max_ukey_len, (uint32_t)key.size() - 8);
-            r.info.max_value_len = std::max(r.info.max_value_len, vl);
-            p += h + ns + vl;
-            n++;
-        }
-        r.blk_rec[b + 1] = r.blk_rec[b] + n;
-        r.ikeys.insert(r.ikeys.end(), key.begin(), key.end() - 8);
-        r.ikey_off[b + 1] = (uint32_t)r.ikeys.size();
-        r.info.max_block_size = std::max(r.info.max_block_size, size);
-        r.info.max_block_records = std::max(r.info.max_block_records, n);
-        r.info.n_records += n;
-    }
-    r.ikeys.resize(r.ikeys.size() + 16); // the product's slack (engine.cu)
-    r.rec_off.push_back(0);
-    // the Bloom filter k_index_walk builds at upload: whole keys + hash-key prefixes
-    std::vector<std::string> pres;
-    for (auto &k : all_keys) {
-        const uint32_t pl = hashkey_prefix_len((const uint8_t *)k.data(), (uint32_t)k.size());
-        if (pl && (pres.empty() || pres.back() != k.substr(0, pl))) pres.push_back(k.substr(0, pl));
-    }
-    const uint32_t lines = bloom_lines_for(all_keys.size() + pres.size());
+    if (!index_layout(nrec.data(), lastlen.data(), nb, r.blk_rec.data(), r.ikey_off.data())) return false;
+    r.ikeys.assign(r.ikey_off[nb] + 16, 0); // the product's slack (engine.cu)
+    r.rec_off.assign(r.blk_rec[nb] + 1, 0);
+    r.n_bloom_entries = st.n_records + st.n_prefix;
+    const uint32_t lines = bloom_lines_for(r.n_bloom_entries);
     r.bloom.assign((size_t)lines * 16, 0);
-    for (auto *v : {&all_keys, &pres})
-        for (auto &k : *v) {
-            const unsigned long long h = bloom_hash_bytes((const uint8_t *)k.data(), (uint32_t)k.size());
-            for (uint32_t s = 0; s < 6; s++) bloom_add_bit(r.bloom.data(), lines, h, s);
-        }
+    if (nb)
+        PGS_LAUNCH(k_index_walk<true>, grid, kIdxWarps * 32, smem, 0, (const uint8_t *)r.data.data(), (const uint64_t *)r.blk_off.data(),
+                   (const uint32_t *)r.blk_size.data(), nb, (uint32_t *)nullptr, (uint32_t *)nullptr, (const uint32_t *)r.ikey_off.data(),
+                   r.ikeys.data(), (const uint32_t *)r.blk_rec.data(), r.rec_off.data(), r.bloom.data(), lines, &st, 0u);
+    if (st.error) return false;
+    r.info.n_blocks = nb;
+    r.info.n_records = st.n_records;
+    r.info.n_tombstones = st.n_tomb;
+    r.info.raw_key_bytes = st.raw_key;
+    r.info.raw_value_bytes = st.raw_val;
+    r.info.max_ukey_len = st.max_ukey;
+    r.info.max_value_len = st.max_vlen;
+    r.info.max_block_records = st.max_blk_rec;
+    r.info.smallest_seq = st.min_seq;
+    r.info.largest_seq = st.max_seq;
+    for (uint32_t b = 0; b < nb; b++) r.info.max_block_size = std::max(r.info.max_block_size, r.blk_size[b]);
     return true;
 }
 
@@ -141,6 +118,7 @@ int32_t sim_compact(uint32_t k, const uint8_t **data, const uint64_t *data_bytes
     MergeParams P{};
     P.k = k;
     CompactTotals T{};
+    uint64_t bloom_entries = 0;
     for (uint32_t i = 0; i < k; i++) {
         HostRun &r = runs[i];
         r.data.assign(data[i], data[i] + data_bytes[i]);
@@ -161,6 +139,7 @@ int32_t sim_compact(uint32_t k, const uint8_t **data, const uint64_t *data_bytes
         T.raw_key += r.info.raw_key_bytes;
         T.raw_val += r.info.raw_value_bytes;
         T.in_block_bytes += r.info.data_bytes;
+        bloom_entries += r.n_bloom_entries; // as compact.cu sizes the output's filter
     }
     P.block_size = block_size;
     P.restart_interval = restart_interval;
@@ -212,7 +191,7 @@ int32_t sim_compact(uint32_t k, const uint8_t **data, const uint64_t *data_bytes
     R.ikey_off.assign(geo.blk_cap + 1, 0);
     R.ikeys.assign(geo.ikey_cap, 0);
     R.rec_off.assign(T.n_rec + 1, 0);
-    R.bloom_lines = bloom_lines_for(2 * T.n_rec);
+    R.bloom_lines = bloom_lines_for(bloom_entries);
     R.bloom.assign((size_t)R.bloom_lines * 16, 0);
     P.out_bloom = R.bloom.data();
     P.out_bloom_lines = R.bloom_lines;
@@ -296,6 +275,29 @@ int32_t sim_result_bloom_check(const uint8_t *key, uint32_t len)
     return bloom_may_contain(g_res.bloom.data(), g_res.bloom_lines, bloom_hash_bytes(key, len)) ? 1 : 0;
 }
 
+// the Bloom filter of the last sim_compact output (the one k_emit built): up to cap words; returns its number of lines
+uint32_t sim_result_bloom(uint32_t *out, uint64_t cap)
+{
+    memcpy(out, g_res.bloom.data(), 4 * std::min<uint64_t>(cap, g_res.bloom.size()));
+    return g_res.bloom_lines;
+}
+
+// the Bloom filter the upload builds for one run (k_index_walk): up to cap words; returns its number of lines (0: corrupt run)
+uint32_t sim_run_bloom(const uint8_t *data, uint64_t data_bytes, const uint64_t *blk_off, const uint32_t *blk_size, uint32_t n_blocks,
+                       uint32_t *out, uint64_t cap)
+{
+    HostRun r;
+    r.data.assign(data, data + data_bytes);
+    r.data.resize(r.data.size() + 256, 0);
+    r.blk_off.assign(blk_off, blk_off + n_blocks);
+    r.blk_size.assign(blk_size, blk_size + n_blocks);
+    const uint64_t end = n_blocks ? r.blk_off.back() + r.blk_size.back() : 0;
+    r.blk_off.push_back((end + 15) & ~15ull);
+    if (!build_index(r)) return 0;
+    memcpy(out, r.bloom.data(), 4 * std::min<uint64_t>(cap, r.bloom.size()));
+    return (uint32_t)(r.bloom.size() / 16);
+}
+
 static bool load_runs(uint32_t k, const uint8_t **data, const uint64_t *data_bytes, const uint64_t **blk_off, const uint32_t **blk_size,
                       const uint32_t *n_blocks, std::vector<HostRun> &runs, ReadRuns &rr, uint32_t &max_ukey)
 {
@@ -317,7 +319,8 @@ static bool load_runs(uint32_t k, const uint8_t **data, const uint64_t *data_byt
     return true;
 }
 
-// k_get over k runs (newest first); results / arena as pgs_get_batch.  stats[0] = arena bytes, [1] = blocks probed, [2] = runs skipped
+// k_get over k runs (newest first); results / arena as pgs_get_batch.  stats[0] = arena bytes, [1] = blocks probed, [2] = runs skipped.
+// use_bloom: 1 = the runs' filters are used; 2 = the multi-partition shape (below); 4 = the last sim_compact output is the oldest run
 int32_t sim_get(uint32_t k, const uint8_t **data, const uint64_t *data_bytes, const uint64_t **blk_off, const uint32_t **blk_size,
                 const uint32_t *n_blocks, const uint8_t *keys, const uint32_t *key_off, uint32_t n, uint32_t now, uint8_t *arena,
                 uint64_t arena_cap, pgs_get_result *results, uint64_t *stats, uint32_t use_bloom)
@@ -326,6 +329,14 @@ int32_t sim_get(uint32_t k, const uint8_t **data, const uint64_t *data_bytes, co
     GetParams P{};
     uint32_t mk = 0;
     if (!load_runs(k, data, data_bytes, blk_off, blk_size, n_blocks, runs, P.rr, mk)) return PGS_CORRUPTION;
+    if (use_bloom & 4) { // the run of the last sim_compact call joins as the oldest run, with the index and filter k_emit wrote
+        const Result &R = g_res;
+        if (k >= kMaxReadRuns || !R.st.tot_blocks) return PGS_INVALID_ARGUMENT;
+        P.rr.runs[k] = RunDev{R.data.data(), R.blk_off.data(), R.blk_size.data(), R.blk_rec.data(), R.ikey_off.data(), R.ikeys.data(),
+                              R.rec_off.data(), R.bloom.data(), R.bloom_lines, (uint32_t)R.st.tot_blocks, (uint32_t)R.st.mx[SM_UKEY], 0};
+        mk = std::max(mk, (uint32_t)R.st.mx[SM_UKEY]);
+        P.rr.n = ++k;
+    }
     if (!(use_bloom & 1)) for (uint32_t i = 0; i < k; i++) { P.rr.runs[i].bloom = nullptr; P.rr.runs[i].bloom_lines = 0; }
     std::vector<uint8_t> kcopy(keys, keys + key_off[n]);
     kcopy.resize(kcopy.size() + 16); // as lookup.cu allocates the key buffer
@@ -333,7 +344,7 @@ int32_t sim_get(uint32_t k, const uint8_t **data, const uint64_t *data_bytes, co
     uint32_t err[4] = {0, 0, 0, 0};
     P.keys = kcopy.data(); P.key_off = key_off; P.n = n; P.now = now; P.data_version = 1;
     P.results = results; P.arena = arena; P.arena_cap = arena_cap; P.arena_cursor = cur; P.error = err; P.ticket = err + 1;
-    P.KS = std::max(8u, (mk + 3) & ~3u);
+    P.KS = std::max(8u, (mk + 7) & ~7u); // as snapshot_runs
     P.KSW = (P.KS + 8) / 4 + 1;
     P.group_smem = (uint32_t)((sizeof(CurState) + 2 * P.KSW * 4 + 15) & ~(size_t)15);
     const uint32_t dyn = kMaxReadRuns * (uint32_t)sizeof(RunDev) + (kReadThreads / 8) * P.group_smem;
