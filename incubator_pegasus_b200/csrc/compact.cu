@@ -10,22 +10,7 @@
 #include "engine.h"
 
 namespace pgs {
-const uint64_t *crc64_table();
-static uint64_t *g_crc_dev[16] = {nullptr};
-static std::mutex g_crc_mu;
 // the opt-in shared-memory maximum of the compaction kernels, once per device (a per-call cudaFuncSetAttribute would race)
-typedef void (*walk_kernel_t)(const MergeParams);
-static const uint32_t kWalkGs[] = {1, 2, 4, 8, 16};
-static walk_kernel_t walk_kernel(uint32_t G)
-{
-    switch (G) {
-    case 1: return k_walk<1>;
-    case 2: return k_walk<2>;
-    case 4: return k_walk<4>;
-    case 8: return k_walk<8>;
-    default: return k_walk<16>;
-    }
-}
 int32_t compact_init_kernels(int max_smem)
 {
     cudaFuncAttributes a;
@@ -81,19 +66,10 @@ extern "C" int32_t pgs_compact_ex(pgs_partition *ph, const uint64_t *run_ids, ui
     MergeParams P{};
     P.k = k;
     CompactTotals T{};
-    uint64_t bloom_entries = 0;
     for (uint32_t i = 0; i < k; i++) {
         P.runs[i] = in[i]->dev();
         const pgs_run_info &fi = in[i]->info;
-        T.max_ukey = std::max(T.max_ukey, fi.max_ukey_len);
-        T.max_blk = std::max(T.max_blk, fi.max_block_size);
-        T.max_blk_rec = std::max(T.max_blk_rec, fi.max_block_records);
-        T.total_blocks += fi.n_blocks;
-        T.n_rec += fi.n_records;
-        T.raw_key += fi.raw_key_bytes;
-        T.raw_val += fi.raw_value_bytes;
-        T.in_block_bytes += fi.data_bytes;
-        bloom_entries += in[i]->n_bloom_entries ? in[i]->n_bloom_entries : 2 * fi.n_records;
+        T.add(fi, in[i]->n_bloom_entries);
         if (fi.n_blocks >= (1u << 28) || fi.data_bytes >= (1ull << 40)) return PGS_NOT_SUPPORTED;
     }
     if (T.max_ukey > kMaxUkeyLen) { set_error("compact: user key of %u bytes > %u", T.max_ukey, kMaxUkeyLen); return PGS_NOT_SUPPORTED; }
@@ -133,69 +109,41 @@ extern "C" int32_t pgs_compact_ex(pgs_partition *ph, const uint64_t *run_ids, ui
     auto outr = std::make_shared<Run>();
     outr->level = out_level;
     outr->data_cap = geo.out_cap + 256;
-    uint32_t *d_split_pos = nullptr, *d_split_ref = nullptr, *d_ticket = nullptr;
-    SegLayout *d_seg = nullptr;
-    SegAgg *d_agg = nullptr;
-    SegBase *d_base = nullptr;
-    Desc *d_desc = nullptr;
-    uint8_t *d_heads = nullptr;
-    MergeStats *d_stats = nullptr;
-    uint8_t *d_ops = nullptr;
-    auto cleanup = [&]() {
-        cudaFreeAsync(d_split_pos, st); cudaFreeAsync(d_split_ref, st); cudaFreeAsync(d_ticket, st);
-        cudaFreeAsync(d_seg, st); cudaFreeAsync(d_agg, st); cudaFreeAsync(d_base, st); cudaFreeAsync(d_desc, st); cudaFreeAsync(d_heads, st);
-        cudaFreeAsync(d_stats, st); cudaFreeAsync(d_ops, st);
-    };
+    LaunchScratch S(st);
     outr->pool_stream = st;
-#define CK(expr) do { cudaError_t _e = (expr); if (_e != cudaSuccess) { cleanup(); return cuda_fail(_e, #expr); } } while (0)
     outr->eng = e;
     { uint64_t cap = 0; outr->d_data = outr->data_cap >= (64ull << 20) ? e->take_data(outr->data_cap, &cap) : nullptr; if (outr->d_data) outr->data_cap = cap; }
-    if (!outr->d_data) CK(cudaMallocAsync(&outr->d_data, outr->data_cap, st));
-    CK(cudaMallocAsync(&outr->d_blk_off, sizeof(uint64_t) * (geo.blk_cap + 1), st));
-    CK(cudaMallocAsync(&outr->d_blk_size, sizeof(uint32_t) * (geo.blk_cap + 1), st));
-    CK(cudaMallocAsync(&outr->d_blk_rec, sizeof(uint32_t) * (geo.blk_cap + 1), st));
-    CK(cudaMallocAsync(&outr->d_ikey_off, sizeof(uint32_t) * (geo.blk_cap + 1), st));
-    CK(cudaMallocAsync(&outr->d_ikeys, geo.ikey_cap, st));
-    CK(cudaMallocAsync(&outr->d_rec_off, sizeof(uint32_t) * (T.n_rec + 1), st));
-    outr->bloom_lines = bloom_lines_for(bloom_entries);
-    CK(cudaMallocAsync(&outr->d_bloom, (size_t)outr->bloom_lines * 64, st));
-    CK(cudaMemsetAsync(outr->d_bloom, 0, (size_t)outr->bloom_lines * 64, st));
-    CK(cudaMallocAsync(&d_split_pos, sizeof(uint32_t) * (Q + 1) * k, st));
-    CK(cudaMallocAsync(&d_split_ref, sizeof(uint32_t) * (Q + 1), st));
-    CK(cudaMallocAsync(&d_ticket, 256, st));
-    CK(cudaMallocAsync(&d_seg, sizeof(SegLayout) * Q, st));
-    CK(cudaMallocAsync(&d_agg, sizeof(SegAgg) * Q, st));
-    CK(cudaMallocAsync(&d_base, sizeof(SegBase) * Q, st));
-    CK(cudaMallocAsync(&d_desc, sizeof(Desc) * P.desc_cap, st));
-    CK(cudaMallocAsync(&d_heads, P.head_cap + 64, st));
-    CK(cudaMallocAsync(&d_stats, sizeof(MergeStats), st));
-    CK(cudaMemsetAsync(d_split_pos, 0xFF, sizeof(uint32_t) * (Q + 1) * k, st));
-    CK(cudaMemsetAsync(d_split_ref, 0xFF, sizeof(uint32_t) * (Q + 1), st));
-    CK(cudaMemsetAsync(d_ticket, 0, 256, st));
-    CK(cudaMemsetAsync(d_agg, 0, sizeof(SegAgg) * Q, st));
+    if (!outr->d_data) PGS_CUDA(cudaMallocAsync(&outr->d_data, outr->data_cap, st));
+    PGS_CUDA(cudaMallocAsync(&outr->d_blk_off, sizeof(uint64_t) * (geo.blk_cap + 1), st));
+    PGS_CUDA(cudaMallocAsync(&outr->d_blk_size, sizeof(uint32_t) * (geo.blk_cap + 1), st));
+    PGS_CUDA(cudaMallocAsync(&outr->d_blk_rec, sizeof(uint32_t) * (geo.blk_cap + 1), st));
+    PGS_CUDA(cudaMallocAsync(&outr->d_ikey_off, sizeof(uint32_t) * (geo.blk_cap + 1), st));
+    PGS_CUDA(cudaMallocAsync(&outr->d_ikeys, geo.ikey_cap, st));
+    PGS_CUDA(cudaMallocAsync(&outr->d_rec_off, sizeof(uint32_t) * (T.n_rec + 1), st));
+    outr->bloom_lines = bloom_lines_for(T.bloom_entries);
+    PGS_CUDA(cudaMallocAsync(&outr->d_bloom, (size_t)outr->bloom_lines * 64, st));
+    PGS_CUDA(cudaMemsetAsync(outr->d_bloom, 0, (size_t)outr->bloom_lines * 64, st));
+    PGS_CUDA(S.alloc(P.split_pos, sizeof(uint32_t) * (Q + 1) * k));
+    PGS_CUDA(S.alloc(P.split_ref, sizeof(uint32_t) * (Q + 1)));
+    PGS_CUDA(S.alloc(P.ticket, 256));
+    PGS_CUDA(S.alloc(P.seg, sizeof(SegLayout) * Q));
+    PGS_CUDA(S.alloc(P.agg, sizeof(SegAgg) * Q));
+    PGS_CUDA(S.alloc(P.base, sizeof(SegBase) * Q));
+    PGS_CUDA(S.alloc(P.desc, sizeof(Desc) * P.desc_cap));
+    PGS_CUDA(S.alloc(P.heads, P.head_cap + 64));
+    PGS_CUDA(cudaMemsetAsync(P.split_pos, 0xFF, sizeof(uint32_t) * (Q + 1) * k, st));
+    PGS_CUDA(cudaMemsetAsync(P.split_ref, 0xFF, sizeof(uint32_t) * (Q + 1), st));
+    PGS_CUDA(cudaMemsetAsync(P.ticket, 0, 256, st));
+    PGS_CUDA(cudaMemsetAsync(P.agg, 0, sizeof(SegAgg) * Q, st));
     MergeStats hs{};
     hs.error_seg = 0xFFFFFFFFu;
-    CK(cudaMemcpyAsync(d_stats, &hs, sizeof hs, cudaMemcpyHostToDevice, st));
+    PGS_CUDA(S.upload(P.stats, &hs, 1));
     if (!ops_host.empty()) {
-        CK(cudaMallocAsync(&d_ops, ops_host.size(), st));
-        CK(cudaMemcpyAsync(d_ops, ops_host.data(), ops_host.size(), cudaMemcpyHostToDevice, st));
+        uint8_t *d_ops = nullptr;
+        PGS_CUDA(S.upload(d_ops, ops_host.data(), ops_host.size()));
         P.ops = d_ops;
     }
-    if (P.validate_hash) {
-        std::lock_guard<std::mutex> g(g_crc_mu);
-        int dev = e->device;
-        if (!g_crc_dev[dev & 15]) {
-            uint64_t *t = nullptr;
-            CK(cudaMalloc(&t, 256 * 8));
-            CK(cudaMemcpyAsync(t, crc64_table(), 256 * 8, cudaMemcpyHostToDevice, st));
-            g_crc_dev[dev & 15] = t;
-        }
-        P.crc_table = (const unsigned long long *)g_crc_dev[dev & 15];
-    }
-    P.split_pos = d_split_pos;
-    P.split_ref = d_split_ref;
-    P.ticket = d_ticket;
-    P.seg = d_seg; P.agg = d_agg; P.base = d_base; P.desc = d_desc; P.heads = d_heads;
+    if (P.validate_hash) P.crc_table = (const unsigned long long *)e->d_crc;
     P.out_data = outr->d_data;
     P.out_blk_off = (unsigned long long *)outr->d_blk_off;
     P.out_blk_size = outr->d_blk_size;
@@ -205,67 +153,44 @@ extern "C" int32_t pgs_compact_ex(pgs_partition *ph, const uint64_t *run_ids, ui
     P.out_rec_off = outr->d_rec_off;
     P.out_bloom = outr->d_bloom;
     P.out_bloom_lines = outr->bloom_lines;
-    P.stats = d_stats;
 
     cudaEvent_t ev[4];
-    for (auto &x : ev) CK(cudaEventCreate(&x));
+    for (auto &x : ev) PGS_CUDA(S.event(x));
     walk_kernel_t walk = walk_kernel(geo.G);
     int occ_w = 0, occ_e = 0;
-    CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_w, walk, (int)kWalkThreads, (size_t)geo.walk_dyn));
-    CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_e, k_emit, (int)(geo.emit_warps * 32), (size_t)geo.emit_dyn));
+    PGS_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_w, walk, (int)kWalkThreads, (size_t)geo.walk_dyn));
+    PGS_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_e, k_emit, (int)(geo.emit_warps * 32), (size_t)geo.emit_dyn));
     const uint32_t seg_per_cta_w = kWalkThreads / geo.G;
     const uint32_t grid_w = (uint32_t)std::min<uint64_t>((Q + seg_per_cta_w - 1) / seg_per_cta_w, (uint64_t)std::max(1, occ_w) * e->sm_count);
     const uint32_t grid_e = (uint32_t)std::min<uint64_t>((Q + geo.emit_warps - 1) / geo.emit_warps, (uint64_t)std::max(1, occ_e) * e->sm_count);
-    CK(cudaEventRecord(ev[0], st));
+    PGS_CUDA(cudaEventRecord(ev[0], st));
     k_plan<<<(uint32_t)((T.total_blocks + 255) / 256), 256, 0, st>>>(P);
     k_seg_bounds<<<(uint32_t)((Q + 255) / 256), 256, 0, st>>>(P);
     k_seg_layout<<<1, 1024, 0, st>>>(P);
-    CK(cudaEventRecord(ev[1], st));
+    PGS_CUDA(cudaEventRecord(ev[1], st));
     walk<<<grid_w, kWalkThreads, geo.walk_dyn, st>>>(P);
-    CK(cudaEventRecord(ev[2], st));
+    PGS_CUDA(cudaEventRecord(ev[2], st));
     k_seg_scan<<<1, 1024, 0, st>>>(P);
     k_emit<<<grid_e, geo.emit_warps * 32, geo.emit_dyn, st>>>(P);
-    CK(cudaEventRecord(ev[3], st));
+    PGS_CUDA(cudaEventRecord(ev[3], st));
     e->launches += 6;
-    CK(cudaMemcpyAsync(&hs, d_stats, sizeof hs, cudaMemcpyDeviceToHost, st));
+    PGS_CUDA(cudaMemcpyAsync(&hs, P.stats, sizeof hs, cudaMemcpyDeviceToHost, st));
     cudaError_t se = cudaStreamSynchronize(st);
-    if (se != cudaSuccess) { cleanup(); return cuda_fail(se, "compaction kernels"); }
+    if (se != cudaSuccess) return cuda_fail(se, "compaction kernels");
     float ms_total = 0, ms_merge = 0, ms_walk = 0, ms_emit = 0;
     cudaEventElapsedTime(&ms_total, ev[0], ev[3]);
     cudaEventElapsedTime(&ms_merge, ev[1], ev[3]);
     cudaEventElapsedTime(&ms_walk, ev[1], ev[2]);
     cudaEventElapsedTime(&ms_emit, ev[2], ev[3]);
-    for (auto &x : ev) cudaEventDestroy(x);
-    cleanup();
-#undef CK
     if (hs.error) {
         set_error("compaction kernel failed with status %u at segment %u of %u", hs.error, hs.error_seg, P.Q);
         return (int32_t)hs.error;
     }
-    res.in_records = hs.cnt[EV_IN]; res.out_records = hs.cnt[EV_OUT];
-    res.in_bytes = hs.bytes[SB_IN]; res.out_bytes = hs.bytes[SB_OUT];
-    res.in_block_bytes = T.in_block_bytes; res.out_block_bytes = hs.tot_bytes;
-    res.dropped_shadowed = hs.cnt[EV_SHADOW]; res.dropped_tombstone = hs.cnt[EV_TOMB];
-    res.dropped_expired = hs.cnt[EV_EXPIRED]; res.dropped_user = hs.cnt[EV_USER]; res.dropped_stale = hs.cnt[EV_STALE];
-    res.ttl_rewritten = hs.cnt[EV_TTL];
+    outr->n_bloom_entries = compact_result_stats(hs, T.in_block_bytes, res, outr->info);
+    outr->info.level = out_level;
     res.n_tiles = P.Q; res.n_launches = 6;
     res.device_ms = ms_total; res.merge_kernel_ms = ms_merge;
     res.walk_ms = ms_walk; res.emit_ms = ms_emit;
-
-    outr->info.level = out_level;
-    outr->info.n_blocks = (uint32_t)hs.tot_blocks;
-    outr->info.n_records = hs.tot_recs;
-    outr->info.n_tombstones = hs.cnt[EV_OUT_TOMB];
-    outr->info.data_bytes = hs.tot_bytes;
-    outr->info.raw_key_bytes = hs.bytes[SB_OUT_KEY];
-    outr->info.raw_value_bytes = hs.bytes[SB_OUT_VAL];
-    outr->info.max_ukey_len = (uint32_t)hs.mx[SM_UKEY];
-    outr->info.max_value_len = (uint32_t)hs.mx[SM_VLEN];
-    outr->info.max_block_size = (uint32_t)hs.mx[SM_BLK_SIZE];
-    outr->info.max_block_records = (uint32_t)hs.mx[SM_BLK_REC];
-    outr->info.smallest_seq = hs.tot_recs ? (~hs.mx[SM_MIN_SEQ_INV] & ((1ull << 56) - 1)) : ~0ull;
-    outr->info.largest_seq = hs.mx[SM_MAX_SEQ];
-    outr->n_bloom_entries = hs.cnt[EV_BLOOM_KEY] + hs.cnt[EV_BLOOM_PREFIX];
     {
         std::lock_guard<std::mutex> g(part.mu);
         if (!(flags & PGS_COMPACT_KEEP_INPUTS))

@@ -27,6 +27,8 @@
 //                 the finished block leaves with ONE bulk TMA store; the new run's index is written alongside.
 //   Output blocks stay contiguous and in key order; every segment starts a new block.
 #pragma once
+#include <algorithm>
+
 #include "group.cuh"
 
 namespace pgs {
@@ -118,7 +120,45 @@ struct MergeParams {
 struct CompactTotals { // sums / maxima over the input runs' pgs_run_info
     uint32_t max_ukey, max_blk, max_blk_rec;
     uint64_t total_blocks, n_rec, raw_key, raw_val, in_block_bytes;
+    uint64_t bloom_entries; // sizes the output's Bloom filter
+    // n_bloom_entries: what went into the input's filter (0: not known, two per record are assumed)
+    void add(const pgs_run_info &fi, uint64_t n_bloom_entries)
+    {
+        max_ukey = std::max(max_ukey, fi.max_ukey_len);
+        max_blk = std::max(max_blk, fi.max_block_size);
+        max_blk_rec = std::max(max_blk_rec, fi.max_block_records);
+        total_blocks += fi.n_blocks;
+        n_rec += fi.n_records;
+        raw_key += fi.raw_key_bytes;
+        raw_val += fi.raw_value_bytes;
+        in_block_bytes += fi.data_bytes;
+        bloom_entries += n_bloom_entries ? n_bloom_entries : 2 * fi.n_records;
+    }
 };
+// a finished merge's counters as pgs_compact_result reports them, and the merged run's pgs_run_info (without level and run
+// id); returns the entries of the merged run's Bloom filter
+inline uint64_t compact_result_stats(const MergeStats &s, uint64_t in_block_bytes, pgs_compact_result &res, pgs_run_info &info)
+{
+    res.in_records = s.cnt[EV_IN]; res.out_records = s.cnt[EV_OUT];
+    res.in_bytes = s.bytes[SB_IN]; res.out_bytes = s.bytes[SB_OUT];
+    res.in_block_bytes = in_block_bytes; res.out_block_bytes = s.tot_bytes;
+    res.dropped_shadowed = s.cnt[EV_SHADOW]; res.dropped_tombstone = s.cnt[EV_TOMB];
+    res.dropped_expired = s.cnt[EV_EXPIRED]; res.dropped_user = s.cnt[EV_USER]; res.dropped_stale = s.cnt[EV_STALE];
+    res.ttl_rewritten = s.cnt[EV_TTL];
+    info.n_blocks = (uint32_t)s.tot_blocks;
+    info.n_records = s.tot_recs;
+    info.n_tombstones = s.cnt[EV_OUT_TOMB];
+    info.data_bytes = s.tot_bytes;
+    info.raw_key_bytes = s.bytes[SB_OUT_KEY];
+    info.raw_value_bytes = s.bytes[SB_OUT_VAL];
+    info.max_ukey_len = (uint32_t)s.mx[SM_UKEY];
+    info.max_value_len = (uint32_t)s.mx[SM_VLEN];
+    info.max_block_size = (uint32_t)s.mx[SM_BLK_SIZE];
+    info.max_block_records = (uint32_t)s.mx[SM_BLK_REC];
+    info.smallest_seq = s.tot_recs ? (~s.mx[SM_MIN_SEQ_INV] & ((1ull << 56) - 1)) : ~0ull;
+    info.largest_seq = s.mx[SM_MAX_SEQ];
+    return s.cnt[EV_BLOOM_KEY] + s.cnt[EV_BLOOM_PREFIX];
+}
 struct CompactGeometry {
     uint32_t G, walk_dyn, emit_warps, emit_dyn;
     uint64_t blk_cap, out_cap, ikey_cap;
@@ -1350,6 +1390,20 @@ __global__ void __launch_bounds__(kEmitThreads, 5) k_emit(const __grid_constant_
         tma_store_wait_all();
         if (n_bloom_keys) atomicAdd(&P.stats->cnt[EV_BLOOM_KEY], (unsigned long long)n_bloom_keys);
         if (n_bloom_prefixes) atomicAdd(&P.stats->cnt[EV_BLOOM_PREFIX], (unsigned long long)n_bloom_prefixes);
+    }
+}
+
+// the k_walk instantiation for G lanes per merge group (host side)
+typedef void (*walk_kernel_t)(const MergeParams);
+constexpr uint32_t kWalkGs[] = {1, 2, 4, 8, 16};
+inline walk_kernel_t walk_kernel(uint32_t G)
+{
+    switch (G) {
+    case 1: return k_walk<1>;
+    case 2: return k_walk<2>;
+    case 4: return k_walk<4>;
+    case 8: return k_walk<8>;
+    default: return k_walk<16>;
     }
 }
 

@@ -9,7 +9,6 @@
 
 #include "engine.h"
 #include "index_kernel.cuh"
-#include "read_kernels.cuh"
 
 namespace pgs {
 
@@ -128,6 +127,7 @@ Engine::~Engine()
     for (auto &s : rd_streams) if (s) cudaStreamDestroy(s);
     if (up_copy) cudaStreamDestroy(up_copy);
     for (auto &pn : pins) cudaFreeHost(pn.p);
+    if (d_crc) cudaFree(d_crc);
     if (stream) cudaStreamDestroy(stream);
 }
 cudaStream_t Engine::read_stream()
@@ -337,16 +337,7 @@ static int32_t upload_stage_c(Engine *e, Partition &p, UploadJob &j, uint64_t *r
     PGS_CUDA(cudaEventSynchronize(j.pass1));
     cudaFreeAsync(j.d_stats, e->stream);
     j.d_stats = nullptr;
-    r->info.n_records = j.hs.n_records;
-    r->info.n_tombstones = j.hs.n_tomb;
-    r->info.raw_key_bytes = j.hs.raw_key;
-    r->info.raw_value_bytes = j.hs.raw_val;
-    r->info.max_ukey_len = j.hs.max_ukey;
-    r->info.max_value_len = j.hs.max_vlen;
-    r->info.max_block_size = j.max_blk;
-    r->info.max_block_records = j.hs.max_blk_rec;
-    r->info.smallest_seq = j.hs.min_seq;
-    r->info.largest_seq = j.hs.max_seq;
+    run_info_from_index(j.hs, r->info.n_blocks, r->info.data_bytes, j.max_blk, r->info);
     r->id = e->next_run_id++;
     r->info.run_id = r->id;
     {
@@ -406,6 +397,12 @@ int32_t pgs_engine_open(const pgs_engine_config *cfg, pgs_engine **out)
     }
     for (auto &s : e.rd_streams) if (err == cudaSuccess) err = cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking);
     if (err == cudaSuccess) err = cudaStreamCreateWithFlags(&e.up_copy, cudaStreamNonBlocking);
+    if (err == cudaSuccess) {
+        uint64_t tab[256];
+        crc64_make_table(tab);
+        err = cudaMalloc(&e.d_crc, sizeof tab);
+        if (err == cudaSuccess) err = cudaMemcpy(e.d_crc, tab, sizeof tab, cudaMemcpyHostToDevice);
+    }
     if (err == cudaSuccess && (lookup_init_kernels(e.max_smem_optin) != PGS_OK || compact_init_kernels(e.max_smem_optin) != PGS_OK ||
                                index_init_kernels() != PGS_OK)) {
         delete h; // the failing call left its description in pgs_last_error()

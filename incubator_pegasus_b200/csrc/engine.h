@@ -7,6 +7,7 @@
 #include <memory>
 #include <mutex>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "../../include/pegasus_b200.h"
@@ -45,6 +46,7 @@ struct Engine {
     pgs_engine_config cfg{};
     int sm_count = 0;
     int max_smem_optin = 0;
+    uint64_t *d_crc = nullptr; // the crc64 table (2 KB) of partition-hash validation in reads and compactions
     std::atomic<uint64_t> launches{0};
     std::atomic<uint64_t> next_run_id{1};
     // reads of different host threads go to different streams (runs are complete before they become visible, so a reader
@@ -94,6 +96,39 @@ int32_t cuda_fail(cudaError_t e, const char *what);
         cudaError_t _e = (expr);                                                                   \
         if (_e != cudaSuccess) return ::pgs::cuda_fail(_e, #expr);                                 \
     } while (0)
+
+// the device scratch and events of one launch.  They are released when the owner goes out of scope, after the launch's
+// final synchronise or on an error return; buffers go back with cudaFreeAsync on the launch's stream.
+struct LaunchScratch {
+    cudaStream_t st;
+    std::vector<void *> bufs;
+    std::vector<cudaEvent_t> events;
+    explicit LaunchScratch(cudaStream_t s) : st(s) {}
+    LaunchScratch(const LaunchScratch &) = delete;
+    LaunchScratch &operator=(const LaunchScratch &) = delete;
+    ~LaunchScratch()
+    {
+        for (void *p : bufs) cudaFreeAsync(p, st);
+        for (cudaEvent_t ev : events) cudaEventDestroy(ev);
+    }
+    template <class T> cudaError_t alloc(T *&p, size_t bytes)
+    {
+        cudaError_t e = cudaMallocAsync((void **)&p, bytes, st);
+        if (e == cudaSuccess) bufs.push_back((void *)p);
+        return e;
+    }
+    template <class T> cudaError_t upload(T *&p, const std::remove_const_t<T> *src, size_t n) // a device copy of n host elements
+    {
+        cudaError_t e = alloc(p, sizeof(T) * n);
+        return e == cudaSuccess ? cudaMemcpyAsync((void *)p, src, sizeof(T) * n, cudaMemcpyHostToDevice, st) : e;
+    }
+    cudaError_t event(cudaEvent_t &ev)
+    {
+        cudaError_t e = cudaEventCreate(&ev);
+        if (e == cudaSuccess) events.push_back(ev);
+        return e;
+    }
+};
 
 // scans an uploaded / freshly merged run's blocks on the device and fills the index + info
 

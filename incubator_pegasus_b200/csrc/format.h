@@ -37,6 +37,20 @@ PGS_HD uint32_t varint_len(uint32_t v) { return v < 128 ? 1 : v < 16384 ? 2 : v 
 PGS_HD uint32_t user_data_offset(uint32_t version) { return version == 1 ? 12u : 4u; }
 PGS_HD bool ts_expired(uint32_t now, uint32_t ts) { return ts > 0 && ts <= now; }
 
+// crc64 table (host): reflected CRC-64, table driven; polynomial bits from utils/crc.cpp:289-295
+inline void crc64_make_table(uint64_t tab[256])
+{
+    const int bits[] = {63, 61, 59, 58, 56, 55, 52, 49, 48, 47, 46, 44, 41, 37, 36, 34,
+                        32, 31, 28, 26, 23, 22, 19, 16, 13, 12, 10, 9,  6,  4,  3,  0};
+    uint64_t poly = 0;
+    for (int b : bits) poly |= 1ull << (63 - b);
+    for (uint32_t i = 0; i < 256; i++) {
+        uint64_t c = i;
+        for (int r = 0; r < 8; r++) c = (c >> 1) ^ ((c & 1) ? poly : 0);
+        tab[i] = c;
+    }
+}
+
 // binary ops table handed to the compaction kernel (pgs_compaction_ops_parse):
 //   u32 n_ops
 //   per op : u8 op_type(0 update_ttl,1 delete) u8 ttl_type u16 n_rules u32 ttl_value

@@ -135,4 +135,22 @@ inline bool index_layout(const uint32_t *nrec, const uint32_t *lastlen, uint32_t
     return true;
 }
 
+// host, after the second pass: the run's pgs_run_info from the index statistics, the block count, the 16-aligned end of its
+// blocks and its largest block (level and run id are the caller's)
+inline void run_info_from_index(const IndexStats &st, uint32_t n_blocks, uint64_t data_bytes, uint32_t max_blk, pgs_run_info &info)
+{
+    info.n_blocks = n_blocks;
+    info.data_bytes = data_bytes;
+    info.n_records = st.n_records;
+    info.n_tombstones = st.n_tomb;
+    info.raw_key_bytes = st.raw_key;
+    info.raw_value_bytes = st.raw_val;
+    info.max_ukey_len = st.max_ukey;
+    info.max_value_len = st.max_vlen;
+    info.max_block_size = max_blk;
+    info.max_block_records = st.max_blk_rec;
+    info.smallest_seq = st.min_seq;
+    info.largest_seq = st.max_seq;
+}
+
 } // namespace pgs

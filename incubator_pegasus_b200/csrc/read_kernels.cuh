@@ -15,6 +15,11 @@
 //               step on different requests; entries are read straight from HBM, records are copied to the output arena.
 //   (reverse scans keep the block-staging kernel k_scan of lookup.cu.)
 #pragma once
+#include <algorithm>
+#include <cstring>
+#include <string>
+#include <vector>
+
 #include "group.cuh"
 
 namespace pgs {
@@ -525,6 +530,97 @@ __global__ void __launch_bounds__(kReadThreads) k_scan_fwd(const __grid_constant
         }
         g.sync();
     }
+}
+
+// ---- launch planning (host side; shared with the CPU simulation driver under tools/simt) -------------------------------------
+// user-key capacity of a read launch's key rows: the longest user key of its runs, at least 8 bytes, a multiple of 8
+inline uint32_t read_key_slot(uint32_t max_ukey) { return std::max(8u, (max_ukey + 7) & ~7u); }
+
+// the requests of a scan batch as the kernels read them: fixed-size records + their byte strings back to back in one blob
+struct ScanBatch {
+    std::vector<ScanReqDev> reqs;
+    std::string blob;          // + 16 bytes of slack
+    bool need_crc = false;     // a request validates partition hashes
+    bool any_reverse = false;  // a request iterates backwards (k_scan)
+};
+inline ScanBatch flatten_scan_requests(const pgs_scan_request *reqs, uint32_t n)
+{
+    ScanBatch b;
+    b.reqs.resize(n);
+    auto put = [&](const pgs_blob &x, uint32_t &off, uint32_t &len) {
+        off = (uint32_t)b.blob.size();
+        len = x.len;
+        if (x.len) b.blob.append((const char *)x.data, x.len);
+    };
+    for (uint32_t i = 0; i < n; i++) {
+        const pgs_scan_request &q = reqs[i];
+        ScanReqDev &d = b.reqs[i];
+        memset(&d, 0, sizeof d);
+        put(q.start, d.start_off, d.start_len);
+        put(q.stop, d.stop_off, d.stop_len);
+        put(q.hash_filter, d.hf_off, d.hf_len);
+        put(q.sort_filter, d.sf_off, d.sf_len);
+        d.start_inclusive = q.start_inclusive; d.stop_inclusive = q.stop_inclusive; d.reverse = q.reverse;
+        d.no_value = q.no_value; d.key_mode = q.key_mode; d.return_expire_ts = q.return_expire_ts;
+        d.count_only = q.count_only; d.validate_hash = q.validate_hash; d.prefix_same_as_start = q.prefix_same_as_start;
+        d.has_upper = q.reserved[0]; // iterate_upper_bound (internal flag used by sortkey_count)
+        d.hash_filter_type = q.hash_filter_type; d.sort_filter_type = q.sort_filter_type;
+        d.max_count = q.max_count; d.max_iter_count = q.max_iter_count; d.max_iter_size = q.max_iter_size;
+        d.pidx = q.pidx; d.partition_version = q.partition_version;
+        b.need_crc |= q.validate_hash != 0;
+        b.any_reverse |= q.reverse != 0;
+    }
+    b.blob.append(16, '\0');
+    return b;
+}
+
+// a multi-partition launch: rr.n = the most runs of one partition slot, and every entry of rr.runs is a valid dummy run for
+// the groups that have no request (packed[begin[s] .. begin[s + 1]) are the runs of slot s)
+inline void multi_read_runs(const std::vector<RunDev> &packed, const std::vector<uint32_t> &begin, ReadRuns &rr)
+{
+    rr.n = 0;
+    for (size_t s = 0; s + 1 < begin.size(); s++) rr.n = std::max(rr.n, begin[s + 1] - begin[s]);
+    for (uint32_t i = 0; i < kMaxReadRuns; i++) rr.runs[i] = packed.empty() ? RunDev{} : packed[0];
+}
+
+// shared memory of a k_get / k_scan_fwd launch: G lanes per group, KS / KSW the key row's bytes / 32-bit words, group_smem
+// one group's cursor states and key rows, dyn the launch's dynamic shared memory
+struct ReadGeometry {
+    uint32_t G, KS, KSW, group_smem, dyn;
+    template <class Params> void apply(Params &P) const { P.KS = KS; P.KSW = KSW; P.group_smem = group_smem; }
+};
+inline ReadGeometry get_geometry(uint32_t KS)
+{
+    ReadGeometry g;
+    g.G = 8;
+    g.KS = KS;
+    g.KSW = (KS + 8) / 4 + 1;
+    g.group_smem = (uint32_t)((sizeof(CurState) + 2 * g.KSW * 4 + 15) & ~(size_t)15);
+    g.dyn = kMaxReadRuns * (uint32_t)sizeof(RunDev) + (kReadThreads / g.G) * g.group_smem;
+    return g;
+}
+// n_runs = the most runs one request reads; force_G overrides the lanes per group (tests)
+inline ReadGeometry scan_fwd_geometry(uint32_t n_runs, uint32_t KS, uint32_t force_G = 0)
+{
+    ReadGeometry g;
+    g.G = force_G ? force_G : n_runs <= 8 ? 8 : n_runs <= 16 ? 16 : 32;
+    g.KS = KS;
+    g.KSW = (KS + 8) / 4 + 1;
+    g.group_smem = (uint32_t)((n_runs * (sizeof(CurState) + g.KSW * 4) + 3 * g.KSW * 4 + 15) & ~(size_t)15);
+    g.dyn = 2048 + kMaxReadRuns * (uint32_t)sizeof(RunDev) + (kReadThreads / g.G) * g.group_smem;
+    return g;
+}
+
+typedef void (*scan_fwd_kernel_t)(const ScanParams);
+constexpr uint32_t kScanFwdGs[] = {8, 16, 32};
+// a template only so that the kernels are instantiated where it is first called, which keeps their order in the binary
+template <class = void>
+inline scan_fwd_kernel_t scan_fwd_kernel(uint32_t G, bool multi)
+{
+    const scan_fwd_kernel_t k[3][2] = {{k_scan_fwd<8, false>, k_scan_fwd<8, true>},
+                                       {k_scan_fwd<16, false>, k_scan_fwd<16, true>},
+                                       {k_scan_fwd<32, false>, k_scan_fwd<32, true>}};
+    return k[G == 8 ? 0 : G == 16 ? 1 : 2][multi ? 1 : 0];
 }
 
 } // namespace pgs

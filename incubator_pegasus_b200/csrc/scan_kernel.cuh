@@ -773,21 +773,37 @@ __global__ void __launch_bounds__(kScanThreads, 4) k_scan(const __grid_constant_
     }
 }
 
-// Host side: the dynamic shared memory of a k_scan launch over n_runs runs (largest block: max_blk bytes, max_rec records)
-// for a batch of n_req requests.  Every chunk stages at least one block of every run that still has blocks, so a launch
-// needs room for one largest block of each run, plus scan_carve's padding; max_dyn is what the device leaves for dynamic shared memory.  Returns the
-// launch's dynamic size and sets *pool to the staging pool inside it, or returns 0 when one block of every run does not fit.
+// Host side (shared with the CPU simulation driver under tools/simt).
+// the largest block of a launch's runs, in bytes and in records
+struct ScanBlockBound {
+    uint32_t max_blk = 0, max_rec = 0;
+    void add(const pgs_run_info &i) { max_blk = std::max(max_blk, i.max_block_size); max_rec = std::max(max_rec, i.max_block_records); }
+};
+
+// what the device leaves k_scan for dynamic shared memory, given its opt-in limit and the kernel's static shared memory
+inline uint64_t scan_max_dyn(uint64_t max_smem_optin, uint64_t static_smem) { return max_smem_optin - static_smem - 256; }
+
+// the smallest staging pool a launch accepts: every chunk stages at least one block of every run that still has blocks, so
+// the pool holds one largest block of each run, plus scan_carve's padding
+inline uint64_t scan_min_pool(uint32_t n_runs, uint32_t KS, uint32_t max_blk, uint32_t max_rec)
+{
+    const uint64_t one = (((uint64_t)max_blk + 15) & ~15ull) + 32 + (uint64_t)max_rec * (KS + kScanRecExtra);
+    return one * (n_runs ? n_runs : 1) + 64 + scan_carve_slack(KS);
+}
+
+// the dynamic shared memory of a k_scan launch over n_runs runs (largest block: max_blk bytes, max_rec records) for a batch
+// of n_req requests; max_dyn is what the device leaves for dynamic shared memory.  Returns the launch's dynamic size and sets
+// *pool to the staging pool inside it, or returns 0 when the smallest pool (scan_min_pool) does not fit.
 inline uint64_t scan_dyn_bytes(uint32_t n_runs, uint32_t KS, uint32_t max_blk, uint32_t max_rec, uint32_t n_req, uint64_t max_dyn,
                                uint32_t *pool)
 {
     const uint64_t fixed_dyn = (4 + (uint64_t)n_runs) * ((KS + 8 + 15) & ~15u); // + kScanWarps * warp_scratch, which is 0
-    const uint64_t runs = n_runs ? n_runs : 1;
-    const uint64_t one = (((uint64_t)max_blk + 15) & ~15ull) + 32 + (uint64_t)max_rec * (KS + kScanRecExtra);
-    uint64_t want = one * runs + scan_carve_slack(KS) + 4096;
+    const uint64_t min_pool = scan_min_pool(n_runs, KS, max_blk, max_rec);
+    uint64_t want = min_pool - 64 + 4096;
     if (want < 48 * 1024) want = 48 * 1024;
     if (n_req == 1 && want < 160 * 1024) want = 160 * 1024;
     uint64_t dyn = fixed_dyn + want < max_dyn ? fixed_dyn + want : max_dyn;
-    if (dyn < fixed_dyn + one * runs + 64 + scan_carve_slack(KS)) return 0;
+    if (dyn < fixed_dyn + min_pool) return 0;
     dyn &= ~127ull;
     *pool = (uint32_t)(dyn - fixed_dyn);
     return dyn;
