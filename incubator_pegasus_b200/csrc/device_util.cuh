@@ -177,6 +177,29 @@ PGS_DEV int cmp_bytes4(const uint8_t *a, uint32_t la, const uint8_t *b, uint32_t
     }
     return la < lb ? -1 : (la > lb ? 1 : 0);
 }
+// does v match a NON-EMPTY pattern: anywhere in it, as its prefix or as its postfix (match_type: MATCH_* of format.h; any other
+// type never matches).  What an empty pattern means is the caller's rule.
+PGS_DEV bool pattern_match(uint32_t match_type, const uint8_t *pat, uint32_t pl, const uint8_t *v, uint32_t vl)
+{
+    if (vl < pl) return false;
+    if (match_type == MATCH_PREFIX) {
+        for (uint32_t i = 0; i < pl; i++) if (v[i] != pat[i]) return false;
+        return true;
+    }
+    if (match_type == MATCH_POSTFIX) {
+        const uint8_t *s = v + vl - pl;
+        for (uint32_t i = 0; i < pl; i++) if (s[i] != pat[i]) return false;
+        return true;
+    }
+    if (match_type == MATCH_ANYWHERE) {
+        for (uint32_t s = 0; s + pl <= vl; s++) {
+            uint32_t i = 0;
+            while (i < pl && v[s + i] == pat[i]) i++;
+            if (i == pl) return true;
+        }
+    }
+    return false;
+}
 PGS_DEV uint64_t bswap64(uint64_t x)
 {
     uint32_t lo = (uint32_t)x, hi = (uint32_t)(x >> 32);
@@ -305,38 +328,6 @@ PGS_DEV uint32_t block_excl_scan(uint32_t v, uint32_t *scratch, uint32_t *total)
 PGS_DEV void warp_copy_bytes(uint8_t *dst, const uint8_t *src, uint32_t n, uint32_t lane)
 {
     for (uint32_t i = lane; i < n; i += 32) dst[i] = src[i];
-}
-// shared -> global copy of n bytes, arbitrary alignment on both sides.  The body is written with
-// 16-byte stores aligned on the destination; source words are re-aligned with funnel shifts.
-PGS_DEV void warp_copy_s2g(uint8_t *dst, const uint8_t *src, uint32_t n, uint32_t lane)
-{
-    uint32_t head = (uint32_t)((16 - ((uintptr_t)dst & 15)) & 15);
-    if (head > n) head = n;
-    if (lane < head) dst[lane] = src[lane];
-    dst += head;
-    src += head;
-    n -= head;
-    uint32_t chunks = n >> 4;
-    uint32_t sh = (uint32_t)((uintptr_t)src & 3) * 8;
-    const uint32_t *sw = (const uint32_t *)((uintptr_t)src & ~(uintptr_t)3);
-    for (uint32_t c = lane; c < chunks; c += 32) {
-        const uint32_t *w = sw + c * 4;
-        uint32_t w0 = w[0], w1 = w[1], w2 = w[2], w3 = w[3];
-        uint4 o;
-        if (sh == 0) {
-            o = make_uint4(w0, w1, w2, w3);
-        } else {
-            uint32_t w4 = w[4];
-            o.x = __funnelshift_r(w0, w1, sh);
-            o.y = __funnelshift_r(w1, w2, sh);
-            o.z = __funnelshift_r(w2, w3, sh);
-            o.w = __funnelshift_r(w3, w4, sh);
-        }
-        *reinterpret_cast<uint4 *>(dst + c * 16) = o;
-    }
-    uint32_t done = chunks << 4;
-    uint32_t tail = n - done;
-    if (lane < tail) dst[done + lane] = src[done + lane];
 }
 
 } // namespace pgs

@@ -33,9 +33,37 @@ PGS_HD uint32_t be32(const uint8_t *p)
     return ((uint32_t)p[0] << 24) | ((uint32_t)p[1] << 16) | ((uint32_t)p[2] << 8) | p[3];
 }
 PGS_HD uint16_t be16(const uint8_t *p) { return (uint16_t)((p[0] << 8) | p[1]); }
+PGS_HD uint32_t le32(const uint8_t *p) { return p[0] | (p[1] << 8) | (p[2] << 16) | ((uint32_t)p[3] << 24); }
+PGS_HD uint32_t le16(const uint8_t *p) { return p[0] | (p[1] << 8); }
 PGS_HD uint32_t varint_len(uint32_t v) { return v < 128 ? 1 : v < 16384 ? 2 : v < 2097152 ? 3 : v < 268435456 ? 4 : 5; }
 PGS_HD uint32_t user_data_offset(uint32_t version) { return version == 1 ? 12u : 4u; }
 PGS_HD bool ts_expired(uint32_t now, uint32_t ts) { return ts > 0 && ts <= now; }
+
+// the hash key and sort key of a raw key.  A hash-key length that runs past the key is clamped to it (the reference CHECKs),
+// so a malformed key is never read outside its buffer; a key shorter than two bytes has neither.
+struct KeyParts {
+    const uint8_t *hk, *sk;
+    uint32_t hkl, skl;
+};
+PGS_HD KeyParts split_key(const uint8_t *key, uint32_t len)
+{
+    uint32_t hkl = len >= 2 ? be16(key) : 0u;
+    if (hkl + 2 > len) hkl = len >= 2 ? len - 2 : 0u;
+    return {key + 2, key + 2 + hkl, hkl, len >= 2 ? len - 2 - hkl : 0u};
+}
+
+// pegasus_key_hash (pegasus_key_schema.h:150-165): crc64 of the hash key, or of the sort key when the hash key is empty.
+// `table` = the crc64 table of crc64_make_table (uint64_t on the host, unsigned long long copies on the device).
+template <class T>
+PGS_HD uint64_t pegasus_key_hash(const T *table, const uint8_t *key, uint32_t len)
+{
+    const KeyParts k = split_key(key, len);
+    const uint8_t *p = k.hkl ? k.hk : k.sk;
+    const uint32_t n = k.hkl ? k.hkl : k.skl;
+    uint64_t c = ~0ull;
+    for (uint32_t i = 0; i < n; i++) c = table[(uint8_t)(c ^ p[i])] ^ (c >> 8);
+    return ~c;
+}
 
 // crc64 table (host): reflected CRC-64, table driven; polynomial bits from utils/crc.cpp:289-295
 inline void crc64_make_table(uint64_t tab[256])

@@ -189,10 +189,9 @@ static int32_t scan_launch(Partition &part, const std::vector<std::shared_ptr<Ru
     PGS_CUDA(cudaSetDevice(e->device));
     cudaStream_t st = e->read_stream();
     const ScanBatch B = flatten_scan_requests(reqs, n);
-    if (resume_stride < P.KS) resume_stride = 0; // caller gave no room: resume keys are not reported
+    if (!scan_output_strides(P, arena_stride, kv_stride, resume_stride)) resume_stride = 0; // caller gave no room for resume keys
     P.n = n; P.now = now; P.data_version = part.data_version;
     P.use_tma = (e->cfg.flags & PGS_ENGINE_NO_TMA) ? 0 : 1;
-    P.kv_stride = kv_stride; P.arena_stride = (arena_stride + 15) & ~15ull; P.resume_stride = resume_stride ? resume_stride : P.KS;
     if (multi ? multi->packed.empty() : P.rr.n == 0) { // empty DB: every iterator is invalid from the start
         memset(results, 0, sizeof(pgs_scan_result) * n);
         if (arena_base) for (uint32_t i = 0; i <= n; i++) arena_base[i] = 0;
@@ -241,7 +240,6 @@ static int32_t scan_launch(Partition &part, const std::vector<std::shared_ptr<Ru
         // ---- reverse scans (and forward ones with long keys): the block-staging kernel ---------------------------------
         cudaFuncAttributes attr;
         PGS_CUDA(cudaFuncGetAttributes(&attr, k_scan));
-        P.warp_scratch = 0;
         ScanBlockBound bb;
         for (auto &r : runs) bb.add(r->info);
         const uint64_t dyn = scan_dyn_bytes((uint32_t)runs.size(), P.KS, bb.max_blk, bb.max_rec, n,

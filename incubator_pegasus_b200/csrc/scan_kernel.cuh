@@ -9,36 +9,6 @@
 
 namespace pgs {
 
-PGS_DEV uint32_t ld32le(const uint8_t *p) { return p[0] | (p[1] << 8) | (p[2] << 16) | ((uint32_t)p[3] << 24); }
-
-// warp-cooperative 33-ary search over the block index: every round the 32 lanes probe 32 pivots at once, so the
-// chain of dependent global loads is ~log33(nb) long instead of log2(nb).  upper=false: first block whose last key
-// >= key; upper=true: first block whose last key > key.  All lanes return the same value.
-PGS_DEV uint32_t warp_index_bound(const RunDev &r, const uint8_t *key, uint32_t klen, uint32_t lane, bool upper)
-{
-    uint32_t lo = 0, hi = r.nb;
-    while (hi - lo > 32) {
-        uint32_t span = hi - lo;
-        uint32_t piv = lo + (uint32_t)(((unsigned long long)span * (lane + 1)) / 33);
-        uint32_t o = r.ikey_off[piv], l = r.ikey_off[piv + 1] - o;
-        int c = cmp_bytes4(r.ikeys + o, l, key, klen);
-        bool before = upper ? c <= 0 : c < 0; // pivot block lies strictly before the answer
-        uint32_t m = __ballot_sync(kFull, before);
-        uint32_t cnt = __popc(m); // monotone: lanes 0..cnt-1 are true
-        uint32_t nlo = cnt == 0 ? lo : __shfl_sync(kFull, piv, cnt - 1) + 1;
-        uint32_t nhi = cnt == 32 ? hi : __shfl_sync(kFull, piv, cnt & 31);
-        lo = nlo;
-        hi = nhi;
-    }
-    bool before = false;
-    if (lo + lane < hi) {
-        uint32_t o = r.ikey_off[lo + lane], l = r.ikey_off[lo + lane + 1] - o;
-        int c = cmp_bytes4(r.ikeys + o, l, key, klen);
-        before = upper ? c <= 0 : c < 0;
-    }
-    return lo + __popc(__ballot_sync(kFull, before));
-}
-
 // ------------------------------------------------------------------------------------------------
 // k_scan (reverse scans)
 // ------------------------------------------------------------------------------------------------
@@ -61,7 +31,7 @@ struct ScanShared {
     // carried loop state
     uint32_t count, iter_count, expire_count, filter_count, n_out;
     unsigned long long size, arena_used;
-    uint32_t complete, iter_valid, lookahead, resume_len, first_chunk;
+    uint32_t complete, iter_valid, lookahead, resume_len;
     uint32_t P, F; // per chunk
     uint32_t cand_len[kMaxReadRuns];
     uint32_t grec0[kMaxReadRuns]; // index of the slice's first record inside its run
@@ -121,13 +91,14 @@ __global__ void __launch_bounds__(kScanThreads, 4) k_scan(const __grid_constant_
     PGS_SMEM_DYN(dyn);
     PGS_SMEM_STATIC(ScanShared S);
     const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const Grp<32> wg; // the warp as one lane group (index search, value copies)
     const uint32_t KS = P.KS, NR = P.rr.n;
     // bounds of the current chunk, zero padded slots: lo = exclusive/inclusive lower, hi = upper
     const uint32_t slot = (KS + 8 + 15) & ~15u; // keeps `pool` (the TMA destination) 16-byte aligned
     uint8_t *klo = dyn, *khi = dyn + slot, *kpre = dyn + 2 * slot;
     uint8_t *kend = dyn + 3 * slot;  // the range end (first KS+8 bytes: no stored key is longer than KS)
     uint8_t *cand = dyn + 4 * slot;  // one slot per run: its candidate for the chunk's far bound
-    uint8_t *pool = dyn + (4 + NR) * slot + kScanWarps * P.warp_scratch;
+    uint8_t *pool = dyn + (4 + NR) * slot;
 
     if (tid == 0) { mbar_init((uint64_t *)&S.mbar, 1); mbar_fence_init(); }
     __syncthreads();
@@ -138,7 +109,6 @@ __global__ void __launch_bounds__(kScanThreads, 4) k_scan(const __grid_constant_
     for (uint32_t rq = blockIdx.x; rq < P.n; rq += gridDim.x) {
         const ScanReqDev &Q = P.reqs[rq];
         const uint8_t *start = P.blob + Q.start_off, *stop = P.blob + Q.stop_off;
-        const uint8_t *hf = P.blob + Q.hf_off, *sf = P.blob + Q.sf_off;
         const bool rev = Q.reverse != 0;
         // the range end in iteration direction ("stop" forward, "start" reverse) and its inclusiveness
         const uint8_t *endk = rev ? start : stop;
@@ -156,7 +126,7 @@ __global__ void __launch_bounds__(kScanThreads, 4) k_scan(const __grid_constant_
         if (tid == 0) {
             S.count = S.iter_count = S.expire_count = S.filter_count = S.n_out = 0;
             S.size = 0; S.arena_used = 0;
-            S.complete = 0; S.iter_valid = 0; S.lookahead = 0; S.resume_len = 0; S.done = 0; S.error = 0; S.first_chunk = 1;
+            S.complete = 0; S.iter_valid = 0; S.lookahead = 0; S.resume_len = 0; S.done = 0; S.error = 0;
         }
         if (P.crc_table && Q.validate_hash)
             for (uint32_t i = tid; i < 256; i += kScanThreads) S.crc[i] = P.crc_table[i];
@@ -167,12 +137,12 @@ __global__ void __launch_bounds__(kScanThreads, 4) k_scan(const __grid_constant_
             const uint32_t j = task >> 1;
             const RunDev &r = P.rr.runs[j];
             if (task & 1) {
-                uint32_t we = warp_index_bound(r, endk, endl, lane, false);
+                uint32_t we = grp_index_bound(wg, true, r, endk, endl, false);
                 if (lane == 0) S.want_end[j] = we;
             } else {
                 const uint8_t *sk = rev ? stop : start;
                 uint32_t sl = rev ? Q.stop_len : Q.start_len;
-                uint32_t b = warp_index_bound(r, sk, sl, lane, false);
+                uint32_t b = grp_index_bound(wg, true, r, sk, sl, false);
                 if (rev && b >= r.nb) b = r.nb ? r.nb - 1 : 0;
                 if (lane == 0) S.cur[j] = b;
             }
@@ -392,7 +362,7 @@ __global__ void __launch_bounds__(kScanThreads, 4) k_scan(const __grid_constant_
                     const uint32_t size = S.tb_size[t], i = r - S.tb_rec[t], cnt = S.tb_nrec[t];
                     uint32_t err = 0, nr = 0;
                     if (size < 8) err = PGS_CORRUPTION;
-                    if (!err) { nr = ld32le(base + size - 4); if (nr == 0 || (unsigned long long)nr * 4 + 4 > size) err = PGS_CORRUPTION; }
+                    if (!err) { nr = le32(base + size - 4); if (nr == 0 || (unsigned long long)nr * 4 + 4 > size) err = PGS_CORRUPTION; }
                     const uint32_t limit = err ? 0 : size - 4 - 4 * nr;
                     const uint32_t p = err ? 0 : P.rr.runs[j].rec_off[S.grec0[j] + (r - S.rec_base[j])];
                     if (!err && (p >= limit || (i == 0 && p != 0))) err = PGS_CORRUPTION;
@@ -567,12 +537,13 @@ __global__ void __launch_bounds__(kScanThreads, 4) k_scan(const __grid_constant_
             __syncthreads();
             // prefix bound: visible records outside the seek prefix end the iterator
             // per visible record: in-prefix, in-range, state, sizes
-            //   A2 <- 1 if state==normal (count prefix), A3 <- output bytes if normal (size prefix)
+            //   A2 <- 1 if state==normal (count prefix), A3 <- output bytes if normal (size prefix), rank (free once the
+            //   visible list stands) <- the output key's offset in the user key (the output key runs to the key's end)
+            const uint32_t hdr = user_data_offset(P.data_version);
             for (uint32_t v = tid; v < nvis; v += kScanThreads) {
                 uint32_t r = A.vis[v];
                 const uint8_t *key = A.arena + (size_t)r * KS;
                 uint32_t kl = A.klen[r];
-                uint8_t st;
                 bool in_prefix = true;
                 if (pre_len) {
                     in_prefix = kl >= pre_len;
@@ -581,37 +552,12 @@ __global__ void __launch_bounds__(kScanThreads, 4) k_scan(const __grid_constant_
                 int c = cmp_bytes(key, kl, kend, endl); // reads at most min(kl, endl) <= KS bytes of the staged range end
                 bool in_range = rev ? (c > 0 || (c == 0 && end_incl)) : (c < 0 || (c == 0 && end_incl));
                 if (Q.has_upper && !rev) in_prefix = in_prefix && c < 0; // iterate_upper_bound (sortkey_count)
-                const uint8_t *val = A.in + A.voff[r];
-                uint32_t vl = A.vlen[r];
-                uint32_t ets = vl >= 4 ? be32(val) : 0;
-                uint32_t hkl = kl >= 2 ? be16(key) : 0;
-                if (hkl + 2 > kl) hkl = kl >= 2 ? kl - 2 : 0;
-                const uint8_t *hk = key + 2, *sk = key + 2 + hkl;
-                uint32_t skl = kl >= 2 ? kl - 2 - hkl : 0;
-                if (ts_expired(P.now, ets)) st = RS_EXPIRED;
-                else {
-                    st = RS_NORMAL;
-                    if (Q.validate_hash) { // validate_key_value_for_scan: :2397-2404
-                        bool bad = Q.partition_version < 0 || Q.pidx > Q.partition_version;
-                        if (!bad && kl >= 2) {
-                            unsigned long long hcrc = ~0ull;
-                            const uint8_t *hp = hkl ? hk : sk;
-                            uint32_t hn = hkl ? hkl : skl;
-                            for (uint32_t i = 0; i < hn; i++) hcrc = S.crc[(uint8_t)(hcrc ^ hp[i])] ^ (hcrc >> 8);
-                            hcrc = ~hcrc;
-                            bad = (long long)(hcrc & (unsigned long long)(long long)Q.partition_version) != (long long)Q.pidx;
-                        }
-                        if (bad) st = RS_HASH_INVALID;
-                    }
-                    if (st == RS_NORMAL && Q.hash_filter_type != PGS_FT_NO_FILTER && !dev_validate_filter(Q.hash_filter_type, hf, Q.hf_len, hk, hkl)) st = RS_FILTERED;
-                    if (st == RS_NORMAL && Q.sort_filter_type != PGS_FT_NO_FILTER && !dev_validate_filter(Q.sort_filter_type, sf, Q.sf_len, sk, skl)) st = RS_FILTERED;
-                }
-                uint32_t hdr = user_data_offset(P.data_version);
-                uint32_t out_k = Q.key_mode == 1 ? skl : kl;
-                uint32_t out_v = Q.no_value ? 0 : (vl >= hdr ? vl - hdr : 0);
-                A.state[v] = st | (in_prefix ? 0x10 : 0) | (in_range ? 0x20 : 0);
-                A.A2[v] = st == RS_NORMAL ? 1u : 0u;
-                A.A3[v] = st == RS_NORMAL ? out_k + out_v : 0u;
+                const uint32_t vl = A.vlen[r];
+                const ScanRecord o = scan_record(Q, P.blob, S.crc, P.now, hdr, key, kl, vl, vl >= 4 ? be32(A.in + A.voff[r]) : 0u);
+                A.state[v] = o.st | (in_prefix ? 0x10 : 0) | (in_range ? 0x20 : 0);
+                A.A2[v] = o.st == RS_NORMAL ? 1u : 0u;
+                A.A3[v] = o.st == RS_NORMAL ? o.klen + o.vlen : 0u;
+                A.rank[v] = (uint16_t)o.koff;
             }
             __syncthreads();
             SPT(8);
@@ -620,7 +566,7 @@ __global__ void __launch_bounds__(kScanThreads, 4) k_scan(const __grid_constant_
             for (uint32_t v = tid; v <= nvis; v += kScanThreads) A.A2[v] = A.A1[v];
             __syncthreads();
             scan_chunked(nvis, A.A1, S.scan, [&](uint32_t v) -> uint32_t { return A.A3[v]; });
-            // A1 = size prefix, A2 = count prefix
+            // A1 = size prefix, A2 = count prefix, A3 = output bytes
             // ---- the reference loop, evaluated for all positions at once ---------------------------------------------
             if (tid == 0) { S.P = nvis; S.F = nvis; S.n_vis = nvis; }
             __syncthreads();
@@ -639,19 +585,16 @@ __global__ void __launch_bounds__(kScanThreads, 4) k_scan(const __grid_constant_
             const uint32_t nproc = min(Pp, Ff); // processed positions [0, nproc)
             // ---- emit ------------------------------------------------------------------------------------------------------
             if (!S.lookahead && nproc > 0 && !Q.count_only) {
-                uint32_t hdr = user_data_offset(P.data_version);
                 for (uint32_t v = warp; v < nproc; v += kScanWarps) {
                     if ((A.state[v] & 0xF) != RS_NORMAL) continue;
                     uint32_t r = A.vis[v], kl = A.klen[r], vl = A.vlen[r];
                     const uint8_t *key = A.arena + (size_t)r * KS;
-                    uint32_t koff = 0, klen_out = kl;
-                    if (Q.key_mode == 1) { uint32_t hkl = kl >= 2 ? be16(key) : 0; if (hkl + 2 > kl) hkl = kl >= 2 ? kl - 2 : 0; koff = 2 + hkl; klen_out = kl >= 2 ? kl - koff : 0; }
-                    uint32_t vlen_out = Q.no_value ? 0 : (vl >= hdr ? vl - hdr : 0);
+                    const uint32_t koff = A.rank[v], klen_out = kl > koff ? kl - koff : 0u, vlen_out = A.A3[v] - klen_out;
                     uint32_t slot = S.n_out + (A.A2[v]);
                     unsigned long long aoff = S.arena_used + A.A1[v];
                     if (slot >= P.kv_stride || aoff + klen_out + vlen_out > P.arena_stride) { if (lane == 0) atomicMax(&S.error, (uint32_t)PGS_ABORTED); continue; }
                     warp_copy_bytes(arena + aoff, key + koff, klen_out, lane);
-                    if (vlen_out) warp_copy_s2g(arena + aoff + klen_out, A.in + A.voff[r] + hdr, vlen_out, lane);
+                    if (vlen_out) grp_copy(wg, arena + aoff + klen_out, A.in + A.voff[r] + hdr, vlen_out);
                     if (lane == 0) {
                         pgs_kv kv;
                         kv.key_off = (uint32_t)aoff; kv.key_len = klen_out;
@@ -666,6 +609,7 @@ __global__ void __launch_bounds__(kScanThreads, 4) k_scan(const __grid_constant_
             // ---- advance the loop state -----------------------------------------------------------------------------------------
             if (tid == 0) {
                 uint32_t nvis_ = S.n_vis;
+                uint32_t stand = 0xFFFFFFFFu; // the loop ended by its limits with the iterator on visible record `stand`
                 if (!S.lookahead) {
                     uint32_t exp = 0, fil = 0;
                     for (uint32_t v = 0; v < nproc; v++) { uint8_t s = A.state[v] & 0xF; exp += s == RS_EXPIRED; fil += s == RS_FILTERED; }
@@ -682,12 +626,8 @@ __global__ void __launch_bounds__(kScanThreads, 4) k_scan(const __grid_constant_
                         hit_end = cmp_bytes(A.arena + (size_t)r * KS, A.klen[r], kend, endl) == 0;
                     }
                     if (hit_end) { S.complete = 1; S.iter_valid = 1; S.done = 1; }
-                    else if (Pp <= Ff && Pp < nvis_) { // limits ended the loop while the iterator stands on vis[Pp]
-                        uint32_t r = A.vis[Pp];
-                        bool valid = (A.state[Pp] & 0x10) != 0;
-                        S.iter_valid = valid; S.done = 1;
-                        if (valid) { S.resume_len = A.klen[r]; for (uint32_t i = 0; i < A.klen[r] && i < P.resume_stride; i++) P.resume[(size_t)rq * P.resume_stride + i] = A.arena[(size_t)r * KS + i]; }
-                    } else if (Ff < nvis_) { // reached a record outside the prefix (iterator invalid) or past the end (complete)
+                    else if (Pp <= Ff && Pp < nvis_) stand = Pp; // limits ended the loop while the iterator stands on vis[Pp]
+                    else if (Ff < nvis_) { // reached a record outside the prefix (iterator invalid) or past the end (complete)
                         uint8_t s = A.state[Ff];
                         if (!(s & 0x10)) { S.iter_valid = 0; S.done = 1; }
                         else { S.complete = 1; S.iter_valid = 1; S.done = 1; }
@@ -696,18 +636,18 @@ __global__ void __launch_bounds__(kScanThreads, 4) k_scan(const __grid_constant_
                         bool ok = (S.count < Q.max_count) && (S.iter_count < Q.max_iter_count) && (Q.max_iter_size == 0 || S.size < Q.max_iter_size);
                         if (!ok) S.lookahead = 1; // need to know whether the iterator is still valid
                     }
-                } else if (nvis_ > 0) { // look-ahead: the iterator stands on the first visible record
-                    uint32_t r = A.vis[0];
-                    bool valid = (A.state[0] & 0x10) != 0;
+                } else if (nvis_ > 0) stand = 0; // look-ahead: the iterator stands on the first visible record
+                if (stand != 0xFFFFFFFFu) {
+                    const uint32_t r = A.vis[stand];
+                    const bool valid = (A.state[stand] & 0x10) != 0;
                     S.iter_valid = valid; S.done = 1;
-                    if (valid) { S.resume_len = A.klen[r]; for (uint32_t i = 0; i < A.klen[r] && i < P.resume_stride; i++) P.resume[(size_t)rq * P.resume_stride + i] = A.arena[(size_t)r * KS + i]; }
+                    if (valid) { S.resume_len = A.klen[r]; put_resume_key(P, rq, A.arena + (size_t)r * KS, A.klen[r], 0, 1); }
                 }
                 if (!S.done) { // move every run's cursor past the consumed key range
                     bool any_more = false;
                     for (uint32_t j = 0; j < NR; j++) any_more |= S.more[j] != 0;
                     if (!any_more) { S.done = 1; S.iter_valid = 0; }
                 }
-                S.first_chunk = 0;
             }
             __syncthreads();
             SPT(11);
@@ -724,7 +664,7 @@ __global__ void __launch_bounds__(kScanThreads, 4) k_scan(const __grid_constant_
                     const RunDev &r = P.rr.runs[j];
                     uint32_t b;
                     if (rev) { // blocks after b hold only keys > bound; b itself may hold keys <= bound
-                        b = warp_index_bound(r, khi, S.hi_len, lane, false);
+                        b = grp_index_bound(wg, true, r, khi, S.hi_len, false);
                         if (b >= r.nb) b = r.nb ? r.nb - 1 : 0xFFFFFFFFu;
                         if (!r.nb) b = 0xFFFFFFFFu;
                     } else {
@@ -751,23 +691,9 @@ __global__ void __launch_bounds__(kScanThreads, 4) k_scan(const __grid_constant_
             }
         }
         // ---- result -----------------------------------------------------------------------------------------------------------------
-        if (tid == 0) {
-            pgs_scan_result res;
-            memset(&res, 0, sizeof res);
-            res.status = S.error ? (int32_t)S.error : PGS_OK;
-            res.n_kvs = S.n_out;
-            res.count = S.count;
-            res.iter_count = S.iter_count;
-            res.expire_count = S.expire_count;
-            res.filter_count = S.filter_count;
-            res.size = S.size;
-            res.complete = (uint8_t)S.complete;
-            res.iter_valid = (uint8_t)S.iter_valid;
-            res.resume_len = S.iter_valid ? S.resume_len : 0;
-            res.arena_used = S.arena_used;
-            P.results[rq] = res;
-            if (S.error) atomicMax(P.error, S.error);
-        }
+        if (tid == 0)
+            put_scan_result(P, rq, S.error, S.n_out, S.count, S.iter_count, S.expire_count, S.filter_count, S.size, S.complete != 0,
+                            S.iter_valid != 0, S.resume_len, S.arena_used);
         __syncthreads();
         SPT(12);
     }
@@ -797,7 +723,7 @@ inline uint64_t scan_min_pool(uint32_t n_runs, uint32_t KS, uint32_t max_blk, ui
 inline uint64_t scan_dyn_bytes(uint32_t n_runs, uint32_t KS, uint32_t max_blk, uint32_t max_rec, uint32_t n_req, uint64_t max_dyn,
                                uint32_t *pool)
 {
-    const uint64_t fixed_dyn = (4 + (uint64_t)n_runs) * ((KS + 8 + 15) & ~15u); // + kScanWarps * warp_scratch, which is 0
+    const uint64_t fixed_dyn = (4 + (uint64_t)n_runs) * ((KS + 8 + 15) & ~15u);
     const uint64_t min_pool = scan_min_pool(n_runs, KS, max_blk, max_rec);
     uint64_t want = min_pool - 64 + 4096;
     if (want < 48 * 1024) want = 48 * 1024;

@@ -61,10 +61,7 @@ std::string make_next(std::string k) // pegasus_key_schema.h:65-98
 uint64_t key_hash(std::string_view key) // pegasus_key_schema.h:150-165
 {
     if (key.size() < 2) return 0;
-    size_t l = be16((const uint8_t *)key.data());
-    if (l > key.size() - 2) l = key.size() - 2; // a malformed key never reads past its buffer (the reference CHECKs; the device filter clamps alike)
-    if (l > 0) return crc64((const uint8_t *)key.data() + 2, l, 0);
-    return crc64((const uint8_t *)key.data() + 2, key.size() - 2, 0);
+    return pegasus_key_hash(crc64_table(), (const uint8_t *)key.data(), (uint32_t)key.size());
 }
 
 // ---- run builder ----------------------------------------------------------------------------

@@ -212,6 +212,19 @@ def scan_list(hks):
     return reqs
 
 
+def filter_list(full):
+    """the record rules over a whole-range request `full`: every hash- and sort-key filter type, an empty pattern, and
+    validate_hash with a stale partition index, an invalid partition version and a valid one"""
+    reqs = []
+    for ft in (1, 2, 3):
+        reqs += [dict(full, hft=ft, hpat=b"h1"), dict(full, sft=ft, spat=b"1", max_count=50), dict(full, hft=ft, hpat=b"", sft=ft, spat=b"00")]
+    reqs += [dict(full, validate_hash=1, pidx=5, partition_version=3),          # stale partition index: every record kHashInvalid
+             dict(full, validate_hash=1, pidx=0, partition_version=-1),
+             dict(full, validate_hash=1, pidx=2, partition_version=7, max_count=40),
+             dict(full, key_mode=1, no_value=1, return_expire_ts=1), dict(full, count_only=1), dict(full, return_expire_ts=1, max_count=60)]
+    return reqs
+
+
 def mirror(q):
     """the same request iterated the other way (prefix_same_as_start and has_upper then have no effect)"""
     return dict(q, reverse=not q.get("reverse"))

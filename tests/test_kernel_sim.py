@@ -11,6 +11,7 @@ import numpy as np
 import pytest
 
 from incubator_pegasus_b200 import synth
+from scan_model import make_db
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 SIM_DIR = os.path.join(ROOT, "tools", "simt")
@@ -152,6 +153,11 @@ OPS_JSON = (
     '{"type":"FRT_TTL_RANGE","params":"{\\"start_ttl\\":0,\\"stop_ttl\\":50000}"}]}]}'
 )
 
+OPS_ANYWHERE_JSON = (
+    '{"ops":[{"type":"COT_DELETE","params":"","rules":[{"type":"FRT_SORTKEY_PATTERN","params":'
+    '"{\\"pattern\\":\\"01\\",\\"match_type\\":\\"SMT_MATCH_ANYWHERE\\"}"}]}]}'
+)
+
 
 @pytest.mark.parametrize("bottommost", [True, False])
 def test_sim_l0_to_l1(pgs, oracle, sim, bottommost):
@@ -248,3 +254,14 @@ def test_sim_long_keys_widen_the_groups(pgs, oracle, sim):
             seq += 1
         runs.append(pgs.Records.from_list([items[k] for k in sorted(items)]))
     check(pgs, oracle, sim, runs, bottommost=True, lanes=0, seg_weight=64 * 1024)
+
+
+def test_sim_anywhere_rule_and_empty_hash_keys(pgs, oracle, sim):
+    """a delete rule whose pattern matches inside the sort key ("01" of s0001, s0010..s0019, never at its start), and
+    validate_hash over records with an empty hash key, whose sort key is hashed instead"""
+    rng = np.random.default_rng(21)
+    runs, _ = make_db(pgs, rng, 3, [b"", b"h1", b"a01b", b"h22"], 60)
+    x = check(pgs, oracle, sim, runs, bottommost=True, ops_json=OPS_ANYWHERE_JSON, seg_weight=16 * 1024)
+    assert x["stats"][7] > 0
+    x = check(pgs, oracle, sim, runs, bottommost=True, validate_hash=True, pidx=1, partition_version=3, seg_weight=16 * 1024)
+    assert x["stats"][8] > 0

@@ -11,7 +11,7 @@ import pytest
 from get_model import (check_results, compacted_run, flat_keys, key_slot, model_get, model_stats, query_keys, sweep_items, sweep_keys,
                        uploaded_run)
 from incubator_pegasus_b200 import synth
-from scan_model import answer, diff, make_db, mirror, model_scan, next_key, raw_key, scan_list, scan_requests, visible
+from scan_model import answer, diff, filter_list, make_db, mirror, model_scan, next_key, raw_key, scan_list, scan_requests, visible
 from test_kernel_sim import sim, sim_compact  # noqa: F401  (fixture + helper)
 
 NOW = synth.NOW
@@ -137,7 +137,9 @@ def test_sim_scan_forward(pgs, sim, n_runs, lanes):
     runs, items = make_db(pgs, rng, n_runs, SCAN_HKS, 30)
     vis, best = visible(items)
     args, keep = run_args(pgs, runs, block_size=512, ri=4)
-    reqs = scan_list(SCAN_HKS)
+    full = dict(start=b"", stop=b"\xff" * 4, start_inclusive=True, stop_inclusive=True, key_mode=0, max_count=1000, max_iter_count=1000,
+                max_iter_size=0)
+    reqs = scan_list(SCAN_HKS) + filter_list(full)
     check_scans(vis, reqs, do_scans(pgs, sim, args, reqs, lanes))
 
 
@@ -160,6 +162,7 @@ def test_sim_scan_reverse_and_mixed(pgs, sim, n_runs, pool):
             for ti in (True, False):
                 fwd += [dict(full, start=k + b"\x00", start_inclusive=si, stop_inclusive=ti),
                         dict(full, stop=k + b"\x00", start_inclusive=si, stop_inclusive=ti)]
+    fwd += filter_list(full)
     rev = [mirror(q) for q in fwd]
     p = 0 if pool == "product" else 1
     check_scans(vis, rev, do_scans(pgs, sim, args, rev, pool=p))

@@ -9,7 +9,7 @@ import numpy as np
 import pytest
 
 from incubator_pegasus_b200 import synth
-from scan_model import answer, diff, mirror, model_scan, next_key, raw_key, scan_list, scan_requests, value, visible
+from scan_model import answer, diff, filter_list, mirror, model_scan, next_key, raw_key, scan_list, scan_requests, value, visible
 
 pytestmark = pytest.mark.gpu
 NOW = synth.NOW
@@ -114,12 +114,7 @@ def request_list(vis):
     reqs += [dict(full, start=last, stop=first),                                 # empty: start > stop
              dict(full, start=b"", stop=b"\x00"), dict(full, start=b"", stop=b"", stop_inclusive=False),  # before every key
              dict(full, start=last + b"\x00", stop=b"\xff" * 6), dict(full, start=b"\xff" * 5)]          # after every key
-    for ft in (1, 2, 3):
-        reqs += [dict(full, hft=ft, hpat=b"h1"), dict(full, sft=ft, spat=b"1", max_count=50), dict(full, hft=ft, hpat=b"", sft=ft, spat=b"00")]
-    reqs += [dict(full, validate_hash=1, pidx=5, partition_version=3),          # stale partition index: every record kHashInvalid
-             dict(full, validate_hash=1, pidx=0, partition_version=-1),
-             dict(full, validate_hash=1, pidx=2, partition_version=7, max_count=40),
-             dict(full, key_mode=1, no_value=1, return_expire_ts=1), dict(full, count_only=1), dict(full, return_expire_ts=1, max_count=60)]
+    reqs += filter_list(full)
     sizes = np.cumsum([len(k) + len(v) - 12 for k, v in vis])
     for i in range(1, len(vis) + 2):
         reqs.append(dict(full, max_iter_count=i))
