@@ -247,7 +247,68 @@ inline bool compact_geometry(MergeParams &P, const CompactTotals &T, uint32_t ma
     const uint64_t per_head = 15 + P.KS + 8 + 4;
     P.desc_cap = Nb + 1;
     P.head_cap = Nb * per_head + (2 * (Bb + Nb * per_head) / P.block_size + 2 * Q + 2) * (uint64_t)(P.KS + 8) + 64 * Q + 64;
+    P.out_bloom_lines = bloom_lines_for(T.bloom_entries);
     return true;
+}
+
+// the shared memory a compaction launch is planned for: the device's opt-in maximum per CTA less 1 KB (226 KB on an H100)
+inline uint32_t compact_smem_budget(uint32_t max_smem_optin) { return max_smem_optin - 1024; }
+
+// the filter and policy fields of P from the caller's filter parameters (nullptr: no filter); returns how many bytes of
+// fp->ops the launch needs in device memory at P.ops (0: no user ops)
+inline uint32_t compact_filter(MergeParams &P, const pgs_filter_params *fp)
+{
+    if (!fp) return 0;
+    P.enabled = fp->enabled;
+    P.validate_hash = fp->validate_hash;
+    P.default_ttl = fp->default_ttl;
+    P.pidx = fp->pidx;
+    P.partition_version = fp->partition_version;
+    if (!fp->ops || fp->ops_len < 4) return 0;
+    memcpy(&P.n_ops, fp->ops, 4);
+    return fp->ops_len;
+}
+
+// Every buffer of one launch: buf(pointer, elements, fill, out) allocates the elements and, unless fill is kNoFill, sets each
+// byte to fill before the first kernel.  The scratch (out = false) lives as long as the launch; the merged run's buffers
+// (out = true) are fields of `run` (the library's Run, or the simulator's host copy), which outlives it.  P points at all of them.
+constexpr int kNoFill = -1;
+template <class R, class F>
+inline void compact_buffers(MergeParams &P, const CompactGeometry &geo, const CompactTotals &T, R &run, F &&buf)
+{
+    const uint64_t Q = P.Q, nb = geo.blk_cap + 1;
+    buf(P.split_pos, (Q + 1) * P.k, 0xFF, false); // no boundary yet (seg_slice)
+    buf(P.split_ref, Q + 1, 0xFF, false);
+    buf(P.ticket, 64, 0, false);
+    buf(P.seg, Q, kNoFill, false);
+    buf(P.agg, Q, 0, false);                      // a walk that did not run produced nothing
+    buf(P.base, Q, kNoFill, false);
+    buf(P.desc, P.desc_cap, kNoFill, false);
+    buf(P.heads, P.head_cap + 64, kNoFill, false);
+    buf(run.d_data, geo.out_cap + 256, kNoFill, true);
+    buf(run.d_blk_off, nb, kNoFill, true);
+    buf(run.d_blk_size, nb, kNoFill, true);
+    buf(run.d_blk_rec, nb, kNoFill, true);
+    buf(run.d_ikey_off, nb, kNoFill, true);
+    buf(run.d_ikeys, geo.ikey_cap, kNoFill, true);
+    buf(run.d_rec_off, T.n_rec + 1, kNoFill, true);
+    buf(run.d_bloom, (uint64_t)P.out_bloom_lines * 16, 0, true); // k_emit only sets bits
+    run.bloom_lines = P.out_bloom_lines;
+    P.out_data = run.d_data;
+    P.out_blk_off = (unsigned long long *)run.d_blk_off;
+    P.out_blk_size = run.d_blk_size;
+    P.out_blk_rec = run.d_blk_rec;
+    P.out_ikey_off = run.d_ikey_off;
+    P.out_ikeys = run.d_ikeys;
+    P.out_rec_off = run.d_rec_off;
+    P.out_bloom = run.d_bloom;
+}
+// what P.stats holds before the first kernel: no error, no failing segment
+inline MergeStats merge_stats_init()
+{
+    MergeStats s{};
+    s.error_seg = 0xFFFFFFFFu;
+    return s;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -347,36 +408,16 @@ __global__ void __launch_bounds__(256) k_seg_bounds(const __grid_constant__ Merg
 
 __global__ void __launch_bounds__(1024) k_seg_layout(const __grid_constant__ MergeParams P)
 {
-    PGS_SMEM_STATIC(unsigned long long s_d[33]);
-    PGS_SMEM_STATIC(unsigned long long s_h[33]);
-    const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nw = blockDim.x >> 5;
-    const uint32_t per = (P.Q + blockDim.x - 1) / blockDim.x;
-    const uint32_t q0 = min(tid * per, P.Q), q1 = min(q0 + per, P.Q);
-    unsigned long long ld = 0, lh = 0;
-    for (uint32_t q = q0; q < q1; q++) { ld += P.seg[q].desc_off; lh += P.seg[q].head_off; }
-    unsigned long long id = ld, ih = lh;
-#pragma unroll
-    for (uint32_t d = 1; d < 32; d <<= 1) {
-        unsigned long long a = __shfl_up_sync(kFull, id, d), b = __shfl_up_sync(kFull, ih, d);
-        if (lane >= d) { id += a; ih += b; }
-    }
-    if (lane == 31) { s_d[warp] = id; s_h[warp] = ih; }
-    __syncthreads();
-    unsigned long long wd = lane < nw ? s_d[lane] : 0, wh = lane < nw ? s_h[lane] : 0, xd = wd, xh = wh;
-#pragma unroll
-    for (uint32_t d = 1; d < 32; d <<= 1) {
-        unsigned long long a = __shfl_up_sync(kFull, xd, d), b = __shfl_up_sync(kFull, xh, d);
-        if (lane >= d) { xd += a; xh += b; }
-    }
-    unsigned long long pd = __shfl_sync(kFull, xd - wd, (int)warp) + id - ld, ph = __shfl_sync(kFull, xh - wh, (int)warp) + ih - lh;
-    const unsigned long long td = __shfl_sync(kFull, xd, 31), th = __shfl_sync(kFull, xh, 31);
-    if (tid == 0 && (td > P.desc_cap || th > P.head_cap)) { atomicMax(&P.stats->error, (uint32_t)PGS_ABORTED); atomicMin(&P.stats->error_seg, 0u); }
+    uint32_t q0, q1;
+    unsigned long long pre[2], tot[2];
+    cta_excl_scan<2>(P.Q, [&](uint32_t q, unsigned long long (&v)[2]) { v[0] += P.seg[q].desc_off; v[1] += P.seg[q].head_off; }, q0, q1, pre, tot);
+    if (threadIdx.x == 0 && (tot[0] > P.desc_cap || tot[1] > P.head_cap)) { atomicMax(&P.stats->error, (uint32_t)PGS_ABORTED); atomicMin(&P.stats->error_seg, 0u); }
     for (uint32_t q = q0; q < q1; q++) {
         const unsigned long long a = P.seg[q].desc_off, b = P.seg[q].head_off;
-        P.seg[q].desc_off = pd;
-        P.seg[q].head_off = ph;
-        pd += a;
-        ph += b;
+        P.seg[q].desc_off = pre[0];
+        P.seg[q].head_off = pre[1];
+        pre[0] += a;
+        pre[1] += b;
     }
 }
 
@@ -866,7 +907,7 @@ __global__ void __launch_bounds__(kWalkThreads, 4) k_walk(const __grid_constant_
         for (uint32_t i = threadIdx.x; i < 256; i += blockDim.x) crc[i] = P.crc_table[i];
     for (uint32_t i = threadIdx.x; i < kMaxRuns; i += blockDim.x) runs[i] = P.runs[i < P.k ? i : 0];
     for (uint32_t i = threadIdx.x; i < sizeof(WalkCtaStats) / 4; i += blockDim.x) ((uint32_t *)cta)[i] = 0;
-    __syncthreads();
+    if (__syncthreads_or(P.stats->error != 0)) return; // the planner rejected the layout: the output is discarded
     uint8_t *gs = dyn + kWalkFixedSmem + (size_t)(warp * NGW + g.shift / G) * P.group_smem;
     CurState *cs = (CurState *)gs;
     uint32_t *rows = (uint32_t *)(gs + (size_t)P.k * sizeof(CurState));
@@ -910,38 +951,13 @@ __global__ void __launch_bounds__(kWalkThreads, 4) k_walk(const __grid_constant_
 // ------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(1024) k_seg_scan(const __grid_constant__ MergeParams P)
 {
-    PGS_SMEM_STATIC(unsigned long long s_w[4][33]);
-    const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nw = blockDim.x >> 5;
-    const uint32_t per = (P.Q + blockDim.x - 1) / blockDim.x;
-    const uint32_t q0 = min(tid * per, P.Q), q1 = min(q0 + per, P.Q);
-    unsigned long long loc[4] = {0, 0, 0, 0};
-    for (uint32_t q = q0; q < q1; q++) {
+    uint32_t q0, q1;
+    unsigned long long pre[4], tot[4];
+    cta_excl_scan<4>(P.Q, [&](uint32_t q, unsigned long long (&v)[4]) {
         const SegAgg a = P.agg[q];
-        loc[0] += a.out_bytes; loc[1] += a.n_blocks; loc[2] += a.n_entries; loc[3] += a.keyb;
-    }
-    unsigned long long inc[4], pre[4], tot[4];
-#pragma unroll
-    for (uint32_t x = 0; x < 4; x++) {
-        inc[x] = loc[x];
-#pragma unroll
-        for (uint32_t d = 1; d < 32; d <<= 1) {
-            unsigned long long o = __shfl_up_sync(kFull, inc[x], d);
-            if (lane >= d) inc[x] += o;
-        }
-        if (lane == 31) s_w[x][warp] = inc[x];
-    }
-    __syncthreads();
-#pragma unroll
-    for (uint32_t x = 0; x < 4; x++) {
-        unsigned long long w = lane < nw ? s_w[x][lane] : 0, ws = w;
-#pragma unroll
-        for (uint32_t d = 1; d < 32; d <<= 1) {
-            unsigned long long o = __shfl_up_sync(kFull, ws, d);
-            if (lane >= d) ws += o;
-        }
-        tot[x] = __shfl_sync(kFull, ws, 31);
-        pre[x] = __shfl_sync(kFull, ws - w, (int)warp) + inc[x] - loc[x];
-    }
+        v[0] += a.out_bytes; v[1] += a.n_blocks; v[2] += a.n_entries; v[3] += a.keyb;
+    }, q0, q1, pre, tot);
+    const uint32_t tid = threadIdx.x;
     for (uint32_t q = q0; q < q1; q++) {
         const SegAgg a = P.agg[q];
         SegBase b;
@@ -1072,6 +1088,7 @@ __global__ void __launch_bounds__(kEmitThreads, 5) k_emit(const __grid_constant_
 {
     PGS_SMEM_DYN(dyn);
     const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    if (__shfl_sync(kFull, P.stats->error, 0)) return; // the plan or the walk failed: the output is discarded
     const uint32_t RI = P.restart_interval, OB = P.emit_obuf;
     uint8_t *ws = dyn + (size_t)warp * P.emit_warp_smem;
     uint8_t *obuf = ws;                                          // OB + 32 bytes
@@ -1374,6 +1391,30 @@ inline walk_kernel_t walk_kernel(uint32_t G)
     case 8: return k_walk<8>;
     default: return k_walk<16>;
     }
+}
+
+// The six kernels of one compaction on stream st.  k_walk and k_emit loop over the segments: walk_ctas / emit_ctas = how many
+// of their CTAs the device runs at once.  mark(i) is called before k_plan (0), after k_seg_layout (1), after k_walk (2) and
+// after k_emit (3).  Returns the number of launches.
+template <class Mark>
+inline uint32_t compact_launch(const MergeParams &P, const CompactGeometry &geo, uint64_t walk_ctas, uint64_t emit_ctas, cudaStream_t st,
+                               Mark &&mark)
+{
+    const walk_kernel_t walk = walk_kernel(geo.G);
+    const uint32_t seg_per_cta = kWalkThreads / geo.G;
+    const uint32_t grid_w = (uint32_t)std::min<uint64_t>((P.Q + seg_per_cta - 1) / seg_per_cta, walk_ctas);
+    const uint32_t grid_e = (uint32_t)std::min<uint64_t>((P.Q + geo.emit_warps - 1) / geo.emit_warps, emit_ctas);
+    mark(0);
+    PGS_LAUNCH(k_plan, (P.total_blocks + 255ull) / 256, 256, 0, st, P);
+    PGS_LAUNCH(k_seg_bounds, (P.Q + 255ull) / 256, 256, 0, st, P);
+    PGS_LAUNCH(k_seg_layout, 1, 1024, 0, st, P);
+    mark(1);
+    PGS_LAUNCH(walk, grid_w, kWalkThreads, geo.walk_dyn, st, P);
+    mark(2);
+    PGS_LAUNCH(k_seg_scan, 1, 1024, 0, st, P);
+    PGS_LAUNCH(k_emit, grid_e, geo.emit_warps * 32, geo.emit_dyn, st, P);
+    mark(3);
+    return 6;
 }
 
 } // namespace pgs

@@ -322,6 +322,45 @@ PGS_DEV uint32_t block_excl_scan(uint32_t v, uint32_t *scratch, uint32_t *total)
     *total = scratch[32];
     return scratch[warp] + inc - v;
 }
+// exclusive scan of N u64 fields over n items in ONE CTA (blockDim.x <= 1024, a multiple of 32).  Thread t owns the contiguous
+// items [q0, q1) (returned); add(q, v) adds the fields of item q to v.  pre = the sums over the items before q0, tot = the sums
+// over all n items.
+template <uint32_t N, class Add>
+PGS_DEV void cta_excl_scan(uint32_t n, Add add, uint32_t &q0, uint32_t &q1, unsigned long long (&pre)[N], unsigned long long (&tot)[N])
+{
+    PGS_SMEM_STATIC(unsigned long long s_w[N][33]);
+    const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nw = blockDim.x >> 5;
+    const uint32_t per = (n + blockDim.x - 1) / blockDim.x;
+    q0 = min(tid * per, n);
+    q1 = min(q0 + per, n);
+    unsigned long long loc[N], inc[N];
+#pragma unroll
+    for (uint32_t x = 0; x < N; x++) loc[x] = 0;
+    for (uint32_t q = q0; q < q1; q++) add(q, loc);
+#pragma unroll
+    for (uint32_t x = 0; x < N; x++) {
+        inc[x] = loc[x];
+#pragma unroll
+        for (uint32_t d = 1; d < 32; d <<= 1) {
+            const unsigned long long o = __shfl_up_sync(kFull, inc[x], d);
+            if (lane >= d) inc[x] += o;
+        }
+        if (lane == 31) s_w[x][warp] = inc[x];
+    }
+    __syncthreads();
+#pragma unroll
+    for (uint32_t x = 0; x < N; x++) {
+        const unsigned long long w = lane < nw ? s_w[x][lane] : 0;
+        unsigned long long ws = w;
+#pragma unroll
+        for (uint32_t d = 1; d < 32; d <<= 1) {
+            const unsigned long long o = __shfl_up_sync(kFull, ws, d);
+            if (lane >= d) ws += o;
+        }
+        tot[x] = __shfl_sync(kFull, ws, 31);
+        pre[x] = __shfl_sync(kFull, ws - w, (int)warp) + inc[x] - loc[x];
+    }
+}
 
 // ---- warp copies ------------------------------------------------------------------------------------
 // byte-granular copy (any address space), all 32 lanes participate

@@ -41,17 +41,22 @@ constexpr uint64_t kSpareMin = 64ull << 20; // only buffers this large are worth
 constexpr size_t kSpareMax = 8;
 constexpr uint64_t kSpareMemDivisor = 8; // spare buffers hold at most 1/8 of the device memory (10 GB on an 80 GB H100)
 
-uint8_t *Engine::take_data(uint64_t need, uint64_t *cap)
+cudaError_t Engine::alloc_data(Run &r, uint64_t need)
 {
-    std::lock_guard<std::mutex> g(spare_mu);
-    int best = -1;
-    for (size_t i = 0; i < spares.size(); i++)
-        if (spares[i].cap >= need && spares[i].cap <= 2 * need + kSpareMin && (best < 0 || spares[i].cap < spares[best].cap)) best = (int)i;
-    if (best < 0) return nullptr;
-    uint8_t *p = spares[best].p;
-    *cap = spares[best].cap;
-    spares.erase(spares.begin() + best);
-    return p;
+    if (need >= kSpareMin) {
+        std::lock_guard<std::mutex> g(spare_mu);
+        int best = -1;
+        for (size_t i = 0; i < spares.size(); i++)
+            if (spares[i].cap >= need && spares[i].cap <= 2 * need + kSpareMin && (best < 0 || spares[i].cap < spares[best].cap)) best = (int)i;
+        if (best >= 0) {
+            r.d_data = spares[best].p;
+            r.data_cap = spares[best].cap;
+            spares.erase(spares.begin() + best);
+            return cudaSuccess;
+        }
+    }
+    r.data_cap = need;
+    return cudaMallocAsync(&r.d_data, need, stream);
 }
 void *Engine::take_pinned(size_t need, size_t *cap)
 {
@@ -92,28 +97,20 @@ void Engine::give_data(uint8_t *p, uint64_t cap)
     }
 }
 
+// stream-ordered pool: repeated flush / compaction cycles reuse the same HBM without driver calls
+Run::Run(Engine *e) : pool_stream(e->stream), eng(e) {}
 Run::~Run()
 {
-    if (pool_stream) { // stream-ordered pool: the bytes go back to the pool without a device sync
-        if (eng && d_data && data_cap >= kSpareMin && engine_alive(eng)) eng->give_data(d_data, data_cap);
-        else cudaFreeAsync(d_data, pool_stream);
-        cudaFreeAsync(d_blk_off, pool_stream);
-        cudaFreeAsync(d_blk_size, pool_stream);
-        cudaFreeAsync(d_blk_rec, pool_stream);
-        cudaFreeAsync(d_ikey_off, pool_stream);
-        cudaFreeAsync(d_ikeys, pool_stream);
-        cudaFreeAsync(d_rec_off, pool_stream);
-        cudaFreeAsync(d_bloom, pool_stream);
-        return;
-    }
-    cudaFree(d_data);
-    cudaFree(d_blk_off);
-    cudaFree(d_blk_size);
-    cudaFree(d_blk_rec);
-    cudaFree(d_ikey_off);
-    cudaFree(d_ikeys);
-    cudaFree(d_rec_off);
-    cudaFree(d_bloom);
+    // the bytes go back to the pool without a device sync
+    if (d_data && data_cap >= kSpareMin && engine_alive(eng)) eng->give_data(d_data, data_cap);
+    else cudaFreeAsync(d_data, pool_stream);
+    cudaFreeAsync(d_blk_off, pool_stream);
+    cudaFreeAsync(d_blk_size, pool_stream);
+    cudaFreeAsync(d_blk_rec, pool_stream);
+    cudaFreeAsync(d_ikey_off, pool_stream);
+    cudaFreeAsync(d_ikeys, pool_stream);
+    cudaFreeAsync(d_rec_off, pool_stream);
+    cudaFreeAsync(d_bloom, pool_stream);
 }
 Engine::~Engine()
 {
@@ -221,7 +218,7 @@ static int32_t upload_stage_a(Engine *e, int32_t level, const uint8_t *data, uin
         prev_end = blk_off[b] + blk_size[b];
         j.max_blk = std::max(j.max_blk, blk_size[b]);
     }
-    auto r = std::make_shared<Run>();
+    auto r = std::make_shared<Run>(e);
     j.r = r;
     j.eng = e;
     {
@@ -244,12 +241,8 @@ static int32_t upload_stage_a(Engine *e, int32_t level, const uint8_t *data, uin
     const uint64_t end = (prev_end + kBlockAlign - 1) / kBlockAlign * kBlockAlign;
     const uint64_t nbytes = data_bytes < end ? data_bytes : end;
     r->info.data_bytes = end;
-    r->data_cap = end + 256;
     cudaStream_t st = e->stream, cp = e->up_copy;
-    r->pool_stream = st; // stream-ordered pool: repeated flush / compaction cycles reuse the same HBM without driver calls
-    r->eng = e;
-    if (r->data_cap >= kSpareMin) { uint64_t cap = 0; r->d_data = e->take_data(r->data_cap, &cap); if (r->d_data) r->data_cap = cap; }
-    if (!r->d_data) PGS_CUDA(cudaMallocAsync(&r->d_data, r->data_cap, st));
+    PGS_CUDA(e->alloc_data(*r, end + 256));
     PGS_CUDA(cudaMallocAsync(&r->d_blk_off, sizeof(uint64_t) * (nb + 1), st));
     PGS_CUDA(cudaMallocAsync(&r->d_blk_size, sizeof(uint32_t) * nb, st));
     PGS_CUDA(cudaMallocAsync(&j.d_nrec, sizeof(uint32_t) * nb, st));

@@ -31,8 +31,9 @@ struct Run {
     uint32_t bloom_lines = 0;
     uint64_t n_bloom_entries = 0; // user keys + distinct hash-key prefixes that went into the filter (sizes a merged run's filter)
     uint64_t data_cap = 0;
-    cudaStream_t pool_stream = nullptr; // set when the buffers came from cudaMallocAsync on that stream
-    struct Engine *eng = nullptr;       // set with pool_stream: large data buffers go back to the engine's spare list
+    cudaStream_t pool_stream;  // the buffers come from cudaMallocAsync on the engine's stream
+    struct Engine *eng;        // large data buffers go back to the engine's spare list
+    explicit Run(struct Engine *e);
     RunDev dev() const
     {
         return RunDev{d_data, d_blk_off, d_blk_size, d_blk_rec, d_ikey_off, d_ikeys, d_rec_off, d_bloom, bloom_lines, info.n_blocks, info.max_ukey_len, 0};
@@ -67,7 +68,7 @@ struct Engine {
     std::mutex spare_mu;
     std::vector<Spare> spares;
     uint64_t spare_bytes_max = 0; // set at open from the device's memory size
-    uint8_t *take_data(uint64_t need, uint64_t *cap); // nullptr when nothing suitable is kept
+    cudaError_t alloc_data(Run &r, uint64_t need); // r.d_data / r.data_cap: a kept buffer when one fits, else a new one
     void give_data(uint8_t *p, uint64_t cap);
     // pinned host staging for the small arrays of an upload (block handles in, per-block counts out): with pageable memory a
     // cudaMemcpyAsync waits for everything queued before it on its stream, which stalls the upload pipeline between runs

@@ -9,6 +9,8 @@
 #include "../../incubator_pegasus_b200/csrc/read_kernels.cuh"
 #include "../../incubator_pegasus_b200/csrc/scan_kernel.cuh"
 
+#include <memory>
+#include <new>
 #include <string>
 #include <vector>
 
@@ -16,61 +18,65 @@ using namespace pgs;
 
 namespace {
 
+constexpr uint32_t kSimSmemOptin = 227 * 1024; // the opt-in shared memory per CTA of an H100
+
+// host buffers standing in for device memory: each one its own allocation of exactly the size the library allocates, so that
+// AddressSanitizer checks the kernels against the library's bounds
+using HostMem = std::vector<std::shared_ptr<void>>;
+template <class T>
+T *host_alloc(HostMem &mem, T *&p, uint64_t n, int fill)
+{
+    const size_t bytes = sizeof(T) * n;
+    void *b = ::operator new(bytes ? bytes : 1, std::align_val_t(64));
+    memset(b, fill, bytes);
+    mem.emplace_back(b, [](void *x) { ::operator delete(x, std::align_val_t(64)); });
+    return p = (T *)b;
+}
+
+// a run in host memory, with the buffer fields of the library's Run (engine.h)
 struct HostRun {
-    std::vector<uint8_t> data;
-    std::vector<uint64_t> blk_off;
-    std::vector<uint32_t> blk_size, blk_rec, ikey_off, rec_off;
-    std::vector<uint8_t> ikeys;
-    std::vector<uint32_t> bloom;
+    HostMem mem;
+    uint8_t *d_data = nullptr, *d_ikeys = nullptr;
+    uint64_t *d_blk_off = nullptr;
+    uint32_t *d_blk_size = nullptr, *d_blk_rec = nullptr, *d_ikey_off = nullptr, *d_rec_off = nullptr, *d_bloom = nullptr;
+    uint32_t bloom_lines = 0;
     uint64_t n_bloom_entries = 0;
     pgs_run_info info{};
     RunDev dev() const
     {
-        return RunDev{data.data(), blk_off.data(), blk_size.data(), blk_rec.data(), ikey_off.data(), ikeys.data(), rec_off.data(),
-                      bloom.data(), (uint32_t)(bloom.size() / 16), (uint32_t)blk_size.size(), info.max_ukey_len, 0};
+        return RunDev{d_data, d_blk_off, d_blk_size, d_blk_rec, d_ikey_off, d_ikeys, d_rec_off, d_bloom, bloom_lines, info.n_blocks, info.max_ukey_len, 0};
     }
 };
 
-uint32_t varint(const uint8_t *p, uint32_t &v)
-{
-    v = 0;
-    for (uint32_t i = 0; i < 5; i++) {
-        v |= (uint32_t)(p[i] & 127) << (7 * i);
-        if (!(p[i] & 128)) return i + 1;
-    }
-    return 0;
-}
-
 // the run's index and Bloom filter as pgs_run_upload builds them (engine.cu): the two passes of k_index_walk with the host
 // layout between them
-bool build_index(HostRun &r)
+bool build_index(HostRun &r, uint32_t nb)
 {
-    const uint32_t nb = (uint32_t)r.blk_size.size();
     std::vector<uint32_t> nrec(nb + 1), lastlen(nb + 1);
     IndexStats st{};
     st.min_seq = ~0ull;
     const uint32_t grid = (nb + kIdxWarps - 1) / kIdxWarps, smem = kIdxWarps * kIdxScratch;
     if (nb)
-        PGS_LAUNCH(k_index_walk<false>, grid, kIdxWarps * 32, smem, 0, (const uint8_t *)r.data.data(), (const uint64_t *)r.blk_off.data(),
-                   (const uint32_t *)r.blk_size.data(), nb, nrec.data(), lastlen.data(), (const uint32_t *)nullptr, (uint8_t *)nullptr,
+        PGS_LAUNCH(k_index_walk<false>, grid, kIdxWarps * 32, smem, 0, (const uint8_t *)r.d_data, (const uint64_t *)r.d_blk_off,
+                   (const uint32_t *)r.d_blk_size, nb, nrec.data(), lastlen.data(), (const uint32_t *)nullptr, (uint8_t *)nullptr,
                    (const uint32_t *)nullptr, (uint32_t *)nullptr, (uint32_t *)nullptr, 0u, &st, 0u);
     if (st.error) return false;
-    r.blk_rec.assign(nb + 1, 0);
-    r.ikey_off.assign(nb + 1, 0);
-    if (!index_layout(nrec.data(), lastlen.data(), nb, r.blk_rec.data(), r.ikey_off.data())) return false;
-    r.ikeys.assign(r.ikey_off[nb] + 16, 0); // the product's slack (engine.cu)
-    r.rec_off.assign(r.blk_rec[nb] + 1, 0);
+    host_alloc(r.mem, r.d_blk_rec, nb + 1, 0);
+    host_alloc(r.mem, r.d_ikey_off, nb + 1, 0);
+    if (!index_layout(nrec.data(), lastlen.data(), nb, r.d_blk_rec, r.d_ikey_off)) return false;
+    host_alloc(r.mem, r.d_ikeys, r.d_ikey_off[nb] + 16, 0); // the product's slack (engine.cu)
+    host_alloc(r.mem, r.d_rec_off, r.d_blk_rec[nb] + 1, 0);
     r.n_bloom_entries = st.n_records + st.n_prefix;
-    const uint32_t lines = bloom_lines_for(r.n_bloom_entries);
-    r.bloom.assign((size_t)lines * 16, 0);
+    r.bloom_lines = bloom_lines_for(r.n_bloom_entries);
+    host_alloc(r.mem, r.d_bloom, (uint64_t)r.bloom_lines * 16, 0);
     if (nb)
-        PGS_LAUNCH(k_index_walk<true>, grid, kIdxWarps * 32, smem, 0, (const uint8_t *)r.data.data(), (const uint64_t *)r.blk_off.data(),
-                   (const uint32_t *)r.blk_size.data(), nb, (uint32_t *)nullptr, (uint32_t *)nullptr, (const uint32_t *)r.ikey_off.data(),
-                   r.ikeys.data(), (const uint32_t *)r.blk_rec.data(), r.rec_off.data(), r.bloom.data(), lines, &st, 0u);
+        PGS_LAUNCH(k_index_walk<true>, grid, kIdxWarps * 32, smem, 0, (const uint8_t *)r.d_data, (const uint64_t *)r.d_blk_off,
+                   (const uint32_t *)r.d_blk_size, nb, (uint32_t *)nullptr, (uint32_t *)nullptr, (const uint32_t *)r.d_ikey_off,
+                   r.d_ikeys, (const uint32_t *)r.d_blk_rec, r.d_rec_off, r.d_bloom, r.bloom_lines, &st, 0u);
     if (st.error) return false;
     uint32_t max_blk = 0;
-    for (uint32_t b = 0; b < nb; b++) max_blk = std::max(max_blk, r.blk_size[b]);
-    run_info_from_index(st, nb, r.blk_off[nb], max_blk, r.info);
+    for (uint32_t b = 0; b < nb; b++) max_blk = std::max(max_blk, r.d_blk_size[b]);
+    run_info_from_index(st, nb, r.d_blk_off[nb], max_blk, r.info);
     return true;
 }
 
@@ -78,24 +84,18 @@ bool build_index(HostRun &r)
 // blocks as blk_off[nb], the index and the filter
 bool load_run(HostRun &r, const uint8_t *data, uint64_t data_bytes, const uint64_t *blk_off, const uint32_t *blk_size, uint32_t nb)
 {
-    r.data.assign(data, data + data_bytes);
-    r.data.resize(r.data.size() + 256, 0);
-    r.blk_off.assign(blk_off, blk_off + nb);
-    r.blk_size.assign(blk_size, blk_size + nb);
-    const uint64_t end = nb ? r.blk_off.back() + r.blk_size.back() : 0;
-    r.blk_off.push_back((end + 15) & ~15ull);
-    return build_index(r);
+    memcpy(host_alloc(r.mem, r.d_data, data_bytes + 256, 0), data, data_bytes);
+    memcpy(host_alloc(r.mem, r.d_blk_off, nb + 1, 0), blk_off, 8 * (size_t)nb);
+    memcpy(host_alloc(r.mem, r.d_blk_size, nb, 0), blk_size, 4 * (size_t)nb);
+    const uint64_t end = nb ? blk_off[nb - 1] + blk_size[nb - 1] : 0;
+    r.d_blk_off[nb] = (end + 15) & ~15ull;
+    return build_index(r, nb);
 }
 
 uint64_t crc_tab[256];
 
-struct Result {
-    std::vector<uint8_t> data;
-    std::vector<uint64_t> blk_off;
-    std::vector<uint32_t> blk_size, blk_rec, ikey_off, rec_off;
-    std::vector<uint8_t> ikeys;
-    std::vector<uint32_t> bloom;
-    uint32_t bloom_lines = 0;
+struct Merged { // the output of the last sim_compact call
+    HostRun run;
     MergeStats st{};
     uint32_t Q = 0;
 } g_res;
@@ -123,70 +123,30 @@ int32_t sim_compact(uint32_t k, const uint8_t **data, const uint64_t *data_bytes
     P.bottommost = bottommost ? 1 : 0;
     P.now = now;
     P.data_version = 1;
-    std::vector<uint8_t> ops;
-    if (fp) {
-        P.enabled = fp->enabled; P.validate_hash = fp->validate_hash; P.default_ttl = fp->default_ttl;
-        P.pidx = fp->pidx; P.partition_version = fp->partition_version;
-        if (fp->ops && fp->ops_len >= 4) { memcpy(&P.n_ops, fp->ops, 4); ops.assign(fp->ops, fp->ops + fp->ops_len); ops.resize(ops.size() + 16); P.ops = ops.data(); }
+    HostMem scratch;
+    if (const uint32_t n = compact_filter(P, fp)) {
+        uint8_t *ops;
+        memcpy(host_alloc(scratch, ops, n, 0), fp->ops, n);
+        P.ops = ops;
     }
-    CompactGeometry geo{};
-    if (group_lanes && group_lanes != 1 && group_lanes != 2 && group_lanes != 4 && group_lanes != 8 && group_lanes != 16) return PGS_INVALID_ARGUMENT;
-    // seg_weight: smaller segments, so that a small test crosses many segment boundaries
-    if (!compact_geometry(P, T, 227 * 1024, geo, group_lanes, seg_weight)) return PGS_NOT_SUPPORTED;
-    const uint64_t Q = P.Q;
-    std::vector<uint32_t> split_pos((Q + 1) * k, 0xFFFFFFFFu), split_ref(Q + 1, 0xFFFFFFFFu), ticket(64, 0);
-    std::vector<SegLayout> seg(Q);
-    std::vector<SegAgg> agg(Q);
-    std::vector<SegBase> base(Q);
-    std::vector<Desc> desc(P.desc_cap);
-    std::vector<uint8_t> heads(P.head_cap + 64, 0xEE);
-    MergeStats st{};
-    st.error_seg = 0xFFFFFFFFu;
-    Result &R = g_res;
-    R = Result{};
-    R.data.assign(geo.out_cap + 256, 0xDD);
-    R.blk_off.assign(geo.blk_cap + 1, 0);
-    R.blk_size.assign(geo.blk_cap + 1, 0);
-    R.blk_rec.assign(geo.blk_cap + 1, 0);
-    R.ikey_off.assign(geo.blk_cap + 1, 0);
-    R.ikeys.assign(geo.ikey_cap, 0);
-    R.rec_off.assign(T.n_rec + 1, 0);
-    R.bloom_lines = bloom_lines_for(T.bloom_entries);
-    R.bloom.assign((size_t)R.bloom_lines * 16, 0);
-    P.out_bloom = R.bloom.data();
-    P.out_bloom_lines = R.bloom_lines;
-    P.split_pos = split_pos.data(); P.split_ref = split_ref.data(); P.ticket = ticket.data();
-    P.seg = seg.data(); P.agg = agg.data(); P.base = base.data(); P.desc = desc.data(); P.heads = heads.data();
-    P.out_data = R.data.data(); P.out_blk_off = (unsigned long long *)R.blk_off.data(); P.out_blk_size = R.blk_size.data();
-    P.out_blk_rec = R.blk_rec.data(); P.out_ikey_off = R.ikey_off.data(); P.out_ikeys = R.ikeys.data(); P.out_rec_off = R.rec_off.data();
-    P.stats = &st;
     if (P.validate_hash) {
         if (crc_table) memcpy(crc_tab, crc_table, sizeof crc_tab); else crc64_make_table(crc_tab);
         P.crc_table = (const unsigned long long *)crc_tab;
     }
-    PGS_LAUNCH(k_plan, (T.total_blocks + 255) / 256, 256, 0, 0, P);
-    PGS_LAUNCH(k_seg_bounds, (P.Q + 255) / 256, 256, 0, 0, P);
-    PGS_LAUNCH(k_seg_layout, 1, 1024, 0, 0, P);
-    if (!st.error) PGS_LAUNCH(walk_kernel(geo.G), 2, kWalkThreads, geo.walk_dyn, 0, P);
-    if (getenv("PGS_SIM_DUMP")) {
-        for (uint32_t q = 0; q < P.Q; q++) {
-            const Desc *d = desc.data() + seg[q].desc_off;
-            const uint8_t *h = heads.data() + seg[q].head_off;
-            uint32_t hp = 0;
-            for (uint32_t e = 0; e < agg[q].n_entries; e++) {
-                uint32_t fl = d[e].loc >> 60, hl = (d[e].loc >> 44) & 0xffff;
-                fprintf(stderr, "seg %u e %u fl %u hl %u vlen %u aux %u", q, e, fl, hl, d[e].vlen, d[e].aux);
-                if (fl & 1) { fprintf(stderr, " prevkey ..%.*s", 6, h + hp + (d[e].aux > 6 ? d[e].aux - 6 : 0)); hp += d[e].aux; }
-                if (fl & 2) hp += 4;
-                fprintf(stderr, " head:");
-                for (uint32_t i = 0; i < hl && i < 70; i++) fprintf(stderr, "%02x", h[hp + i]);
-                fprintf(stderr, "\n");
-                hp += hl;
-            }
-        }
-    }
-    if (!st.error) PGS_LAUNCH(k_seg_scan, 1, 1024, 0, 0, P);
-    if (!st.error) PGS_LAUNCH(k_emit, 2, geo.emit_warps * 32, geo.emit_dyn, 0, P);
+    CompactGeometry geo{};
+    if (group_lanes && group_lanes != 1 && group_lanes != 2 && group_lanes != 4 && group_lanes != 8 && group_lanes != 16) return PGS_INVALID_ARGUMENT;
+    // seg_weight: smaller segments, so that a small test crosses many segment boundaries
+    if (!compact_geometry(P, T, compact_smem_budget(kSimSmemOptin), geo, group_lanes, seg_weight)) return PGS_NOT_SUPPORTED;
+    Merged &R = g_res;
+    R = Merged{};
+    compact_buffers(P, geo, T, R.run, [&](auto *&p, uint64_t n, int fill, bool out) {
+        host_alloc(out ? R.run.mem : scratch, p, n, fill == kNoFill ? 0xEE : fill); // poisoned until the kernels write it
+    });
+    MergeStats st = merge_stats_init();
+    P.stats = &st;
+    compact_launch(P, geo, 2, 2, nullptr, [](int) {});
+    pgs_compact_result res{};
+    R.run.n_bloom_entries = compact_result_stats(st, T.in_block_bytes, res, R.run.info);
     R.st = st;
     R.Q = P.Q;
     if (st.error) { fprintf(stderr, "sim_compact: status %u at segment %u of %u\n", st.error, st.error_seg, P.Q); return (int32_t)st.error; }
@@ -201,14 +161,15 @@ void sim_result_sizes(uint64_t *data_bytes, uint32_t *n_blocks, uint32_t *n_segm
 }
 void sim_result_copy(uint8_t *data, uint64_t *blk_off, uint32_t *blk_size, uint32_t *blk_rec, uint32_t *ikey_off, uint8_t *ikeys, uint32_t *rec_off)
 {
+    const HostRun &r = g_res.run;
     const uint32_t nb = (uint32_t)g_res.st.tot_blocks;
-    memcpy(data, g_res.data.data(), g_res.st.tot_bytes);
-    memcpy(blk_off, g_res.blk_off.data(), 8 * (size_t)(nb + 1));
-    memcpy(blk_size, g_res.blk_size.data(), 4 * (size_t)nb);
-    if (blk_rec) memcpy(blk_rec, g_res.blk_rec.data(), 4 * (size_t)(nb + 1));
-    if (ikey_off) memcpy(ikey_off, g_res.ikey_off.data(), 4 * (size_t)(nb + 1));
-    if (ikeys) memcpy(ikeys, g_res.ikeys.data(), g_res.st.tot_keyb);
-    if (rec_off) memcpy(rec_off, g_res.rec_off.data(), 4 * (size_t)g_res.st.tot_recs);
+    memcpy(data, r.d_data, g_res.st.tot_bytes);
+    memcpy(blk_off, r.d_blk_off, 8 * (size_t)(nb + 1));
+    memcpy(blk_size, r.d_blk_size, 4 * (size_t)nb);
+    if (blk_rec) memcpy(blk_rec, r.d_blk_rec, 4 * (size_t)(nb + 1));
+    if (ikey_off) memcpy(ikey_off, r.d_ikey_off, 4 * (size_t)(nb + 1));
+    if (ikeys) memcpy(ikeys, r.d_ikeys, g_res.st.tot_keyb);
+    if (rec_off) memcpy(rec_off, r.d_rec_off, 4 * (size_t)g_res.st.tot_recs);
 }
 // the counters of pgs_compact_result, in its order: in_records, out_records, in_bytes, out_bytes, dropped_shadowed,
 // dropped_tombstone, dropped_expired, dropped_user, dropped_stale, ttl_rewritten, + run info: tombstones, raw key, raw value,
@@ -227,24 +188,25 @@ void sim_result_stats(uint64_t *o)
 // 1 when the merged run's Bloom filter admits the byte string (a user key or a hash-key prefix)
 int32_t sim_result_bloom_check(const uint8_t *key, uint32_t len)
 {
-    return bloom_may_contain(g_res.bloom.data(), g_res.bloom_lines, bloom_hash_bytes(key, len)) ? 1 : 0;
+    return bloom_may_contain(g_res.run.d_bloom, g_res.run.bloom_lines, bloom_hash_bytes(key, len)) ? 1 : 0;
 }
 
-// the Bloom filter of the last sim_compact output (the one k_emit built): up to cap words; returns its number of lines
-uint32_t sim_result_bloom(uint32_t *out, uint64_t cap)
+// up to cap words of a run's Bloom filter; returns its number of lines
+static uint32_t copy_bloom(const HostRun &r, uint32_t *out, uint64_t cap)
 {
-    memcpy(out, g_res.bloom.data(), 4 * std::min<uint64_t>(cap, g_res.bloom.size()));
-    return g_res.bloom_lines;
+    memcpy(out, r.d_bloom, 4 * std::min<uint64_t>(cap, (uint64_t)r.bloom_lines * 16));
+    return r.bloom_lines;
 }
 
-// the Bloom filter the upload builds for one run (k_index_walk): up to cap words; returns its number of lines (0: corrupt run)
+// the Bloom filter of the last sim_compact output (the one k_emit built)
+uint32_t sim_result_bloom(uint32_t *out, uint64_t cap) { return copy_bloom(g_res.run, out, cap); }
+
+// the Bloom filter the upload builds for one run (k_index_walk); 0 lines: a corrupt run
 uint32_t sim_run_bloom(const uint8_t *data, uint64_t data_bytes, const uint64_t *blk_off, const uint32_t *blk_size, uint32_t n_blocks,
                        uint32_t *out, uint64_t cap)
 {
     HostRun r;
-    if (!load_run(r, data, data_bytes, blk_off, blk_size, n_blocks)) return 0;
-    memcpy(out, r.bloom.data(), 4 * std::min<uint64_t>(cap, r.bloom.size()));
-    return (uint32_t)(r.bloom.size() / 16);
+    return load_run(r, data, data_bytes, blk_off, blk_size, n_blocks) ? copy_bloom(r, out, cap) : 0;
 }
 
 static bool load_runs(uint32_t k, const uint8_t **data, const uint64_t *data_bytes, const uint64_t **blk_off, const uint32_t **blk_size,
@@ -272,11 +234,9 @@ int32_t sim_get(uint32_t k, const uint8_t **data, const uint64_t *data_bytes, co
     uint32_t mk = 0;
     if (!load_runs(k, data, data_bytes, blk_off, blk_size, n_blocks, runs, P.rr, mk)) return PGS_CORRUPTION;
     if (use_bloom & 4) { // the run of the last sim_compact call joins as the oldest run, with the index and filter k_emit wrote
-        const Result &R = g_res;
-        if (k >= kMaxReadRuns || !R.st.tot_blocks) return PGS_INVALID_ARGUMENT;
-        P.rr.runs[k] = RunDev{R.data.data(), R.blk_off.data(), R.blk_size.data(), R.blk_rec.data(), R.ikey_off.data(), R.ikeys.data(),
-                              R.rec_off.data(), R.bloom.data(), R.bloom_lines, (uint32_t)R.st.tot_blocks, (uint32_t)R.st.mx[SM_UKEY], 0};
-        mk = std::max(mk, (uint32_t)R.st.mx[SM_UKEY]);
+        if (k >= kMaxReadRuns || !g_res.st.tot_blocks) return PGS_INVALID_ARGUMENT;
+        P.rr.runs[k] = g_res.run.dev();
+        mk = std::max(mk, g_res.run.info.max_ukey_len);
         P.rr.n = ++k;
     }
     if (!(use_bloom & 1)) for (uint32_t i = 0; i < k; i++) { P.rr.runs[i].bloom = nullptr; P.rr.runs[i].bloom_lines = 0; }
@@ -329,7 +289,7 @@ int32_t sim_scan(uint32_t k, const uint8_t **data, const uint64_t *data_bytes, c
         ScanBlockBound bb;
         for (auto &r : runs) bb.add(r.info);
         P.use_tma = 0;
-        uint64_t dyn = scan_dyn_bytes(k, P.KS, bb.max_blk, bb.max_rec, n, scan_max_dyn(227 * 1024, sizeof(ScanShared)), &P.pool_bytes);
+        uint64_t dyn = scan_dyn_bytes(k, P.KS, bb.max_blk, bb.max_rec, n, scan_max_dyn(kSimSmemOptin, sizeof(ScanShared)), &P.pool_bytes);
         if (!dyn) return PGS_NOT_SUPPORTED;
         if (pool_bytes) {
             const uint32_t fixed_dyn = (uint32_t)dyn - P.pool_bytes;

@@ -181,6 +181,16 @@ struct simt_idx_ { uint32_t x, y = 0, z = 0; };
 #define gridDim (simt_idx_{simt::cta()->grid})
 
 inline void __syncthreads() { simt::wait_barrier(simt::cta()->cta_bar, simt::cta()->live); }
+inline int __syncthreads_or(int pred) // every thread deposits, all meet, all read, all meet again before a slot is reused
+{
+    simt::Cta *c = simt::cta();
+    c->xchg[simt::tid_()] = pred != 0;
+    __syncthreads();
+    int any = 0;
+    for (uint32_t t = 0; t < c->nthreads; t++) any |= c->fibers[t].done ? 0 : (int)c->xchg[t];
+    __syncthreads();
+    return any;
+}
 inline void __syncwarp(uint32_t mask = 0xffffffffu) { simt::sync_mask(mask); }
 inline void simt_named_bar(uint32_t id, uint32_t n) { simt::wait_barrier(simt::cta()->named_bars[id], n); }
 
@@ -293,6 +303,7 @@ struct uint4 { uint32_t x, y, z, w; } __attribute__((aligned(16)));
 inline uint2 make_uint2(uint32_t x, uint32_t y) { return uint2{x, y}; }
 inline uint4 make_uint4(uint32_t x, uint32_t y, uint32_t z, uint32_t w) { return uint4{x, y, z, w}; }
 
+typedef struct simt_stream_ *cudaStream_t; // launches run synchronously, in order
 #define PGS_SMEM_DYN(name) uint8_t *name = simt::cta()->dyn
 #define PGS_SMEM_STATIC(decl) static decl
 #define PGS_LAUNCH(kernel, grid, block, dyn, stream, ...) simt::launch(kernel, (uint32_t)(grid), (uint32_t)(block), (size_t)(dyn), __VA_ARGS__)
