@@ -84,10 +84,8 @@ typedef struct {
                                   overridden by Pegasus: pegasus_server_impl_init.cpp:666-848) */
     uint32_t restart_interval; /* 0 -> 16 (pegasus_server_impl_init.cpp:716-718)              */
     uint32_t ctas_per_sm;      /* unused since round 2 (the walker sizes its own grid); kept for ABI stability              */
-    uint32_t flags;            /* PGS_ENGINE_* below                                          */
+    uint32_t flags;            /* reserved and ignored; kept for ABI stability                                              */
 } pgs_engine_config;
-
-#define PGS_ENGINE_NO_TMA 1u /* debug: the reverse-scan kernel stages blocks with plain loads instead of cp.async.bulk */
 
 PGS_API int32_t pgs_engine_open(const pgs_engine_config *cfg, pgs_engine **out);
 PGS_API void pgs_engine_close(pgs_engine *e);

@@ -367,9 +367,8 @@ def parse_ops(json_text: str, data_version: int = 1) -> np.ndarray:
 
 
 class Engine:
-    def __init__(self, device: int = -1, ctas_per_sm: int = 0, flags: int = 0, block_size: int = 0,
-                 restart_interval: int = 0):
-        cfg = EngineConfig(device, block_size, restart_interval, ctas_per_sm, flags)
+    def __init__(self, device: int = -1, ctas_per_sm: int = 0, block_size: int = 0, restart_interval: int = 0):
+        cfg = EngineConfig(device, block_size, restart_interval, ctas_per_sm, 0)
         self.h = C.c_void_p()
         _check(lib().pgs_engine_open(C.byref(cfg), C.byref(self.h)), "engine_open")
 
@@ -414,8 +413,8 @@ class Engine:
 class Router:
     """One engine per visible GPU; replica (app_id, pidx) lives on GPU pidx % n (pgs_router_*, include/pegasus_b200.h §7)."""
 
-    def __init__(self, n_devices: int = 0, ctas_per_sm: int = 0, flags: int = 0, block_size: int = 0, restart_interval: int = 0):
-        cfg = EngineConfig(-1, block_size, restart_interval, ctas_per_sm, flags)
+    def __init__(self, n_devices: int = 0, ctas_per_sm: int = 0, block_size: int = 0, restart_interval: int = 0):
+        cfg = EngineConfig(-1, block_size, restart_interval, ctas_per_sm, 0)
         self.h = C.c_void_p()
         _check(lib().pgs_router_open(C.byref(cfg), n_devices, C.byref(self.h)), "router_open")
 

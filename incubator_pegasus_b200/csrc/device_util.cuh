@@ -35,11 +35,9 @@ PGS_DEV void tma_load_1d(void *smem_dst, const void *gmem_src, uint32_t bytes, u
 PGS_DEV void tma_store_1d(void *gmem_dst, const void *smem_src, uint32_t bytes) { memcpy(gmem_dst, smem_src, bytes); }
 PGS_DEV void tma_store_commit() {}
 PGS_DEV void tma_store_wait_read0() {}
-PGS_DEV void tma_store_wait_read1() {}
 PGS_DEV void tma_store_wait_all() {}
 PGS_DEV void fence_proxy_async() {}
 PGS_DEV void async_copy4(void *smem_dst, const void *gmem_src) { memcpy(smem_dst, gmem_src, 4); }
-PGS_DEV void async_copy8(void *smem_dst, const void *gmem_src) { memcpy(smem_dst, gmem_src, 8); }
 PGS_DEV void async_copy16(void *smem_dst, const void *gmem_src) { memcpy(smem_dst, gmem_src, 16); }
 PGS_DEV void async_copy_wait_upto(uint32_t) {}
 PGS_DEV void async_copy_commit() {}
@@ -90,7 +88,6 @@ PGS_DEV void tma_store_1d(void *gmem_dst, const void *smem_src, uint32_t bytes)
 PGS_DEV void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 // the source bytes of all but the newest N committed bulk groups have been read (their shared memory may be rewritten)
 PGS_DEV void tma_store_wait_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
-PGS_DEV void tma_store_wait_read1() { asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory"); }
 PGS_DEV void tma_store_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 // generic-proxy writes to shared memory become visible to the async proxy (TMA) that reads them next
 PGS_DEV void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
@@ -98,10 +95,6 @@ PGS_DEV void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;"
 PGS_DEV void async_copy4(void *smem_dst, const void *gmem_src)
 {
     asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(smem_u32(smem_dst)), "l"(gmem_src) : "memory");
-}
-PGS_DEV void async_copy8(void *smem_dst, const void *gmem_src)
-{
-    asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"(smem_u32(smem_dst)), "l"(gmem_src) : "memory");
 }
 // 16 bytes, both addresses 16-aligned, past L1 (streamed data)
 PGS_DEV void async_copy16(void *smem_dst, const void *gmem_src)
@@ -133,13 +126,6 @@ PGS_DEV uint32_t get_varint32(const uint8_t *p, uint32_t avail, uint32_t &v)
         if (!(b & 128u)) { v = r; return i + 1; }
     }
     return 0;
-}
-PGS_DEV uint32_t put_varint32(uint8_t *p, uint32_t v)
-{
-    uint32_t n = 0;
-    while (v >= 128) { p[n++] = (uint8_t)(v | 128); v >>= 7; }
-    p[n++] = (uint8_t)v;
-    return n;
 }
 
 // ---- byte-string compare -------------------------------------------------------------------------
@@ -242,17 +228,9 @@ PGS_DEV int cmp_slots_from(const uint8_t *a, uint32_t la, const uint8_t *b, uint
     *diff = words;
     return la < lb ? -1 : (la > lb ? 1 : 0);
 }
-// 8 bytes at an arbitrary shared-memory address (three aligned 32-bit loads + funnel shifts)
-PGS_DEV uint64_t lds_u64_unaligned(const uint8_t *p)
-{
-    const uint32_t *w = (const uint32_t *)((uintptr_t)p & ~(uintptr_t)3);
-    uint32_t sh = (uint32_t)((uintptr_t)p & 3) * 8;
-    uint32_t w0 = w[0], w1 = w[1], w2 = w[2];
-    uint32_t lo = __funnelshift_r(w0, w1, sh), hi = __funnelshift_r(w1, w2, sh);
-    return ((uint64_t)hi << 32) | lo;
-}
-// same, addressed as (4-byte aligned base, byte offset): plain pointer arithmetic, so the compiler keeps the
-// loads in the shared address space (a uintptr_t round trip turns them into generic loads)
+// 8 bytes at an arbitrary shared-memory address, addressed as (4-byte aligned base, byte offset): three aligned 32-bit loads +
+// funnel shifts.  Plain pointer arithmetic, so the compiler keeps the loads in the shared address space (a uintptr_t round trip
+// turns them into generic loads)
 PGS_DEV uint64_t lds_u64_at(const uint8_t *base4, uint32_t off)
 {
     const uint32_t *w = (const uint32_t *)base4 + (off >> 2);
@@ -275,22 +253,6 @@ PGS_DEV uint32_t parse_header8(uint64_t x, uint32_t &a, uint32_t &b, uint32_t &c
     if (!(b3 & 0x80u)) { c = (b2 & 0x7fu) | (b3 << 7); return 4; }
     if (!(b4 & 0x80u)) { c = (b2 & 0x7fu) | ((b3 & 0x7fu) << 7) | (b4 << 14); return 5; }
     return 0;
-}
-
-// longest common prefix of two zero-padded 8-aligned slots, capped at min(la, lb)
-PGS_DEV uint32_t lcp_slots(const uint8_t *a, uint32_t la, const uint8_t *b, uint32_t lb)
-{
-    uint32_t m = la < lb ? la : lb;
-    uint32_t words = (m + 7) >> 3;
-    const uint64_t *wa = (const uint64_t *)a, *wb = (const uint64_t *)b;
-    for (uint32_t i = 0; i < words; i++) {
-        uint64_t d = wa[i] ^ wb[i];
-        if (d) {
-            uint32_t n = i * 8 + ((__ffsll((long long)d) - 1) >> 3); // little-endian: lowest set byte
-            return n < m ? n : m;
-        }
-    }
-    return m;
 }
 
 // ---- scans -----------------------------------------------------------------------------------------

@@ -49,16 +49,6 @@ struct Grp<1> { // one thread = one group: every "collective" is the identity, n
     PGS_DEV static void sync() {}
 };
 
-// 8 bytes at an arbitrary address (any address space): two aligned 64-bit loads + shift
-PGS_DEV uint64_t ld_u64_any(const uint8_t *p)
-{
-    const uint64_t *w = (const uint64_t *)((uintptr_t)p & ~(uintptr_t)7);
-    const uint32_t sh = (uint32_t)((uintptr_t)p & 7) * 8;
-    const uint64_t a = w[0];
-    if (!sh) return a;
-    return (a >> sh) | (w[1] << (64 - sh));
-}
-
 // Compare two byte strings held in key rows (4-byte aligned shared memory, readable up to the next multiple of 4).
 // Returns <0, 0, >0; dpos = index of the first differing byte, or min(la, lb) when one is a prefix of the other.
 // `from` = a number of leading bytes already known to be equal (the compare starts at the word that holds byte `from`).

@@ -4,8 +4,6 @@
 //   k_scan (scan_kernel.cuh)  REVERSE range scans, every request of a batch that mixes directions, and forward scans
 //           whose user keys are too long for k_scan_fwd: one CTA per request stages chunks of blocks of every run in shared memory.
 #include <algorithm>
-#include <cstdio>
-#include <cstdlib>
 #include <cstring>
 
 #include "engine.h"
@@ -102,6 +100,20 @@ static int32_t snapshot_multi(pgs_partition *const *parts, uint32_t n_parts, con
     return PGS_OK;
 }
 
+// the dynamic shared memory of a k_scan launch of n_req requests over these runs on the current device (scan_dyn_bytes: 0 when
+// one block of every run does not fit); *pool = its staging pool
+static cudaError_t scan_launch_dyn(const Engine &e, const std::vector<std::shared_ptr<Run>> &runs, uint32_t KS, uint32_t n_req,
+                                   uint64_t &dyn, uint32_t *pool)
+{
+    cudaFuncAttributes attr;
+    const cudaError_t rc = cudaFuncGetAttributes(&attr, k_scan);
+    if (rc != cudaSuccess) return rc;
+    ScanBlockBound bb;
+    for (auto &r : runs) bb.add(r->info);
+    dyn = scan_dyn_bytes((uint32_t)runs.size(), KS, bb.max_blk, bb.max_rec, n_req, scan_max_dyn(e.max_smem_optin, attr.sharedSizeBytes), pool);
+    return cudaSuccess;
+}
+
 // true when k_scan can stage one block of every current run of the partition in one request's launch; scan_launch answers
 // a batch with a reverse request with PGS_NOT_SUPPORTED otherwise (the server folds L0 first, server.cpp)
 bool scan_stages_every_run(Partition &part)
@@ -113,13 +125,11 @@ bool scan_stages_every_run(Partition &part)
     }
     if (runs.size() > kMaxReadRuns) return false;
     uint32_t mk = 0;
-    ScanBlockBound bb;
-    for (auto &r : runs) { mk = std::max(mk, r->info.max_ukey_len); bb.add(r->info); }
-    cudaFuncAttributes attr;
-    if (cudaSetDevice(part.eng->device) != cudaSuccess || cudaFuncGetAttributes(&attr, k_scan) != cudaSuccess) return true; // the launch reports it
-    uint32_t pool = 0;
-    return scan_dyn_bytes((uint32_t)runs.size(), read_key_slot(mk), bb.max_blk, bb.max_rec, 1,
-                          scan_max_dyn(part.eng->max_smem_optin, attr.sharedSizeBytes), &pool) != 0;
+    for (auto &r : runs) mk = std::max(mk, r->info.max_ukey_len);
+    uint64_t dyn = 0; uint32_t pool = 0;
+    if (cudaSetDevice(part.eng->device) != cudaSuccess || scan_launch_dyn(*part.eng, runs, read_key_slot(mk), 1, dyn, &pool) != cudaSuccess)
+        return true; // the launch reports it
+    return dyn != 0;
 }
 
 // kernels of this file take their dynamic shared-memory size per launch; the opt-in maximum is set once per device here
@@ -191,7 +201,6 @@ static int32_t scan_launch(Partition &part, const std::vector<std::shared_ptr<Ru
     const ScanBatch B = flatten_scan_requests(reqs, n);
     if (!scan_output_strides(P, arena_stride, kv_stride, resume_stride)) resume_stride = 0; // caller gave no room for resume keys
     P.n = n; P.now = now; P.data_version = part.data_version;
-    P.use_tma = (e->cfg.flags & PGS_ENGINE_NO_TMA) ? 0 : 1;
     if (multi ? multi->packed.empty() : P.rr.n == 0) { // empty DB: every iterator is invalid from the start
         memset(results, 0, sizeof(pgs_scan_result) * n);
         if (arena_base) for (uint32_t i = 0; i <= n; i++) arena_base[i] = 0;
@@ -209,18 +218,15 @@ static int32_t scan_launch(Partition &part, const std::vector<std::shared_ptr<Ru
     PGS_CUDA(S.alloc(P.kvs, sizeof(pgs_kv) * (size_t)kv_stride * n + 16));
     PGS_CUDA(S.alloc(P.resume, (size_t)P.resume_stride * n + 16));
     PGS_CUDA(S.alloc(P.results, sizeof(pgs_scan_result) * n));
-    PGS_CUDA(S.alloc(P.error, 256));
-    PGS_CUDA(cudaMemsetAsync(P.error, 0, 256, st));
+    PGS_CUDA(S.alloc(P.error, 16));
+    PGS_CUDA(cudaMemsetAsync(P.error, 0, 16, st));
     if (multi) {
         PGS_CUDA(S.upload(P.multi_runs, multi->packed.data(), multi->packed.size()));
         PGS_CUDA(S.upload(P.multi_begin, multi->begin.data(), multi->begin.size()));
         PGS_CUDA(S.upload(P.req_part, req_part, n));
     }
     if (B.need_crc) P.crc_table = (const unsigned long long *)e->d_crc;
-    P.ticket = P.error + 8;
-    const char *pt_env = getenv("PGS_PHASE_TIMING"); // diagnostics: per-phase cycle totals of the reverse kernel on stderr
-    const bool phase_timing = B.any_reverse && pt_env && pt_env[0] == '1';
-    P.phase_cycles = phase_timing ? (unsigned long long *)(P.error + 16) : nullptr;
+    P.ticket = P.error + 1;
     // forward scans: lane-group merging iterators (read_kernels.cuh), unless the groups' key rows do not fit shared memory
     // (user keys of a few KB): then k_scan, which stages records instead of keeping one key row per run and group
     const ReadGeometry fwd = scan_fwd_geometry(P.rr.n, P.KS);
@@ -238,12 +244,8 @@ static int32_t scan_launch(Partition &part, const std::vector<std::shared_ptr<Ru
         PGS_CUDA(cudaEventRecord(ev_b, st));
     } else {
         // ---- reverse scans (and forward ones with long keys): the block-staging kernel ---------------------------------
-        cudaFuncAttributes attr;
-        PGS_CUDA(cudaFuncGetAttributes(&attr, k_scan));
-        ScanBlockBound bb;
-        for (auto &r : runs) bb.add(r->info);
-        const uint64_t dyn = scan_dyn_bytes((uint32_t)runs.size(), P.KS, bb.max_blk, bb.max_rec, n,
-                                            scan_max_dyn(e->max_smem_optin, attr.sharedSizeBytes), &P.pool_bytes);
+        uint64_t dyn = 0;
+        PGS_CUDA(scan_launch_dyn(*e, runs, P.KS, n, dyn, &P.pool_bytes));
         if (!dyn) {
             set_error("scan: blocks too large for shared memory");
             return PGS_NOT_SUPPORTED;
@@ -254,17 +256,6 @@ static int32_t scan_launch(Partition &part, const std::vector<std::shared_ptr<Ru
         PGS_CUDA(cudaEventRecord(ev_a, st));
         k_scan<<<grid, kScanThreads, dyn, st>>>(P);
         PGS_CUDA(cudaEventRecord(ev_b, st));
-        if (phase_timing) {
-            unsigned long long h[16] = {0};
-            cudaMemcpyAsync(h, P.error + 16, sizeof h, cudaMemcpyDeviceToHost, st);
-            cudaStreamSynchronize(st);
-            static const char *names[13] = {"init", "choose", "stage", "farbound", "decode1", "decode2", "window", "rank", "visible", "loop", "emit", "advance", "result"};
-            unsigned long long tot = 0;
-            for (int i = 0; i < 13; i++) tot += h[i];
-            fprintf(stderr, "[k_scan phases] requests=%u grid=%u dyn=%llu", n, grid, (unsigned long long)dyn);
-            for (int i = 0; i < 13; i++) fprintf(stderr, " %s=%.1f%%", names[i], tot ? 100.0 * (double)h[i] / (double)tot : 0.0);
-            fprintf(stderr, " cycles/request=%.0f\n", n ? (double)tot / n : 0.0);
-        }
     }
     e->launches++;
     uint32_t herr = 0;

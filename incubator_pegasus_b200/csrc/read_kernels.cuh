@@ -251,7 +251,7 @@ struct ScanParams {
     ReadRuns rr;
     const ScanReqDev *reqs;
     const uint8_t *blob; // request byte strings
-    uint32_t n, now, data_version, use_tma;
+    uint32_t n, now, data_version;
     uint32_t KS, KSW, group_smem, pool_bytes;
     pgs_scan_result *results;
     pgs_kv *kvs;
@@ -263,7 +263,6 @@ struct ScanParams {
     const unsigned long long *crc_table;
     uint32_t *error;
     uint32_t *ticket;
-    unsigned long long *phase_cycles; // [16] or null (PGS_PHASE_TIMING=1, reverse kernel only)
     // requests of several partitions in one launch (pgs_range_scan_many_multi, forward only): request i reads the runs
     // multi_runs[multi_begin[req_part[i]] .. multi_begin[req_part[i] + 1]); rr.n = the largest run count; null otherwise
     const RunDev *multi_runs;

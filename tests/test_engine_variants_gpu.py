@@ -1,6 +1,6 @@
-"""GPU parity under the non-default settings: every lane-group width of the compaction walker (PGS_WALK_G; the default is 4, wider
-groups are what long keys fall back to) and the plain-load staging path of the reverse-scan kernel (PGS_ENGINE_NO_TMA).
-Same oracle comparison as test_compaction_gpu."""
+"""GPU parity with the oracle for every lane-group width of the compaction walker (PGS_WALK_G; the default is 4, wider groups are
+what long keys fall back to), with the same comparison as test_compaction_gpu, and for the read path over overlapping L0 runs
+through the rrdb surface."""
 import random
 
 import pytest
@@ -12,13 +12,6 @@ from test_compaction_gpu import run_case
 NOW = synth.NOW
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(params=[dict(flags=1)], ids=["no_tma"])
-def variant_engine(pgs, request):
-    eng = pgs.Engine(**request.param)
-    yield eng
-    eng.close()
 
 
 @pytest.mark.parametrize("lanes", [1, 2, 8, 16])
@@ -47,9 +40,9 @@ def test_long_keys_pick_a_wider_group(pgs, oracle, engine):
     run_case(pgs, oracle, engine, runs, bottommost=True)
 
 
-def test_reads_variants(variant_engine):
-    """gets, multi_gets (forward / reverse / limited), sortkey_count and scans through the rrdb surface on the variant engine"""
-    g, o = Backend("gpu", variant_engine, opts={"l0_compaction_trigger": 100}), Backend("oracle", opts={"l0_compaction_trigger": 100})
+def test_reads_variants(engine):
+    """gets, multi_gets (forward / reverse / limited), sortkey_count and scans through the rrdb surface over 4 overlapping L0 runs"""
+    g, o = Backend("gpu", engine, opts={"l0_compaction_trigger": 100}), Backend("oracle", opts={"l0_compaction_trigger": 100})
     rnd = random.Random(5)
     try:
         for round_ in range(4):  # 4 overlapping L0 runs

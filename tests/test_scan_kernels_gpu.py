@@ -174,25 +174,6 @@ def test_scans_against_the_model(pgs, engine, n_runs, block_size, ri, compacted,
         part.close()
 
 
-def test_reverse_scans_without_tma(pgs):
-    """the plain-load staging path of k_scan (PGS_ENGINE_NO_TMA) on the same shapes"""
-    eng = pgs.Engine(flags=1)
-    try:
-        for n_runs, block_size, ri, compacted, long_keys in (CASES[1], CASES[3]):
-            recs, items = build_db(pgs, 1000 + n_runs, n_runs, long_keys, block_size)
-            vis, _ = visible(items)
-            part = load(pgs, eng, recs, block_size, ri, compacted)
-            try:
-                rev = [mirror(q) for q in request_list(vis)]
-                st, got = run_scans(pgs, part, rev, stride(vis))
-                assert st == 0, st
-                check(vis, rev, got, "reverse batch, no TMA")
-            finally:
-                part.close()
-    finally:
-        eng.close()
-
-
 def test_output_limits(pgs, engine):
     """a request's output larger than its arena / kv slice -> PGS_ABORTED; a packed batch larger than arena_cap / kv_cap ->
     PGS_INCOMPLETE; a resume slot shorter than a key -> no resume keys.  For both kernels."""

@@ -265,7 +265,7 @@ int32_t sim_get(uint32_t k, const uint8_t **data, const uint64_t *data_bytes, co
 
 // range scans over k runs; outputs as the device side of scan_many (request i uses arena + i*arena_stride, kvs + i*kv_stride;
 // scan_output_strides rounds arena_stride up to a multiple of 16).
-// A batch without reverse requests runs k_scan_fwd, any other batch k_scan (here without TMA).  pool_bytes (k_scan only): 0 =
+// A batch without reverse requests runs k_scan_fwd, any other batch k_scan.  pool_bytes (k_scan only): 0 =
 // the pool the product gives a batch of n requests; otherwise at most pool_bytes, but never below the smallest pool
 // (scan_min_pool: one block of every run), so that a small value forces chunks of about one block.
 int32_t sim_scan(uint32_t k, const uint8_t **data, const uint64_t *data_bytes, const uint64_t **blk_off, const uint32_t **blk_size,
@@ -278,9 +278,9 @@ int32_t sim_scan(uint32_t k, const uint8_t **data, const uint64_t *data_bytes, c
     uint32_t mk = 0;
     if (!load_runs(k, data, data_bytes, blk_off, blk_size, n_blocks, runs, P.rr, mk)) return PGS_CORRUPTION;
     const ScanBatch B = flatten_scan_requests(reqs, n);
-    uint32_t err[16] = {0};
+    uint32_t err[4] = {0, 0, 0, 0};
     P.reqs = B.reqs.data(); P.blob = (const uint8_t *)B.blob.data(); P.n = n; P.now = now; P.data_version = 1;
-    P.results = results; P.kvs = kvs; P.arena = arena; P.resume = resume; P.error = err; P.ticket = err + 8;
+    P.results = results; P.kvs = kvs; P.arena = arena; P.resume = resume; P.error = err; P.ticket = err + 1;
     P.KS = read_key_slot(mk);
     scan_output_strides(P, arena_stride, kv_stride, resume_stride);
     if (B.need_crc) { crc64_make_table(crc_tab); P.crc_table = (const unsigned long long *)crc_tab; }
@@ -288,7 +288,6 @@ int32_t sim_scan(uint32_t k, const uint8_t **data, const uint64_t *data_bytes, c
         if (lanes) return PGS_INVALID_ARGUMENT; // k_scan has no lane groups and no multi-partition shape
         ScanBlockBound bb;
         for (auto &r : runs) bb.add(r.info);
-        P.use_tma = 0;
         uint64_t dyn = scan_dyn_bytes(k, P.KS, bb.max_blk, bb.max_rec, n, scan_max_dyn(kSimSmemOptin, sizeof(ScanShared)), &P.pool_bytes);
         if (!dyn) return PGS_NOT_SUPPORTED;
         if (pool_bytes) {

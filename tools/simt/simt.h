@@ -285,7 +285,6 @@ inline int __popcll(unsigned long long x) { return __builtin_popcountll(x); }
 inline int __clz(int x) { return x ? __builtin_clz((uint32_t)x) : 32; }
 inline uint32_t __brev(uint32_t x) { uint32_t r = 0; for (int i = 0; i < 32; i++) r |= ((x >> i) & 1u) << (31 - i); return r; }
 inline uint32_t __umulhi(uint32_t a, uint32_t b) { return (uint32_t)(((uint64_t)a * b) >> 32); }
-inline long long clock64() { static long long c = 0; return c += 7; }
 template <class T> inline T min(T a, T b) { return a < b ? a : b; }
 template <class T> inline T max(T a, T b) { return a > b ? a : b; }
 inline uint32_t min(uint32_t a, int b) { return a < (uint32_t)b ? a : (uint32_t)b; }
