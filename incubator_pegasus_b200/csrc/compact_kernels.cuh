@@ -14,17 +14,19 @@
 //                 => cumulative weight of everything <= that key.  Keys where the weight crosses a multiple of the
 //                 segment budget become segment boundaries: segment q = user keys in (U_q, U_q+1], a contiguous
 //                 block range per run.  All versions of a user key fall into one segment.
-//   k_walk        the merge itself.  A *group* of 8 (16, 32) lanes owns one segment and walks it sequentially like
-//                 RocksDB's MergingIterator + CompactionIterator: one cursor per run decoding entries straight from
-//                 HBM (group.cuh), the current keys in shared-memory rows compared with one ballot, newest version
-//                 wins, tombstone / bottommost rules, Filter() per surviving value, prefix compression against the
+//   k_walk        the merge itself.  A *group* of G lanes (4 by default, 1 to 16) owns one segment and walks it
+//                 sequentially like RocksDB's MergingIterator + CompactionIterator: one cursor per run decoding entries
+//                 straight from HBM (group.cuh), the current keys in shared-memory rows compared with one ballot, newest
+//                 version wins, tombstone / bottommost rules, Filter() per surviving value, prefix compression against the
 //                 previous survivor, 4 KB block cuts.  It copies no values: per survivor it emits a 16-byte descriptor
-//                 (where the value lives, lengths, flags) and the finished entry head (varints | key delta | trailer).
-//                 Four (two, one) groups share a warp in lock step; there is no block-wide barrier anywhere.
+//                 (where the value lives, lengths, flags) and a key-stream record (trailer | rewritten expire_ts | user key).
+//                 32/G groups share a warp in lock step; there is no block-wide barrier anywhere.
 //   k_seg_scan    exclusive prefix of the per-segment output sizes (bytes, blocks, records, index-key bytes).
-//   k_emit        one warp per segment builds the output blocks: heads and values are gathered into a shared-memory
-//                 block buffer (16-byte global loads, byte-exact placement), restart array and padding are appended and
-//                 the finished block leaves with ONE bulk TMA store; the new run's index is written alongside.
+//   k_emit        one warp per segment builds the output blocks in batches of up to 32 entries, one thread per entry:
+//                 entry heads (from the key-stream records) and values are gathered into a shared-memory buffer
+//                 (16-byte global loads, byte-exact placement) together with the restart arrays and padding of the
+//                 blocks that close, and each batch leaves with one bulk TMA store; the new run's index and Bloom filter
+//                 are written alongside.
 //   Output blocks stay contiguous and in key order; every segment starts a new block.
 #pragma once
 #include <algorithm>
@@ -41,21 +43,58 @@ constexpr uint32_t kEmitThreads = 128;
 
 enum : uint32_t { DF_NEWBLOCK = 1, DF_REWRITE = 2, DF_BIG = 4 };
 
-// one per surviving record, written by k_walk, read by k_emit
+// ---- what k_walk hands to k_emit ---------------------------------------------------------------------------------------------
+// One descriptor per surviving record.
 struct __align__(16) Desc {
     unsigned long long loc; // bits 0..39 byte offset of the value inside its run, 40..43 run, 44..59 user-key bytes, 60..63 DF_*
     uint32_t vlen;          // value bytes to copy (0 for a tombstone)
     uint32_t aux;           // bytes the user key shares with the previous survivor of the segment
 };
 static_assert(sizeof(Desc) == 16, "Desc");
+PGS_HD unsigned long long desc_loc(unsigned long long voff, unsigned long long run, unsigned long long ulen, unsigned long long flags)
+{
+    return voff | (run << 40) | (ulen << 44) | (flags << 60);
+}
+PGS_HD unsigned long long desc_voff(unsigned long long loc) { return loc & ((1ull << 40) - 1); }
+PGS_HD uint32_t desc_run(unsigned long long loc) { return (uint32_t)(loc >> 40) & 15u; }
+PGS_HD uint32_t desc_ulen(unsigned long long loc) { return (uint32_t)(loc >> 44) & 0xffffu; }
+PGS_HD uint32_t desc_flags(unsigned long long loc) { return (uint32_t)(loc >> 60); }
+
+// One record per survivor in its segment's key stream: trailer (8 bytes) | the rewritten expire_ts (BE32, only with DF_REWRITE) |
+// the whole user key, padded to 4 bytes.  k_emit builds the entry head, the index key and the Bloom filter bits from it.
+PGS_HD uint32_t ks_fixed(uint32_t flags) { return (flags & DF_REWRITE) ? 12u : 8u; }
+PGS_HD uint32_t ks_record(uint32_t flags, uint32_t ulen) { return ks_fixed(flags) + ((ulen + 3) & ~3u); }
+// the key-stream bytes planned per input record for user keys of at most KS bytes (more than ks_record(DF_REWRITE, KS))
+PGS_HD uint32_t ks_record_bound(uint32_t KS) { return 15 + KS + 8 + 4; }
+
+// An output block: entries, then the restart array (one 4-byte offset per restart point) and its 4-byte count, padded to
+// kBlockAlign.  An entry is varint shared | varint non_shared (= key delta + 8) | varint value length | key delta | trailer | value.
+PGS_HD uint32_t entry_head_len(uint32_t shared, uint32_t kd, uint32_t vlen) { return varint_len(shared) + varint_len(kd + 8) + varint_len(vlen) + kd + 8; }
+PGS_HD uint32_t block_bytes(uint32_t entry_bytes, uint32_t nrest) { return entry_bytes + 4 * (nrest + 1); }
+PGS_HD uint32_t block_span(uint32_t size) { return (size + kBlockAlign - 1) & ~(kBlockAlign - 1); }
+PGS_HD uint32_t restart_count(uint32_t n, uint32_t RI) { return (n + RI - 1) / RI; } // restart points of n entries
+PGS_DEV uint32_t put_varint32_s(uint8_t *p, uint32_t v) // shared-memory / generic byte stores
+{
+    uint32_t n = 0;
+    while (v >= 128u) { p[n++] = (uint8_t)(v | 128u); v >>= 7; }
+    p[n++] = (uint8_t)v;
+    return n;
+}
+// the three varints of an entry head at p; returns their bytes
+PGS_DEV uint32_t put_entry_varints(uint8_t *p, uint32_t shared, uint32_t kd, uint32_t vlen)
+{
+    uint32_t n = put_varint32_s(p, shared);
+    n += put_varint32_s(p + n, kd + 8);
+    return n + put_varint32_s(p + n, vlen);
+}
 
 struct SegLayout { // where a segment's scratch lives (k_seg_layout)
     unsigned long long desc_off; // index of its first descriptor
-    unsigned long long head_off; // byte offset of its head stream
+    unsigned long long ks_off;   // byte offset of its key stream
 };
 struct __align__(16) SegAgg { // what a segment produced (k_walk)
     unsigned long long out_bytes; // sum of 16-aligned block sizes
-    uint32_t n_entries, n_blocks, keyb, head_bytes, last_klen, pad;
+    uint32_t n_entries, n_blocks, keyb, ks_bytes, last_klen, pad;
 };
 struct __align__(16) SegBase { // exclusive prefixes over the segments (k_seg_scan)
     unsigned long long bytes;
@@ -90,12 +129,12 @@ struct MergeParams {
     SegAgg *agg;
     SegBase *base;
     Desc *desc;
-    uint8_t *heads;
-    unsigned long long desc_cap, head_cap;
+    uint8_t *kstream; // the segments' key streams
+    unsigned long long desc_cap, ks_cap;
     uint32_t *ticket; // [0] k_walk, [1] k_emit
     uint32_t KS;      // user-key capacity of a key row (multiple of 4)
     uint32_t KSW;     // 32-bit words per key row
-    uint32_t group_smem, emit_warp_smem, emit_obuf, blk_buf, head_stage;
+    uint32_t group_smem, emit_warp_smem, emit_obuf, blk_buf, ks_stage;
     // filter + policy
     uint32_t now, enabled, validate_hash, data_version, default_ttl;
     int32_t pidx, partition_version;
@@ -163,9 +202,15 @@ struct CompactGeometry {
     uint32_t G, walk_dyn, emit_warps, emit_dyn;
     uint64_t blk_cap, out_cap, ikey_cap;
 };
+struct WalkCtaStats { // k_walk's per-CTA totals, shared memory
+    uint32_t cnt[12];
+    unsigned long long bytes[4];
+    unsigned long long mx[6];
+};
+// k_walk's CTA-wide shared memory in front of the groups': crc table (2 KB), run table, WalkCtaStats
+constexpr uint32_t kWalkFixedSmem = 2048 + kMaxRuns * (uint32_t)sizeof(RunDev) + (uint32_t)sizeof(WalkCtaStats);
 // fills the derived fields of P (P.k, P.block_size, P.restart_interval must be set); false = not supported
 constexpr uint32_t kWalkMinG = 4; // default lanes per merge group (see group.cuh)
-inline uint32_t walk_fixed_smem();
 // walk_groups = merge groups the device runs at the same time (0: not known yet, the default segment budget is used)
 inline bool compact_geometry(MergeParams &P, const CompactTotals &T, uint32_t max_smem, CompactGeometry &geo, uint32_t force_G = 0,
                              uint64_t force_weight = 0, uint64_t walk_groups = 0)
@@ -181,28 +226,29 @@ inline bool compact_geometry(MergeParams &P, const CompactTotals &T, uint32_t ma
     // lanes per group: the narrowest shape whose CTA fits shared memory twice per SM (or once); force_G overrides (diagnostics)
     geo.G = 0;
     for (uint32_t G = force_G ? force_G : kWalkMinG; G <= 16 && !geo.G; G *= 2) {
-        const uint64_t dyn = walk_fixed_smem() + (uint64_t)(kWalkThreads / G) * P.group_smem;
+        const uint64_t dyn = kWalkFixedSmem + (uint64_t)(kWalkThreads / G) * P.group_smem;
         if (dyn <= max_smem / 2 || (force_G && dyn <= max_smem)) geo.G = G;
     }
     for (uint32_t G = kWalkMinG; G <= 16 && !geo.G; G *= 2)
-        if (walk_fixed_smem() + (uint64_t)(kWalkThreads / G) * P.group_smem <= max_smem) geo.G = G;
+        if (kWalkFixedSmem + (uint64_t)(kWalkThreads / G) * P.group_smem <= max_smem) geo.G = G;
     if (!geo.G) return false;
-    geo.walk_dyn = walk_fixed_smem() + (kWalkThreads / geo.G) * P.group_smem;
+    geo.walk_dyn = kWalkFixedSmem + (kWalkThreads / geo.G) * P.group_smem;
     const uint32_t hs = (2 * P.KS + 64 + 15) & ~15u;
-    P.head_stage = hs < 2048 ? 2048u : hs;
-    // k_emit per warp: an output assembly buffer (at least one block, normally 8 KB = a batch of ~28 entries), the head stage,
-    // the restart offsets of the open block.  An entry that does not fit a block buffer gets a block of its own, written in place.
+    P.ks_stage = hs < 2048 ? 2048u : hs;
+    // k_emit per warp: an output assembly buffer (at least one block, normally 8 KB = a batch of ~28 entries), the key-stream
+    // stage, the restart offsets of the open block.  An entry that does not fit a block buffer gets a block of its own, written
+    // in place.
     const uint32_t RI = P.restart_interval;
     uint32_t blk_buf = (P.block_size + 24 + 15) & ~15u;
-    if (blk_buf + 1024ull + P.head_stage + 8ull * (blk_buf / (11 * RI) + 4) > max_smem) { // huge block_size: cut smaller blocks
-        if (max_smem < P.head_stage + 8192) return false;
-        blk_buf = (uint32_t)(((max_smem - P.head_stage - 1024) * 11ull / 20)) & ~15u;
+    if (blk_buf + 1024ull + P.ks_stage + 8ull * (blk_buf / (11 * RI) + 4) > max_smem) { // huge block_size: cut smaller blocks
+        if (max_smem < P.ks_stage + 8192) return false;
+        blk_buf = (uint32_t)(((max_smem - P.ks_stage - 1024) * 11ull / 20)) & ~15u;
         if (P.block_size > blk_buf - 24) P.block_size = blk_buf - 24;
     }
     P.blk_buf = blk_buf;
     const uint32_t ob_min = blk_buf + 4 * (blk_buf / (11 * RI) + 4) + 256; // an entry + the restart array of the block it closes
     P.emit_obuf = ob_min < 8192 ? 8192u : ((ob_min + 15) & ~15u);
-    P.emit_warp_smem = (uint32_t)((P.emit_obuf + 32ull + P.head_stage + 32 + 4ull * (blk_buf / (11 * RI) + 4) + 15) & ~15ull);
+    P.emit_warp_smem = (uint32_t)((P.emit_obuf + 32ull + P.ks_stage + 32 + 4ull * (blk_buf / (11 * RI) + 4) + 15) & ~15ull);
     geo.emit_warps = max_smem / P.emit_warp_smem;
     if (geo.emit_warps > kEmitThreads / 32) geo.emit_warps = kEmitThreads / 32;
     if (geo.emit_warps == 0) return false;
@@ -244,9 +290,9 @@ inline bool compact_geometry(MergeParams &P, const CompactTotals &T, uint32_t ma
     // scratch: the blocks on a segment boundary are read by both neighbours
     const uint64_t Nb = T.n_rec + Q * k * (uint64_t)T.max_blk_rec;
     const uint64_t Bb = T.in_block_bytes + Q * k * ((uint64_t)T.max_blk + 16);
-    const uint64_t per_head = 15 + P.KS + 8 + 4;
+    const uint64_t per_rec = ks_record_bound(P.KS);
     P.desc_cap = Nb + 1;
-    P.head_cap = Nb * per_head + (2 * (Bb + Nb * per_head) / P.block_size + 2 * Q + 2) * (uint64_t)(P.KS + 8) + 64 * Q + 64;
+    P.ks_cap = Nb * per_rec + (2 * (Bb + Nb * per_rec) / P.block_size + 2 * Q + 2) * (uint64_t)(P.KS + 8) + 64 * Q + 64;
     P.out_bloom_lines = bloom_lines_for(T.bloom_entries);
     return true;
 }
@@ -284,7 +330,7 @@ inline void compact_buffers(MergeParams &P, const CompactGeometry &geo, const Co
     buf(P.agg, Q, 0, false);                      // a walk that did not run produced nothing
     buf(P.base, Q, kNoFill, false);
     buf(P.desc, P.desc_cap, kNoFill, false);
-    buf(P.heads, P.head_cap + 64, kNoFill, false);
+    buf(P.kstream, P.ks_cap + 64, kNoFill, false);
     buf(run.d_data, geo.out_cap + 256, kNoFill, true);
     buf(run.d_blk_off, nb, kNoFill, true);
     buf(run.d_blk_size, nb, kNoFill, true);
@@ -376,17 +422,17 @@ PGS_DEV bool seg_slice(const MergeParams &P, uint32_t q, uint32_t j, uint32_t &l
     return true;
 }
 
-// upper bounds of a segment's scratch use, from its input slice: records and block bytes it may read
-PGS_HD unsigned long long head_bound(unsigned long long n_in, unsigned long long in_bytes, uint32_t KS, uint32_t block_size)
+// upper bound of a segment's key stream, from its input slice: records and block bytes it may read
+PGS_HD unsigned long long ks_bound(unsigned long long n_in, unsigned long long in_bytes, uint32_t KS, uint32_t block_size)
 {
-    const unsigned long long per_head = 15 + KS + 8 + 4; // varints | whole internal key | rewritten expire_ts
-    unsigned long long blocks = 2 * (in_bytes + n_in * per_head) / block_size + 2;
+    const unsigned long long per_rec = ks_record_bound(KS);
+    unsigned long long blocks = 2 * (in_bytes + n_in * per_rec) / block_size + 2;
     if (blocks > n_in + 1) blocks = n_in + 1;
-    return (n_in * per_head + blocks * (unsigned long long)(KS + 8) + 64 + 15) & ~15ull; // key-stream records are stored as words
+    return (n_in * per_rec + blocks * (unsigned long long)(KS + 8) + 64 + 15) & ~15ull; // key-stream records are stored as words
 }
 
 // ------------------------------------------------------------------------------------------------
-// k_seg_bounds + k_seg_layout: where each segment's descriptor array and head stream live.  One thread per segment computes
+// k_seg_bounds + k_seg_layout: where each segment's descriptor array and key stream live.  One thread per segment computes
 // the bounds of what it may emit (from its input slice); one CTA turns them into offsets with an exclusive scan.
 // ------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) k_seg_bounds(const __grid_constant__ MergeParams P)
@@ -403,19 +449,19 @@ __global__ void __launch_bounds__(256) k_seg_bounds(const __grid_constant__ Merg
     }
     if (!ok) { atomicMax(&P.stats->error, (uint32_t)PGS_ABORTED); atomicMin(&P.stats->error_seg, q); }
     P.seg[q].desc_off = n_in;
-    P.seg[q].head_off = head_bound(n_in, in_bytes, P.KS, P.block_size);
+    P.seg[q].ks_off = ks_bound(n_in, in_bytes, P.KS, P.block_size);
 }
 
 __global__ void __launch_bounds__(1024) k_seg_layout(const __grid_constant__ MergeParams P)
 {
     uint32_t q0, q1;
     unsigned long long pre[2], tot[2];
-    cta_excl_scan<2>(P.Q, [&](uint32_t q, unsigned long long (&v)[2]) { v[0] += P.seg[q].desc_off; v[1] += P.seg[q].head_off; }, q0, q1, pre, tot);
-    if (threadIdx.x == 0 && (tot[0] > P.desc_cap || tot[1] > P.head_cap)) { atomicMax(&P.stats->error, (uint32_t)PGS_ABORTED); atomicMin(&P.stats->error_seg, 0u); }
+    cta_excl_scan<2>(P.Q, [&](uint32_t q, unsigned long long (&v)[2]) { v[0] += P.seg[q].desc_off; v[1] += P.seg[q].ks_off; }, q0, q1, pre, tot);
+    if (threadIdx.x == 0 && (tot[0] > P.desc_cap || tot[1] > P.ks_cap)) { atomicMax(&P.stats->error, (uint32_t)PGS_ABORTED); atomicMin(&P.stats->error_seg, 0u); }
     for (uint32_t q = q0; q < q1; q++) {
-        const unsigned long long a = P.seg[q].desc_off, b = P.seg[q].head_off;
+        const unsigned long long a = P.seg[q].desc_off, b = P.seg[q].ks_off;
         P.seg[q].desc_off = pre[0];
-        P.seg[q].head_off = pre[1];
+        P.seg[q].ks_off = pre[1];
         pre[0] += a;
         pre[1] += b;
     }
@@ -505,11 +551,6 @@ struct WalkAcc {
     uint32_t m_ukey, m_vlen, m_bsize, m_brec;
     unsigned long long m_seq, m_seq_inv;
 };
-struct WalkCtaStats { // per CTA, shared memory
-    uint32_t cnt[12];
-    unsigned long long bytes[4];
-    unsigned long long mx[6];
-};
 PGS_DEV uint32_t spread4(uint32_t x) { return (x * 0x00204081u) & 0x01010101u; } // bits 0..3 -> the low bit of bytes 0..3
 PGS_DEV void acc_flush_events(WalkAcc &acc, WalkCtaStats *cta, bool lane0)
 {
@@ -597,7 +638,6 @@ PGS_DEV void walk_segment(const MergeParams &P, const RunDev *runs, const Grp<G>
     uint32_t live = 0;
     unsigned long long order = 0; // entries 0..live-1: the group's runs in merge order
     uint32_t dpos = 0;
-    bool by_byte = false;
 #pragma unroll 1
     for (uint32_t j = 0; j < k; j++) {
         const bool en = seg_en && !err;
@@ -628,7 +668,7 @@ PGS_DEV void walk_segment(const MergeParams &P, const RunDev *runs, const Grp<G>
 #pragma unroll 1
         for (uint32_t i = 0; g.any(searching && i < live); i++) {
             const bool e = searching && i < live;
-            const bool bf = head_before(g, e, cs, rows, KSW, j, ord_at(order, i), dpos, by_byte);
+            const bool bf = head_before(g, e, cs, rows, KSW, j, ord_at(order, i), dpos);
             if (e && bf) { pos = i; searching = false; }
         }
         if (ins) { order = ord_insert(order, pos, j); live++; }
@@ -638,14 +678,14 @@ PGS_DEV void walk_segment(const MergeParams &P, const RunDev *runs, const Grp<G>
     for (uint32_t i = 0; g.any(seg_en && !err && i + 1 < live) && i < 4; i++) {
         const bool e = seg_en && !err && i + 1 < live;
         uint32_t dp = 0;
-        head_before(g, e, cs, rows, KSW, ord_at(order, i), ord_at(order, i + 1), dp, by_byte);
+        head_before(g, e, cs, rows, KSW, ord_at(order, i), ord_at(order, i + 1), dp);
         if (e) adj = adj_set(adj, i, dp);
     }
 
     // ---- the merge loop --------------------------------------------------------------------------------------------------
     Desc *desc = seg_en ? P.desc + P.seg[q].desc_off : nullptr;
-    uint8_t *heads = seg_en ? P.heads + P.seg[q].head_off : nullptr;
-    uint32_t n_out = 0, hpos = 0;                        // descriptors / head-stream bytes written
+    uint8_t *kstream = seg_en ? P.kstream + P.seg[q].ks_off : nullptr;
+    uint32_t n_out = 0, kpos = 0;                        // descriptors / key-stream bytes written
     uint32_t blk_n = 0, blk_bytes = 0;                   // entries and entry bytes of the open output block
     uint32_t to_restart = 0, nrest = 0;                  // entries until the next restart point, restart points so far (no divisions in the loop)
     uint32_t n_blocks = 0, keyb = 0, lenA = 0;
@@ -654,8 +694,8 @@ PGS_DEV void walk_segment(const MergeParams &P, const RunDev *runs, const Grp<G>
     uint32_t hi_run = 0xffu, hi_l = 0, hi_ulen = 0, sw_lcp = kLcpUnknown; // the run whose last key was compared with the upper bound, and the bytes it shared with it
     uint32_t head_len = 0, last_run = 0xffu, lcpA = 0; // lcpA: bytes the head shares with A (the last survivor's key)
     auto close_block = [&]() { // bookkeeping of a finished block (k_emit derives the same numbers)
-        const uint32_t size = blk_bytes + 4 * (nrest + 1);
-        out_bytes += (size + kBlockAlign - 1) & ~(unsigned long long)(kBlockAlign - 1);
+        const uint32_t size = block_bytes(blk_bytes, nrest);
+        out_bytes += block_span(size);
         n_blocks++;
         keyb += lenA;
         if (size > acc.m_bsize) acc.m_bsize = size;
@@ -739,10 +779,11 @@ PGS_DEV void walk_segment(const MergeParams &P, const RunDev *runs, const Grp<G>
             const uint32_t otr_lo = zero_seq ? otype : ((tr_lo & ~0xffu) | otype), otr_hi = zero_seq ? 0u : tr_hi;
             if (vlen_out > 0xFFF00000u) err = PGS_NOT_SUPPORTED; // entry sizes are 32-bit below
             uint32_t kd = ulen - shared;
+            // entry_head_len + value and ks_record below, written out: through the helpers ptxas schedules this loop differently
             uint32_t e = varint_len(shared) + varint_len(kd + 8) + varint_len(vlen_out) + kd + 8 + vlen_out;
             uint32_t flags = 0;
             // block cut: the entry (and the restart array it may extend) must fit the block
-            if (blk_n > 0 && (prev_big || blk_bytes + e + 4 * (nrest + (restart ? 1u : 0u) + 1) > BS)) {
+            if (blk_n > 0 && (prev_big || block_bytes(blk_bytes + e, nrest + (restart ? 1u : 0u)) > BS)) {
                 close_block();
                 blk_n = 0; blk_bytes = 0; nrest = 0;
                 restart = true; shared = 0; kd = ulen;
@@ -752,18 +793,17 @@ PGS_DEV void walk_segment(const MergeParams &P, const RunDev *runs, const Grp<G>
             const bool big = e + 8 > P.blk_buf; // does not fit the block buffer of k_emit: a block of its own, written in place
             if (big) flags |= DF_BIG;
             if (rewrite) flags |= DF_REWRITE;
-            // the survivor's record in the key stream: trailer | [new expire_ts] | the whole user key, padded to 4 bytes
-            // (k_emit builds the entry head, the index key and the Bloom filter bits from it, one thread per entry)
-            uint32_t *sp = reinterpret_cast<uint32_t *>(heads + hpos);
-            const uint32_t fixed = rewrite ? 3u : 2u;
+            // the survivor's key-stream record (ks_record)
+            uint32_t *sp = reinterpret_cast<uint32_t *>(kstream + kpos);
+            const uint32_t fixed = rewrite ? 3u : 2u; // words
 #pragma unroll
             for (uint32_t i = g.gl; i < 3; i += G)
                 if (i < fixed) sp[i] = i == 0 ? otr_lo : i == 1 ? otr_hi : __byte_perm(nts, 0, 0x0123); // BE32 in memory
             kdst = sp + fixed; // the key words follow below, together with the copy that becomes the new A
-            hpos += 4 * fixed + ((ulen + 3) & ~3u);
+            kpos += 4 * fixed + ((ulen + 3) & ~3u);
             if (g.gl == 0) {
                 Desc d;
-                d.loc = (cur_base(C) + C->voff) | ((unsigned long long)c << 40) | ((unsigned long long)ulen << 44) | ((unsigned long long)flags << 60);
+                d.loc = desc_loc(cur_base(C) + C->voff, c, ulen, flags);
                 d.vlen = vlen_out;
                 d.aux = lcp_KA;
                 *reinterpret_cast<uint4 *>(&desc[n_out]) = *reinterpret_cast<const uint4 *>(&d);
@@ -855,7 +895,7 @@ PGS_DEV void walk_segment(const MergeParams &P, const RunDev *runs, const Grp<G>
                 else if (cur < C->klen - 8 && ((row[cur >> 2] >> (8 * (cur & 3))) & 0xffu) > ((rows[r * KSW + (cur >> 2)] >> (8 * (cur & 3))) & 0xffu)) { d = cur; need = false; }
             }
             if (g.any(need)) {
-                const bool bfc = head_before(g, need, cs, rows, KSW, c, r, dpos, by_byte, from);
+                const bool bfc = head_before(g, need, cs, rows, KSW, c, r, dpos, from);
                 if (need) { bf = bfc; d = dpos; }
             }
             if (e) {
@@ -877,19 +917,16 @@ PGS_DEV void walk_segment(const MergeParams &P, const RunDev *runs, const Grp<G>
         if (!err && blk_n > 0) close_block();
         if (err) {
             if (g.gl == 0) { atomicMax(&P.stats->error, err); atomicMin(&P.stats->error_seg, q); }
-            n_out = 0; n_blocks = 0; keyb = 0; out_bytes = 0; hpos = 0; lenA = 0;
+            n_out = 0; n_blocks = 0; keyb = 0; out_bytes = 0; kpos = 0; lenA = 0;
         }
         if (g.gl == 0) {
             SegAgg a;
-            a.out_bytes = out_bytes; a.n_entries = n_out; a.n_blocks = n_blocks; a.keyb = keyb; a.head_bytes = hpos; a.last_klen = lenA; a.pad = 0;
+            a.out_bytes = out_bytes; a.n_entries = n_out; a.n_blocks = n_blocks; a.keyb = keyb; a.ks_bytes = kpos; a.last_klen = lenA; a.pad = 0;
             P.agg[q] = a;
         }
     }
     g.sync();
 }
-
-constexpr uint32_t kWalkFixedSmem = 2048 + kMaxRuns * (uint32_t)sizeof(RunDev) + (uint32_t)sizeof(WalkCtaStats);
-inline uint32_t walk_fixed_smem() { return kWalkFixedSmem; }
 
 template <uint32_t G>
 __global__ void __launch_bounds__(kWalkThreads, 4) k_walk(const __grid_constant__ MergeParams P)
@@ -1069,13 +1106,6 @@ PGS_DEV void copy_bytes_s2s(uint8_t *dst, const uint8_t *src, uint32_t n)
         for (uint32_t i = 0; i < n; i++) dst[i] = (uint8_t)(v >> (8 * i));
     }
 }
-PGS_DEV uint32_t put_varint32_s(uint8_t *p, uint32_t v) // shared-memory / generic byte stores
-{
-    uint32_t n = 0;
-    while (v >= 128u) { p[n++] = (uint8_t)(v | 128u); v >>= 7; }
-    p[n++] = (uint8_t)v;
-    return n;
-}
 
 // k_emit: one warp per segment, one THREAD per entry.  A batch of up to 32 descriptors is laid out with warp scans (block
 // membership, restart points, entry sizes, offsets inside the block, block starts); every thread builds its entry's head from
@@ -1084,19 +1114,350 @@ PGS_DEV uint32_t put_varint32_s(uint8_t *p, uint32_t v) // shared-memory / gener
 // finish the previous block (restart array, padding, index entry); the batch's bytes leave with one bulk TMA store.  Blocks
 // of a segment are adjacent in the output run, so a batch's bytes are one contiguous range; the partial 16-byte chunk at its
 // end is carried into the next batch.
+
+// a warp's shared memory, its lane, and what it added to the filter (counted by lane 0)
+struct EmitWarp {
+    uint8_t *obuf;  // emit_obuf + 32 bytes: the output buffer
+    uint8_t *stage; // ks_stage + 32 bytes: the key-stream records of a batch
+    uint32_t *rst;  // restart offsets of the open block (it may span batches)
+    uint32_t lane, lt; // lt: the lanes before mine
+    uint32_t RI, OB;   // restart interval, output buffer bytes
+    uint32_t n_bloom_keys, n_bloom_prefixes;
+};
+PGS_DEV void emit_warp(EmitWarp &W, const MergeParams &P, uint8_t *ws, uint32_t lane)
+{
+    W.obuf = ws;
+    W.RI = P.restart_interval;
+    W.OB = P.emit_obuf;
+    W.stage = ws + W.OB + 32;
+    W.rst = (uint32_t *)(W.stage + P.ks_stage + 32);
+    W.lane = lane;
+    W.lt = (1u << lane) - 1u;
+    W.n_bloom_keys = W.n_bloom_prefixes = 0;
+}
+
+// what a warp carries across the batches of a segment (warp-uniform)
+struct EmitSeg {
+    const Desc *desc;
+    const uint8_t *ks;              // the segment's key stream
+    uint32_t n;                     // its entries
+    unsigned long long blk_start;   // global offset of the open block (of the segment's first block before it opens)
+    uint32_t fill, blk_n, blk_rec0; // entry bytes / entries of the open block, its first record
+    bool open;
+    uint32_t blk_idx, rec_idx, keyb, kpos; // the next block, record and index-key byte; the next record in the key stream
+    uint32_t carry;                 // obuf[0, carry) = the bytes of the partial 16-byte chunk in front of the write position
+    uint32_t last_key_off, last_ulen; // the previous entry's user key in the key stream (the index key of a block it ends)
+};
+PGS_DEV void emit_seg(EmitSeg &S, const MergeParams &P, uint32_t q, const SegAgg &A, const SegBase &B)
+{
+    S.desc = P.desc + P.seg[q].desc_off;
+    S.ks = P.kstream + P.seg[q].ks_off;
+    S.n = A.n_entries;
+    S.blk_start = B.bytes;
+    S.fill = 0; S.blk_n = 0; S.blk_rec0 = B.recs;
+    S.open = false;
+    S.blk_idx = B.blocks; S.rec_idx = B.recs; S.keyb = B.keyb; S.kpos = 0;
+    S.carry = 0;
+    S.last_key_off = 0; S.last_ulen = 0;
+}
+
+// finish the open block outside a batch (whole warp): restart array (offsets kept in rst), count and padding go to `at`
+// (where byte `fill` of the block lives: obuf + carry, or global memory for a block written in place), index entry
+PGS_DEV void close_open(const MergeParams &P, EmitSeg &S, const EmitWarp &W, const uint8_t *key, uint32_t klen, uint8_t *at, uint32_t nrest)
+{
+    const uint32_t lane = W.lane;
+    const uint32_t size = block_bytes(S.fill, nrest);
+    const uint32_t asz = block_span(size);
+    __syncwarp();
+    for (uint32_t i = lane; i < 4 * (nrest + 1); i += 32) {
+        const uint32_t v = (i >> 2) < nrest ? W.rst[i >> 2] : nrest;
+        at[i] = (uint8_t)(v >> (8 * (i & 3)));
+    }
+    for (uint32_t i = size - S.fill + lane; i < asz - S.fill; i += 32) at[i] = 0;
+    if (lane == 0) {
+        P.out_blk_off[S.blk_idx] = S.blk_start;
+        P.out_blk_size[S.blk_idx] = size;
+        P.out_blk_rec[S.blk_idx] = S.blk_rec0;
+        P.out_ikey_off[S.blk_idx] = S.keyb;
+    }
+    for (uint32_t i = lane; i < klen; i += 32) P.out_ikeys[S.keyb + i] = key[i];
+    S.keyb += klen;
+    S.blk_idx++;
+    S.blk_start += asz;
+    S.fill = 0; S.blk_n = 0; S.open = false;
+}
+// write obuf[0, bytes) to the run at the 16-aligned global offset gpos (bytes % 16 == 0), wait until it has been read
+PGS_DEV void flush(const MergeParams &P, const EmitWarp &W, unsigned long long gpos, uint32_t bytes)
+{
+    __syncwarp();
+    if (bytes) {
+        fence_proxy_async();
+        __syncwarp();
+        if (W.lane == 0) { tma_store_1d(P.out_data + gpos, W.obuf, bytes); tma_store_commit(); tma_store_wait_read0(); }
+        __syncwarp();
+    }
+}
+// close the open block and send what obuf still holds of it
+PGS_DEV void finish_open(const MergeParams &P, EmitSeg &S, const EmitWarp &W)
+{
+    const unsigned long long obase = S.blk_start + S.fill - S.carry;
+    close_open(P, S, W, S.ks + S.last_key_off, S.last_ulen, W.obuf + S.carry, restart_count(S.blk_n, W.RI));
+    flush(P, W, obase, (uint32_t)(S.blk_start - obase));
+    S.carry = 0;
+}
+// one thread: the key (and its hash-key prefix when the previous survivor did not share it) goes into the filter; returns
+// whether the prefix went in
+PGS_DEV bool bloom_add(const MergeParams &P, const uint32_t *key32, uint32_t ulen, uint32_t lcp)
+{
+    if (!P.out_bloom_lines) return false;
+    const unsigned long long hk = bloom_hash_words(key32, ulen);
+#pragma unroll
+    for (uint32_t i = 0; i < 6; i++) bloom_add_bit(P.out_bloom, P.out_bloom_lines, hk, i);
+    const uint32_t pl = hashkey_prefix_len((const uint8_t *)key32, ulen);
+    if (!pl || lcp >= pl) return false;
+    const unsigned long long hp = bloom_hash_words(key32, pl);
+#pragma unroll
+    for (uint32_t i = 0; i < 6; i++) bloom_add_bit(P.out_bloom, P.out_bloom_lines, hp, i);
+    return true;
+}
+
+// one lane's entry of a batch (lane i: entry e0 + i) and the batch layout as far as it has been computed
+struct EmitBatch {
+    unsigned long long loc;               // my descriptor
+    uint32_t fl, ulen, vl, lcp;
+    bool have;                            // there is an entry e0 + lane
+    // batch_fit
+    bool cand, mine, is_restart;          // before the first oversized entry; in the batch; a restart point
+    int h, ph;                            // the lane of the head (first entry) of my block, of the head before me (-1: none)
+    uint32_t hm_all, cnt;                 // the heads among the candidates; the entries of the batch (lanes 0..cnt-1)
+    uint32_t n_i, sh_out, kd, hl, sz, sb; // my index in my block, shared / non-shared key bytes, head and entry bytes, record bytes
+    uint32_t ps_incl, ss_incl;            // entry / record bytes of the lanes at or before me
+    // stage_records
+    uint32_t total_s;                     // the batch's key-stream bytes
+    const uint8_t *staged;                // the batch's first record in the stage
+    // batch_offsets
+    bool closes;                          // I am a head that closes the block before me
+    uint32_t hm, fill_i, base_i, o_i;     // the heads of the batch; my offset in my block; my block's start from blk_start; my offset in obuf
+    uint32_t T, nrest_c, size_c, asz_c;   // the block I close: entry bytes, restart points, size, aligned size
+    uint32_t span_incl, nclose_incl, kb_incl; // aligned bytes / count / index-key bytes of the blocks closed at or before me
+    uint32_t rec_off_i, key_off_i, pk_off, pk_len; // my record and key in the stage; the key of the entry before me
+    unsigned long long obase;             // the global offset of obuf[0]
+};
+
+// An entry larger than a block buffer (DF_BIG, lane 0's; fl = its flags): a block of its own, written in place by the whole warp.
+PGS_DEV void emit_big(const MergeParams &P, EmitSeg &S, EmitWarp &W, const EmitBatch &b, uint32_t fl)
+{
+    const uint32_t lane = W.lane;
+    const unsigned long long loc = __shfl_sync(kFull, b.loc, 0);
+    const uint32_t vl = __shfl_sync(kFull, b.vl, 0), ulen = __shfl_sync(kFull, b.ulen, 0), lcp = __shfl_sync(kFull, b.lcp, 0);
+    const uint8_t *rec = S.ks + S.kpos; // its key-stream record, read from global memory
+    const uint32_t fixed = ks_fixed(fl);
+    const uint8_t *key = rec + fixed;
+    if (S.open) finish_open(P, S, W); // the block in front of it
+    const uint8_t *vsrc = P.runs[desc_run(loc)].data + desc_voff(loc);
+    uint8_t *o = P.out_data + S.blk_start;
+    uint32_t hv = 0;
+    if (lane == 0) { // a restart point: nothing shared
+        hv = put_entry_varints(o, 0u, ulen, vl);
+        const bool np = bloom_add(P, reinterpret_cast<const uint32_t *>(key), ulen, lcp);
+        W.n_bloom_keys += P.out_bloom_lines ? 1u : 0u;
+        W.n_bloom_prefixes += np ? 1u : 0u;
+    }
+    hv = __shfl_sync(kFull, hv, 0);
+    const uint32_t hl = hv + ulen + 8;
+    for (uint32_t x = lane; x < ulen; x += 32) o[hv + x] = key[x];
+    if (lane < 8) o[hv + ulen + lane] = rec[lane]; // trailer
+    for (uint32_t x = lane; x < vl; x += 32) o[hl + x] = vsrc[x];
+    if ((fl & DF_REWRITE) && vl >= 4 && lane < 4) o[hl + lane] = rec[8 + lane];
+    if (lane == 0) { W.rst[0] = 0; P.out_rec_off[S.rec_idx] = 0; }
+    S.fill = hl + vl; S.blk_n = 1; S.blk_rec0 = S.rec_idx; S.open = true;
+    close_open(P, S, W, key, ulen, o + S.fill, 1u); // the block's last user key is this entry's
+    S.last_key_off = S.kpos + fixed; S.last_ulen = ulen;
+    S.rec_idx++; S.kpos += ks_record(fl, ulen);
+}
+
+// ---- the batch phases, in the order k_emit calls them ---------------------------------------------------------------------------
+// my descriptor: fetched with the batch before (dn, when this batch starts at dn_e0), or read now
+PGS_DEV void batch_desc(EmitBatch &b, const EmitSeg &S, const EmitWarp &W, uint32_t e0, const uint4 &dn, uint32_t dn_e0)
+{
+    const uint32_t idx = e0 + W.lane;
+    Desc d;
+    d.loc = 0; d.vlen = 0; d.aux = 0;
+    if (dn_e0 == e0) *reinterpret_cast<uint4 *>(&d) = dn;
+    else if (idx < S.n) *reinterpret_cast<uint4 *>(&d) = *reinterpret_cast<const uint4 *>(&S.desc[idx]);
+    b.have = idx < S.n;
+    b.loc = d.loc; b.fl = desc_flags(d.loc); b.ulen = desc_ulen(d.loc); b.vl = d.vlen; b.lcp = d.aux;
+}
+// Layout and fit.  Block membership and restart points follow from the flags alone; the batch = the entries before the first
+// oversized one that fit the output buffer and the stage.  Returns its entry count (0: not even one fits).
+PGS_DEV uint32_t batch_fit(const MergeParams &P, const EmitSeg &S, const EmitWarp &W, EmitBatch &b)
+{
+    const uint32_t lane = W.lane, lt = W.lt, RI = W.RI;
+    const uint32_t bigmask = __ballot_sync(kFull, b.have && (b.fl & DF_BIG));
+    b.cand = b.have && !(bigmask & (lt | (1u << lane)));
+    b.hm_all = __ballot_sync(kFull, b.cand && (b.fl & DF_NEWBLOCK));
+    const uint32_t at_or_before = b.hm_all & (lt | (1u << lane)), before = b.hm_all & lt;
+    b.h = at_or_before ? 31 - __clz((int)at_or_before) : -1;
+    b.ph = before ? 31 - __clz((int)before) : -1;
+    b.n_i = b.h >= 0 ? lane - (uint32_t)b.h : S.blk_n + lane;
+    b.is_restart = b.n_i % RI == 0;
+    b.sh_out = b.is_restart ? 0u : (b.lcp < b.ulen ? b.lcp : b.ulen);
+    b.kd = b.ulen - b.sh_out;
+    b.hl = entry_head_len(b.sh_out, b.kd, b.vl);
+    b.sz = b.cand ? b.hl + b.vl : 0u;
+    b.sb = b.cand ? ks_record(b.fl, b.ulen) : 0u;
+    b.ps_incl = warp_incl_scan(b.sz, lane);
+    b.ss_incl = warp_incl_scan(b.sb, lane);
+    // room: the entries, the restart arrays and paddings of the blocks that close here (the carried block brings its earlier
+    // restart points along), the carried partial chunk
+    const uint32_t room = S.carry + 32 * (lane + 1) + 64 + (S.open ? 4 * restart_count(S.blk_n, RI) : 0u);
+    const bool fits = b.cand && room + b.ps_incl <= W.OB && b.ss_incl <= P.ks_stage;
+    b.cnt = (uint32_t)__popc(__ballot_sync(kFull, fits)); // monotone: lanes 0..cnt-1
+    b.mine = lane < b.cnt;
+    return b.cnt;
+}
+// Fetch the next batch's descriptors, start staging this batch's key-stream records.
+PGS_DEV void stage_records(const EmitSeg &S, const EmitWarp &W, EmitBatch &b, uint32_t e0, uint4 &dn, uint32_t &dn_e0)
+{
+    dn_e0 = e0 + b.cnt;
+    dn = dn_e0 + W.lane < S.n ? *reinterpret_cast<const uint4 *>(&S.desc[dn_e0 + W.lane]) : make_uint4(0u, 0u, 0u, 0u);
+    b.total_s = __shfl_sync(kFull, b.ss_incl, (int)b.cnt - 1);
+    const uint8_t *src = S.ks + S.kpos;
+    const uint32_t a = (uint32_t)((uintptr_t)src & 15);
+    for (uint32_t i = W.lane * 16; i < a + b.total_s; i += 512) async_copy16(W.stage + i, src - a + i);
+    async_copy_commit();
+}
+// Offsets and block starts: where my entry goes, the block a head closes, the index key of that block (the user key of the
+// entry before the head).
+PGS_DEV void batch_offsets(const MergeParams &P, const EmitSeg &S, const EmitWarp &W, EmitBatch &b)
+{
+    const uint32_t lane = W.lane, lt = W.lt, RI = W.RI;
+    b.hm = b.cnt >= 32 ? b.hm_all : b.hm_all & ((1u << b.cnt) - 1u);
+    const bool head = b.mine && (b.fl & DF_NEWBLOCK);
+    const uint32_t ps = b.ps_incl - b.sz; // entry bytes of the batch before me
+    const uint32_t ps_h = __shfl_sync(kFull, ps, b.h >= 0 ? b.h : 0), ps_ph = __shfl_sync(kFull, ps, b.ph >= 0 ? b.ph : 0);
+    b.fill_i = b.h >= 0 ? ps - ps_h : S.fill + ps;
+    b.closes = head && (b.ph >= 0 || S.open);
+    b.T = b.ph >= 0 ? ps - ps_ph : S.fill + ps;
+    const uint32_t NN = b.ph >= 0 ? lane - (uint32_t)b.ph : S.blk_n + lane;
+    b.nrest_c = b.closes ? restart_count(NN, RI) : 0u;
+    b.size_c = block_bytes(b.T, b.nrest_c);
+    b.asz_c = b.closes ? block_span(b.size_c) : 0u;
+    b.span_incl = warp_incl_scan(b.asz_c, lane);
+    const uint32_t span_h = __shfl_sync(kFull, b.span_incl, b.h >= 0 ? b.h : 0);
+    b.base_i = b.h >= 0 ? span_h : 0u;
+    b.nclose_incl = (uint32_t)__popc(__ballot_sync(kFull, b.closes) & (lt | (1u << lane)));
+    b.rec_off_i = b.ss_incl - b.sb;
+    b.key_off_i = b.rec_off_i + ks_fixed(b.fl);
+    b.pk_off = __shfl_up_sync(kFull, b.key_off_i, 1);
+    const uint32_t pk_len_l = __shfl_up_sync(kFull, b.ulen, 1);
+    b.pk_len = lane == 0 ? S.last_ulen : pk_len_l;
+    b.kb_incl = warp_incl_scan(b.closes ? b.pk_len : 0u, lane);
+    b.obase = S.blk_start + S.fill - S.carry;
+    b.o_i = (uint32_t)(S.blk_start + b.base_i + b.fill_i - b.obase);
+}
+// Restart points: into obuf when my block closes in this batch, else into rst; my entry's offset into the index.
+PGS_DEV void restart_points(const MergeParams &P, const EmitSeg &S, const EmitWarp &W, const EmitBatch &b)
+{
+    const uint32_t lane = W.lane, lt = W.lt, RI = W.RI;
+    const uint32_t after = b.hm & ~(lt | (1u << lane));
+    const int nh = after ? __ffs((int)after) - 1 : -1;                  // the head that closes my block inside this batch
+    const uint32_t T_mine = __shfl_sync(kFull, b.T, nh >= 0 ? nh : 0); // my block's entry bytes, when it closes here
+    const uint32_t r_i = b.n_i / RI;
+    if (b.mine && b.is_restart) {
+        if (nh >= 0) {
+            const uint32_t ro = (uint32_t)(S.blk_start + b.base_i - b.obase) + T_mine + 4 * r_i;
+            W.obuf[ro] = (uint8_t)b.fill_i; W.obuf[ro + 1] = (uint8_t)(b.fill_i >> 8); W.obuf[ro + 2] = (uint8_t)(b.fill_i >> 16); W.obuf[ro + 3] = (uint8_t)(b.fill_i >> 24);
+        } else W.rst[r_i] = b.fill_i;
+    }
+    if (b.mine) P.out_rec_off[S.rec_idx + lane] = b.fill_i;
+}
+// One thread per entry: head, value, filter bits.
+PGS_DEV void write_entries(const MergeParams &P, EmitWarp &W, const EmitBatch &b)
+{
+    bool new_prefix = false;
+    if (b.mine) {
+        const uint8_t *rec = b.staged + b.rec_off_i;
+        const uint8_t *key = b.staged + b.key_off_i;
+        uint8_t *dst = W.obuf + b.o_i;
+        const uint32_t p = put_entry_varints(dst, b.sh_out, b.kd, b.vl);
+        copy_bytes_s2s(dst + p, key + b.sh_out, b.kd);
+        copy_bytes_s2s(dst + p + b.kd, rec, 8u);
+        const RunDev &r = P.runs[desc_run(b.loc)];
+        thread_copy_g2s(W.obuf, b.o_i + b.hl, r.data + desc_voff(b.loc), b.vl, r.data);
+        if ((b.fl & DF_REWRITE) && b.vl >= 4) { dst[b.hl] = rec[8]; dst[b.hl + 1] = rec[9]; dst[b.hl + 2] = rec[10]; dst[b.hl + 3] = rec[11]; }
+        new_prefix = bloom_add(P, reinterpret_cast<const uint32_t *>(key), b.ulen, b.lcp);
+    }
+    const uint32_t np = (uint32_t)__popc(__ballot_sync(kFull, new_prefix));
+    if (P.out_bloom_lines) { W.n_bloom_keys += b.cnt; W.n_bloom_prefixes += np; }
+}
+// The heads finish the blocks that end in front of them: restart array, count, padding, index entry and index key.
+PGS_DEV void close_blocks(const MergeParams &P, const EmitSeg &S, const EmitWarp &W, const EmitBatch &b)
+{
+    const uint32_t lane = W.lane;
+    const uint32_t first_close = __ffs((int)__ballot_sync(kFull, b.closes)) - 1; // lane of the first closing head (or ~0)
+    // the carried block's earlier restart offsets (from previous batches) go in front of this batch's
+    const bool carried_closes = S.open && first_close < 32;
+    if (carried_closes) {
+        const uint32_t Tc = __shfl_sync(kFull, b.T, (int)first_close);
+        const uint32_t have_r = restart_count(S.blk_n, W.RI); // restart points recorded before this batch
+        const uint32_t ro = (uint32_t)(S.blk_start - b.obase) + Tc;
+        for (uint32_t i = lane; i < 4 * have_r; i += 32) W.obuf[ro + i] = (uint8_t)(W.rst[i >> 2] >> (8 * (i & 3)));
+    }
+    if (b.closes) {
+        const uint32_t bstart = (uint32_t)(S.blk_start - b.obase) + (b.span_incl - b.asz_c); // obuf offset of the block I close
+        uint32_t p = bstart + b.T + 4 * b.nrest_c;
+        W.obuf[p] = (uint8_t)b.nrest_c; W.obuf[p + 1] = (uint8_t)(b.nrest_c >> 8); W.obuf[p + 2] = (uint8_t)(b.nrest_c >> 16); W.obuf[p + 3] = (uint8_t)(b.nrest_c >> 24);
+        for (p += 4; p < bstart + b.asz_c; p++) W.obuf[p] = 0;
+        const uint32_t bi = S.blk_idx + b.nclose_incl - 1;
+        P.out_blk_off[bi] = S.blk_start + (b.span_incl - b.asz_c);
+        P.out_blk_size[bi] = b.size_c;
+        P.out_blk_rec[bi] = b.ph >= 0 ? S.rec_idx + (uint32_t)b.ph : S.blk_rec0;
+        P.out_ikey_off[bi] = S.keyb + b.kb_incl - b.pk_len;
+    }
+    // the closed blocks' index keys: the whole warp copies one key at a time
+    uint32_t cm = __ballot_sync(kFull, b.closes);
+    while (cm) {
+        const int L = __ffs((int)cm) - 1;
+        cm &= cm - 1;
+        const uint32_t klen_b = __shfl_sync(kFull, b.pk_len, L), ko_b = S.keyb + __shfl_sync(kFull, b.kb_incl, L) - klen_b;
+        const uint32_t poff = __shfl_sync(kFull, b.pk_off, L);
+        const uint8_t *pk = L == 0 ? S.ks + S.last_key_off : b.staged + poff; // staged, or the last entry of the batch before
+        for (uint32_t x = lane; x < klen_b; x += 32) P.out_ikeys[ko_b + x] = pk[x];
+    }
+}
+// Carry the state over to the next batch, send the batch's whole 16-byte chunks, move the partial one to the front of obuf.
+PGS_DEV void carry_over(const MergeParams &P, EmitSeg &S, const EmitWarp &W, const EmitBatch &b)
+{
+    const uint32_t lane = W.lane;
+    const uint32_t lastl = b.cnt - 1;
+    const uint32_t l_base = __shfl_sync(kFull, b.base_i, (int)lastl), l_fill = __shfl_sync(kFull, b.fill_i + b.sz, (int)lastl);
+    const uint32_t l_n = __shfl_sync(kFull, b.n_i, (int)lastl) + 1;
+    const int l_h = __shfl_sync(kFull, b.h, (int)lastl);
+    const uint32_t n_closed = (uint32_t)__popc(__ballot_sync(kFull, b.closes));
+    const uint32_t kb_total = __shfl_sync(kFull, b.kb_incl, 31);
+    S.last_key_off = S.kpos + __shfl_sync(kFull, b.key_off_i, (int)lastl);
+    S.last_ulen = __shfl_sync(kFull, b.ulen, (int)lastl);
+    if (l_h >= 0) S.blk_rec0 = S.rec_idx + (uint32_t)l_h;
+    S.blk_start += l_base; S.fill = l_fill; S.blk_n = l_n; S.open = true;
+    S.blk_idx += n_closed; S.keyb += kb_total; S.rec_idx += b.cnt; S.kpos += b.total_s;
+    const unsigned long long wpos = S.blk_start + S.fill;
+    const uint32_t used = (uint32_t)(wpos - b.obase), whole = used & ~15u;
+    flush(P, W, b.obase, whole);
+    S.carry = used - whole;
+    const uint8_t cv = lane < S.carry ? W.obuf[whole + lane] : (uint8_t)0;
+    __syncwarp();
+    if (lane < S.carry) W.obuf[lane] = cv;
+    __syncwarp();
+}
+
 __global__ void __launch_bounds__(kEmitThreads, 5) k_emit(const __grid_constant__ MergeParams P)
 {
     PGS_SMEM_DYN(dyn);
     const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     if (__shfl_sync(kFull, P.stats->error, 0)) return; // the plan or the walk failed: the output is discarded
-    const uint32_t RI = P.restart_interval, OB = P.emit_obuf;
-    uint8_t *ws = dyn + (size_t)warp * P.emit_warp_smem;
-    uint8_t *obuf = ws;                                          // OB + 32 bytes
-    uint8_t *hst = obuf + OB + 32;                               // head_stage + 32 bytes: the key-stream records of a batch
-    uint32_t *rst = (uint32_t *)(hst + P.head_stage + 32);       // restart offsets of the open block (it may span batches)
-    const uint32_t lt = (1u << lane) - 1u;                       // lanes before me
-    uint32_t n_bloom_keys = 0, n_bloom_prefixes = 0;             // lane 0 counts what the warp added to the filter
-
+    EmitWarp W;
+    emit_warp(W, P, dyn + (size_t)warp * P.emit_warp_smem, lane);
     for (;;) {
         uint32_t q = 0;
         if (lane == 0) q = atomicAdd(P.ticket + 1, 1u);
@@ -1105,277 +1466,37 @@ __global__ void __launch_bounds__(kEmitThreads, 5) k_emit(const __grid_constant_
         const SegAgg A = P.agg[q];
         if (A.n_entries == 0) continue;
         const SegBase B = P.base[q];
-        const Desc *desc = P.desc + P.seg[q].desc_off;
-        const uint8_t *heads = P.heads + P.seg[q].head_off;
-        // carried state (warp-uniform)
-        unsigned long long blk_start = B.bytes; // global offset of the open block (of the segment's first block before it opens)
-        uint32_t fill = 0, blk_n = 0, blk_rec0 = B.recs; // entry bytes / entries of the open block, its first record
-        bool open = false;
-        uint32_t blk_idx = B.blocks, rec_idx = B.recs, keyb = B.keyb, hpos = 0, err = 0;
-        uint32_t carry = 0; // obuf[0, carry) = the bytes of the partial 16-byte chunk in front of the write position
-        uint32_t last_key_off = 0, last_ulen = 0; // the previous entry's user key in the key stream (the index key of a block it ends)
-
-        // finish the open block outside a batch (whole warp): restart array (offsets kept in rst), count and padding go to `at`
-        // (where byte `fill` of the block lives: obuf + carry, or global memory for a block written in place), index entry
-        auto close_open = [&](const uint8_t *key, uint32_t klen, uint8_t *at, uint32_t nrest) {
-            const uint32_t size = fill + 4 * (nrest + 1);
-            const uint32_t asz = (size + kBlockAlign - 1) & ~(kBlockAlign - 1);
-            __syncwarp();
-            for (uint32_t i = lane; i < 4 * (nrest + 1); i += 32) {
-                const uint32_t v = (i >> 2) < nrest ? rst[i >> 2] : nrest;
-                at[i] = (uint8_t)(v >> (8 * (i & 3)));
-            }
-            for (uint32_t i = size - fill + lane; i < asz - fill; i += 32) at[i] = 0;
-            if (lane == 0) {
-                P.out_blk_off[blk_idx] = blk_start;
-                P.out_blk_size[blk_idx] = size;
-                P.out_blk_rec[blk_idx] = blk_rec0;
-                P.out_ikey_off[blk_idx] = keyb;
-            }
-            for (uint32_t i = lane; i < klen; i += 32) P.out_ikeys[keyb + i] = key[i];
-            keyb += klen;
-            blk_idx++;
-            blk_start += asz;
-            fill = 0; blk_n = 0; open = false;
-        };
-        // write obuf[0, bytes) to the run at the 16-aligned global offset gpos (bytes % 16 == 0), wait until it has been read
-        auto flush = [&](unsigned long long gpos, uint32_t bytes) {
-            __syncwarp();
-            if (bytes) {
-                fence_proxy_async();
-                __syncwarp();
-                if (lane == 0) { tma_store_1d(P.out_data + gpos, obuf, bytes); tma_store_commit(); tma_store_wait_read0(); }
-                __syncwarp();
-            }
-        };
-        // one thread: the key (and its hash-key prefix when the previous survivor did not share it) goes into the filter
-        auto bloom_add = [&](const uint32_t *key32, uint32_t ulen, uint32_t lcp, bool &new_prefix) {
-            new_prefix = false;
-            if (!P.out_bloom_lines) return;
-            const unsigned long long hk = bloom_hash_words(key32, ulen);
-#pragma unroll
-            for (uint32_t i = 0; i < 6; i++) bloom_add_bit(P.out_bloom, P.out_bloom_lines, hk, i);
-            const uint32_t pl = hashkey_prefix_len((const uint8_t *)key32, ulen);
-            if (pl && lcp < pl) {
-                new_prefix = true;
-                const unsigned long long hp = bloom_hash_words(key32, pl);
-#pragma unroll
-                for (uint32_t i = 0; i < 6; i++) bloom_add_bit(P.out_bloom, P.out_bloom_lines, hp, i);
-            }
-        };
-
+        EmitSeg S;
+        emit_seg(S, P, q, A, B);
+        uint32_t err = 0;
         uint4 dn = make_uint4(0u, 0u, 0u, 0u); // the next batch's descriptors, fetched while this batch's values are copied
         uint32_t dn_e0 = 0xFFFFFFFFu;
-        for (uint32_t e0 = 0; e0 < A.n_entries && !err;) {
-            const uint32_t idx = e0 + lane;
-            Desc d;
-            d.loc = 0; d.vlen = 0; d.aux = 0;
-            if (dn_e0 == e0) *reinterpret_cast<uint4 *>(&d) = dn;
-            else if (idx < A.n_entries) *reinterpret_cast<uint4 *>(&d) = *reinterpret_cast<const uint4 *>(&desc[idx]);
-            const bool have = idx < A.n_entries;
-            const uint32_t fl = (uint32_t)(d.loc >> 60), ulen = (uint32_t)(d.loc >> 44) & 0xffffu, vl = d.vlen, lcp = d.aux;
-            const uint32_t first_fl = __shfl_sync(kFull, fl, 0);
-            if (first_fl & DF_BIG) {
-                // ---- an entry larger than a block buffer: a block of its own, written in place by the whole warp ---------------
-                const unsigned long long loc = __shfl_sync(kFull, d.loc, 0);
-                const uint32_t bvl = __shfl_sync(kFull, vl, 0), bul = __shfl_sync(kFull, ulen, 0), blcp = __shfl_sync(kFull, lcp, 0);
-                const uint32_t bfl = first_fl;
-                const uint32_t *rec = reinterpret_cast<const uint32_t *>(heads + hpos); // its key-stream record, read from global memory
-                const uint32_t fixed = (bfl & DF_REWRITE) ? 12u : 8u;
-                const uint8_t *key = (const uint8_t *)rec + fixed;
-                if (open) { // finish the block in front of it; what that block still has in obuf leaves with it
-                    const unsigned long long obase = blk_start + fill - carry;
-                    close_open(heads + last_key_off, last_ulen, obuf + carry, (blk_n + RI - 1) / RI);
-                    flush(obase, (uint32_t)(blk_start - obase));
-                    carry = 0;
-                }
-                const uint8_t *vsrc = P.runs[(uint32_t)(loc >> 40) & 15u].data + (loc & ((1ull << 40) - 1));
-                uint8_t *o = P.out_data + blk_start;
-                uint32_t hv = 0;
-                if (lane == 0) { // a restart point: nothing shared
-                    hv = put_varint32_s(o, 0u);
-                    hv += put_varint32_s(o + hv, bul + 8);
-                    hv += put_varint32_s(o + hv, bvl);
-                    bool np;
-                    bloom_add(reinterpret_cast<const uint32_t *>(key), bul, blcp, np);
-                    n_bloom_keys += P.out_bloom_lines ? 1u : 0u;
-                    n_bloom_prefixes += np ? 1u : 0u;
-                }
-                hv = __shfl_sync(kFull, hv, 0);
-                const uint32_t bhl = hv + bul + 8;
-                for (uint32_t x = lane; x < bul; x += 32) o[hv + x] = key[x];
-                if (lane < 8) o[hv + bul + lane] = ((const uint8_t *)rec)[lane]; // trailer
-                for (uint32_t x = lane; x < bvl; x += 32) o[bhl + x] = vsrc[x];
-                if ((bfl & DF_REWRITE) && bvl >= 4 && lane < 4) o[bhl + lane] = ((const uint8_t *)rec)[8 + lane];
-                if (lane == 0) { rst[0] = 0; P.out_rec_off[rec_idx] = 0; }
-                fill = bhl + bvl; blk_n = 1; blk_rec0 = rec_idx; open = true;
-                close_open(key, bul, o + fill, 1u); // the block's last user key is this entry's
-                last_key_off = hpos + fixed; last_ulen = bul;
-                rec_idx++; hpos += fixed + ((bul + 3) & ~3u); e0++;
-                continue;
-            }
-            // ---- layout, part 1: block membership and restart points follow from the flags alone ------------------------------------
-            const uint32_t bigmask = __ballot_sync(kFull, have && (fl & DF_BIG));
-            const bool cand = have && !(bigmask & (lt | (1u << lane)));       // before the first oversized entry
-            const uint32_t hm_all = __ballot_sync(kFull, cand && (fl & DF_NEWBLOCK));
-            const uint32_t at_or_before = hm_all & (lt | (1u << lane)), before = hm_all & lt;
-            const int h = at_or_before ? 31 - __clz((int)at_or_before) : -1;  // the block I belong to starts at lane h (-1: the carried block)
-            const int ph = before ? 31 - __clz((int)before) : -1;              // the head before me
-            const uint32_t n_i = h >= 0 ? lane - (uint32_t)h : blk_n + lane;   // my index inside my block
-            const bool is_restart = n_i % RI == 0;
-            const uint32_t sh_out = is_restart ? 0u : (lcp < ulen ? lcp : ulen);
-            const uint32_t kd = ulen - sh_out;
-            const uint32_t hvl = varint_len(sh_out) + varint_len(kd + 8) + varint_len(vl);
-            const uint32_t hl = hvl + kd + 8;
-            // ---- batch = the entries before the first oversized one that fit the output buffer and the stage -------------------------
-            const uint32_t sz = cand ? hl + vl : 0u;
-            const uint32_t sb = cand ? ((fl & DF_REWRITE) ? 12u : 8u) + ((ulen + 3) & ~3u) : 0u; // my key-stream record
-            const uint32_t ps_incl = warp_incl_scan(sz, lane), ss_incl = warp_incl_scan(sb, lane);
-            // room: the entries, the restart arrays and paddings of the blocks that close here (the carried block brings its
-            // earlier restart points along), the carried partial chunk
-            const uint32_t room = carry + 32 * (lane + 1) + 64 + (open ? 4 * ((blk_n + RI - 1) / RI) : 0u);
-            const bool fits = cand && room + ps_incl <= OB && ss_incl <= P.head_stage;
-            const uint32_t cnt = (uint32_t)__popc(__ballot_sync(kFull, fits)); // monotone: lanes 0..cnt-1
-            if (cnt == 0) { err = PGS_ABORTED; break; }
-            const bool mine = lane < cnt;
-            dn_e0 = e0 + cnt;
-            dn = dn_e0 + lane < A.n_entries ? *reinterpret_cast<const uint4 *>(&desc[dn_e0 + lane]) : make_uint4(0u, 0u, 0u, 0u);
-            const uint32_t total_s = __shfl_sync(kFull, ss_incl, (int)cnt - 1);
-            {   // stage the batch's key-stream records
-                const uint8_t *src = heads + hpos;
-                const uint32_t a = (uint32_t)((uintptr_t)src & 15);
-                for (uint32_t i = lane * 16; i < a + total_s; i += 512) async_copy16(hst + i, src - a + i);
-                async_copy_commit();
-            }
-            // ---- layout, part 2: offsets, block starts -------------------------------------------------------------------------------
-            const uint32_t hm = cnt >= 32 ? hm_all : hm_all & ((1u << cnt) - 1u);
-            const bool head = mine && (fl & DF_NEWBLOCK);
-            const uint32_t ps = ps_incl - sz;                                   // entry bytes of the batch before me
-            const uint32_t ps_h = __shfl_sync(kFull, ps, h >= 0 ? h : 0), ps_ph = __shfl_sync(kFull, ps, ph >= 0 ? ph : 0);
-            const uint32_t fill_i = h >= 0 ? ps - ps_h : fill + ps;            // my offset inside my block
-            // a head closes the block before it (if there is one): its entry bytes, entry count, aligned size
-            const bool closes = head && (ph >= 0 || open);
-            const uint32_t T = ph >= 0 ? ps - ps_ph : fill + ps, NN = ph >= 0 ? lane - (uint32_t)ph : blk_n + lane;
-            const uint32_t nrest_c = closes ? (NN + RI - 1) / RI : 0u;
-            const uint32_t size_c = T + 4 * (nrest_c + 1);
-            const uint32_t asz_c = closes ? ((size_c + kBlockAlign - 1) & ~(kBlockAlign - 1)) : 0u;
-            const uint32_t S_incl = warp_incl_scan(asz_c, lane);               // bytes of the blocks closed at or before me
-            const uint32_t S_h = __shfl_sync(kFull, S_incl, h >= 0 ? h : 0);
-            const uint32_t base_i = h >= 0 ? S_h : 0u;                          // start of my block relative to blk_start
-            const uint32_t nclose_incl = (uint32_t)__popc(__ballot_sync(kFull, closes) & (lt | (1u << lane)));
-            // the index key of the block a head closes = the user key of the entry before it
-            const uint32_t rec_off_i = ss_incl - sb;                            // my record inside the stage
-            const uint32_t key_off_i = rec_off_i + ((fl & DF_REWRITE) ? 12u : 8u);
-            const uint32_t pk_off = __shfl_up_sync(kFull, key_off_i, 1), pk_len_l = __shfl_up_sync(kFull, ulen, 1);
-            const uint32_t pk_len = lane == 0 ? last_ulen : pk_len_l;
-            const uint32_t kb_incl = warp_incl_scan(closes ? pk_len : 0u, lane); // index-key bytes of the blocks closed at or before me
-            // obuf[0] corresponds to the global offset obase
-            const unsigned long long obase = blk_start + fill - carry;
-            const uint32_t o_i = (uint32_t)(blk_start + base_i + fill_i - obase); // my entry's offset in obuf
+        for (uint32_t e0 = 0; e0 < S.n && !err;) {
+            EmitBatch b;
+            batch_desc(b, S, W, e0, dn, dn_e0);
+            const uint32_t first_fl = __shfl_sync(kFull, b.fl, 0);
+            if (first_fl & DF_BIG) { emit_big(P, S, W, b, first_fl); e0++; continue; }
+            if (batch_fit(P, S, W, b) == 0) { err = PGS_ABORTED; break; }
+            stage_records(S, W, b, e0, dn, dn_e0);
+            batch_offsets(P, S, W, b);
             async_copy_wait_upto(0);
             __syncwarp();
-            const uint8_t *hs = hst + ((uintptr_t)(heads + hpos) & 15);
-            // ---- restart points ---------------------------------------------------------------------------------------------------------
-            const uint32_t after = hm & ~(lt | (1u << lane));
-            const int nh = after ? __ffs((int)after) - 1 : -1;                   // the head that closes my block inside this batch
-            const uint32_t T_mine = __shfl_sync(kFull, T, nh >= 0 ? nh : 0);    // my block's entry bytes, when it closes here
-            const uint32_t r_i = n_i / RI;
-            if (mine && is_restart) {
-                if (nh >= 0) { // the restart array of my block is assembled in this batch
-                    const uint32_t ro = (uint32_t)(blk_start + base_i - obase) + T_mine + 4 * r_i;
-                    obuf[ro] = (uint8_t)fill_i; obuf[ro + 1] = (uint8_t)(fill_i >> 8); obuf[ro + 2] = (uint8_t)(fill_i >> 16); obuf[ro + 3] = (uint8_t)(fill_i >> 24);
-                } else rst[r_i] = fill_i;
-            }
-            if (mine) P.out_rec_off[rec_idx + lane] = fill_i;
-            // ---- one thread per entry: head, value, filter bits ---------------------------------------------------------------------------
-            bool new_prefix = false;
-            if (mine) {
-                const uint8_t *rec = hs + rec_off_i;
-                const uint8_t *key = hs + key_off_i;
-                uint8_t *dst = obuf + o_i;
-                uint32_t p = put_varint32_s(dst, sh_out);
-                p += put_varint32_s(dst + p, kd + 8);
-                p += put_varint32_s(dst + p, vl);
-                copy_bytes_s2s(dst + p, key + sh_out, kd);
-                copy_bytes_s2s(dst + p + kd, rec, 8u);
-                const RunDev &r = P.runs[(uint32_t)(d.loc >> 40) & 15u];
-                thread_copy_g2s(obuf, o_i + hl, r.data + (d.loc & ((1ull << 40) - 1)), vl, r.data);
-                if ((fl & DF_REWRITE) && vl >= 4) { dst[hl] = rec[8]; dst[hl + 1] = rec[9]; dst[hl + 2] = rec[10]; dst[hl + 3] = rec[11]; }
-                bloom_add(reinterpret_cast<const uint32_t *>(key), ulen, lcp, new_prefix);
-            }
-            {
-                const uint32_t np = (uint32_t)__popc(__ballot_sync(kFull, new_prefix));
-                if (P.out_bloom_lines) { n_bloom_keys += cnt; n_bloom_prefixes += np; }
-            }
+            b.staged = W.stage + ((uintptr_t)(S.ks + S.kpos) & 15);
+            restart_points(P, S, W, b);
+            write_entries(P, W, b);
             __syncwarp();
-            // ---- the heads finish the blocks that end in front of them --------------------------------------------------------------
-            {
-                const uint32_t first_close = __ffs((int)__ballot_sync(kFull, closes)) - 1; // lane of the first closing head (or ~0)
-                // the carried block's earlier restart offsets (from previous batches) go in front of this batch's
-                const bool carried_closes = open && first_close < 32;
-                if (carried_closes) {
-                    const uint32_t Tc = __shfl_sync(kFull, T, (int)first_close);
-                    const uint32_t have_r = (blk_n + RI - 1) / RI; // restart points recorded before this batch
-                    const uint32_t ro = (uint32_t)(blk_start - obase) + Tc;
-                    for (uint32_t i = lane; i < 4 * have_r; i += 32) obuf[ro + i] = (uint8_t)(rst[i >> 2] >> (8 * (i & 3)));
-                }
-                if (closes) {
-                    const uint32_t bstart = (uint32_t)(blk_start - obase) + (S_incl - asz_c); // obuf offset of the block I close
-                    uint32_t p = bstart + T + 4 * nrest_c;
-                    obuf[p] = (uint8_t)nrest_c; obuf[p + 1] = (uint8_t)(nrest_c >> 8); obuf[p + 2] = (uint8_t)(nrest_c >> 16); obuf[p + 3] = (uint8_t)(nrest_c >> 24);
-                    for (p += 4; p < bstart + asz_c; p++) obuf[p] = 0;
-                    const uint32_t bi = blk_idx + nclose_incl - 1;
-                    P.out_blk_off[bi] = blk_start + (S_incl - asz_c);
-                    P.out_blk_size[bi] = size_c;
-                    P.out_blk_rec[bi] = ph >= 0 ? rec_idx + (uint32_t)ph : blk_rec0;
-                    P.out_ikey_off[bi] = keyb + kb_incl - pk_len;
-                }
-                // the closed blocks' index keys (the user key of the entry in front of each closing head): the whole warp copies
-                // one key at a time
-                uint32_t cm = __ballot_sync(kFull, closes);
-                while (cm) {
-                    const int L = __ffs((int)cm) - 1;
-                    cm &= cm - 1;
-                    const uint32_t klen_b = __shfl_sync(kFull, pk_len, L), ko_b = keyb + __shfl_sync(kFull, kb_incl, L) - klen_b;
-                    const uint32_t poff = __shfl_sync(kFull, pk_off, L);
-                    const uint8_t *pk = L == 0 ? heads + last_key_off : hs + poff; // staged, or the last entry of the batch before
-                    for (uint32_t x = lane; x < klen_b; x += 32) P.out_ikeys[ko_b + x] = pk[x];
-                }
-            }
-            // ---- carry the state over, flush ------------------------------------------------------------------------------------------------
-            const uint32_t lastl = cnt - 1;
-            const uint32_t l_base = __shfl_sync(kFull, base_i, (int)lastl), l_fill = __shfl_sync(kFull, fill_i + sz, (int)lastl);
-            const uint32_t l_n = __shfl_sync(kFull, n_i, (int)lastl) + 1;
-            const int l_h = __shfl_sync(kFull, h, (int)lastl);
-            const uint32_t n_closed = (uint32_t)__popc(__ballot_sync(kFull, closes));
-            const uint32_t kb_total = __shfl_sync(kFull, kb_incl, 31);
-            last_key_off = hpos + __shfl_sync(kFull, key_off_i, (int)lastl);
-            last_ulen = __shfl_sync(kFull, ulen, (int)lastl);
-            if (l_h >= 0) blk_rec0 = rec_idx + (uint32_t)l_h;
-            blk_start += l_base; fill = l_fill; blk_n = l_n; open = true;
-            blk_idx += n_closed; keyb += kb_total; rec_idx += cnt; hpos += total_s; e0 += cnt;
-            const unsigned long long wpos = blk_start + fill;
-            const uint32_t used = (uint32_t)(wpos - obase), whole = used & ~15u;
-            flush(obase, whole);
-            carry = used - whole;
-            const uint8_t cv = lane < carry ? obuf[whole + lane] : (uint8_t)0; // the partial chunk moves to the front
-            __syncwarp();
-            if (lane < carry) obuf[lane] = cv;
-            __syncwarp();
+            close_blocks(P, S, W, b);
+            carry_over(P, S, W, b);
+            e0 += b.cnt;
         }
-        if (!err && open) { // the segment's last block
-            const unsigned long long obase = blk_start + fill - carry;
-            close_open(heads + last_key_off, last_ulen, obuf + carry, (blk_n + RI - 1) / RI);
-            flush(obase, (uint32_t)(blk_start - obase));
-            carry = 0;
-        }
-        if (!err && (blk_start != B.bytes + A.out_bytes || blk_idx != B.blocks + A.n_blocks || keyb != B.keyb + A.keyb)) err = PGS_CORRUPTION; // the two passes disagree
+        if (!err && S.open) finish_open(P, S, W); // the segment's last block
+        if (!err && (S.blk_start != B.bytes + A.out_bytes || S.blk_idx != B.blocks + A.n_blocks || S.keyb != B.keyb + A.keyb)) err = PGS_CORRUPTION; // the two passes disagree
         if (err && lane == 0) { atomicMax(&P.stats->error, err); atomicMin(&P.stats->error_seg, q); }
     }
     if (lane == 0) {
         tma_store_wait_all();
-        if (n_bloom_keys) atomicAdd(&P.stats->cnt[EV_BLOOM_KEY], (unsigned long long)n_bloom_keys);
-        if (n_bloom_prefixes) atomicAdd(&P.stats->cnt[EV_BLOOM_PREFIX], (unsigned long long)n_bloom_prefixes);
+        if (W.n_bloom_keys) atomicAdd(&P.stats->cnt[EV_BLOOM_KEY], (unsigned long long)W.n_bloom_keys);
+        if (W.n_bloom_prefixes) atomicAdd(&P.stats->cnt[EV_BLOOM_PREFIX], (unsigned long long)W.n_bloom_prefixes);
     }
 }
 

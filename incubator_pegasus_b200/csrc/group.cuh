@@ -269,9 +269,9 @@ PGS_DEV uint32_t cur_next(const Grp<G> &g, bool en, const RunDev &r, CurState *c
 }
 
 // order of two cursor heads as internal keys: user key ascending, then trailer (seq, type) descending, then run index.
-// Whole warp; by_byte = decided by a differing key byte at dpos (the LCP shortcut of the merge loop relies on that).
+// Whole warp; dpos = the first byte where the user keys differ (their common length when one is a prefix of the other).
 template <uint32_t G>
-PGS_DEV bool head_before(const Grp<G> &g, bool en, const CurState *cs, const uint32_t *rows, uint32_t KSW, uint32_t a, uint32_t b, uint32_t &dpos, bool &by_byte,
+PGS_DEV bool head_before(const Grp<G> &g, bool en, const CurState *cs, const uint32_t *rows, uint32_t KSW, uint32_t a, uint32_t b, uint32_t &dpos,
                          uint32_t from = 0) // from: leading bytes known to be equal
 {
     uint32_t la = 0, lb = 0;
@@ -281,24 +281,22 @@ PGS_DEV bool head_before(const Grp<G> &g, bool en, const CurState *cs, const uin
         const uint32_t ah = cs[a].kp_hi, al = cs[a].kp_lo, bh = cs[b].kp_hi, bl = cs[b].kp_lo;
         if ((ah != bh || al != bl) && la >= 8 && lb >= 8) {
             dpos = ah != bh ? (uint32_t)__clz((int)(ah ^ bh)) >> 3 : 4 + ((uint32_t)__clz((int)(al ^ bl)) >> 3);
-            by_byte = true;
             full = false;
         }
     }
     if (!g.any(full)) {
-        if (!en) { by_byte = false; return false; }
+        if (!en) return false;
         const uint32_t ah = cs[a].kp_hi, bh = cs[b].kp_hi;
         return ah != bh ? ah < bh : cs[a].kp_lo < cs[b].kp_lo;
     }
     uint32_t dfull = 0;
     const int c = row_cmp(g, full, rows + a * KSW, la, rows + b * KSW, lb, dfull, from);
-    if (!en) { by_byte = false; return false; }
+    if (!en) return false;
     if (!full) {
         const uint32_t ah = cs[a].kp_hi, bh = cs[b].kp_hi;
         return ah != bh ? ah < bh : cs[a].kp_lo < cs[b].kp_lo;
     }
     dpos = dfull;
-    by_byte = c != 0 && dpos < (la < lb ? la : lb);
     if (c) return c < 0;
     const unsigned long long ta = cur_trailer(&cs[a]), tb = cur_trailer(&cs[b]);
     if (ta != tb) return ta > tb;
