@@ -15,8 +15,10 @@
 //                 segment budget become segment boundaries: segment q = user keys in (U_q, U_q+1], a contiguous
 //                 block range per run.  All versions of a user key fall into one segment.
 //   k_walk        the merge itself.  A *group* of G lanes (4 by default, 1 to 16) owns one segment and walks it
-//                 sequentially like RocksDB's MergingIterator + CompactionIterator: one cursor per run decoding entries
-//                 straight from HBM (group.cuh), the current keys in shared-memory rows compared with one ballot, newest
+//                 sequentially like RocksDB's MergingIterator + CompactionIterator: one cursor per run, whose next entry's
+//                 head (header, key delta, trailer, expire_ts) is fetched into a 96-byte shared-memory window while the
+//                 current one is handled, in the same block or across into the next (group.cuh, kHeadWin), so a merge step
+//                 waits for no global load of its own; the current keys in shared-memory rows compared with one ballot, newest
 //                 version wins, tombstone / bottommost rules, Filter() per surviving value, prefix compression against the
 //                 previous survivor, 4 KB block cuts.  It copies no values: per survivor it emits a 16-byte descriptor
 //                 (where the value lives, lengths, flags) and a key-stream record (trailer | rewritten expire_ts | user key).
@@ -209,6 +211,14 @@ struct WalkCtaStats { // k_walk's per-CTA totals, shared memory
 };
 // k_walk's CTA-wide shared memory in front of the groups': crc table (2 KB), run table, WalkCtaStats
 constexpr uint32_t kWalkFixedSmem = 2048 + kMaxRuns * (uint32_t)sizeof(RunDev) + (uint32_t)sizeof(WalkCtaStats);
+// Behind the groups' states and key rows: each group's head windows (group.cuh, kHeadWin), one per run, 16-aligned.  The
+// extra 16 bytes per group put the windows of the groups of a warp in different banks.
+PGS_HD uint32_t walk_win_stride(uint32_t k) { return k * kHeadWin + 16; }
+PGS_HD uint32_t walk_win_off(uint32_t G, uint32_t group_smem) { return (kWalkFixedSmem + (kWalkThreads / G) * group_smem + 15) & ~15u; }
+PGS_HD uint64_t walk_dyn_smem(uint32_t G, uint32_t group_smem, uint32_t k)
+{
+    return walk_win_off(G, group_smem) + (uint64_t)(kWalkThreads / G) * walk_win_stride(k);
+}
 // fills the derived fields of P (P.k, P.block_size, P.restart_interval must be set); false = not supported
 constexpr uint32_t kWalkMinG = 4; // default lanes per merge group (see group.cuh)
 // walk_groups = merge groups the device runs at the same time (0: not known yet, the default segment budget is used)
@@ -226,13 +236,13 @@ inline bool compact_geometry(MergeParams &P, const CompactTotals &T, uint32_t ma
     // lanes per group: the narrowest shape whose CTA fits shared memory twice per SM (or once); force_G overrides (diagnostics)
     geo.G = 0;
     for (uint32_t G = force_G ? force_G : kWalkMinG; G <= 16 && !geo.G; G *= 2) {
-        const uint64_t dyn = kWalkFixedSmem + (uint64_t)(kWalkThreads / G) * P.group_smem;
+        const uint64_t dyn = walk_dyn_smem(G, P.group_smem, k);
         if (dyn <= max_smem / 2 || (force_G && dyn <= max_smem)) geo.G = G;
     }
     for (uint32_t G = kWalkMinG; G <= 16 && !geo.G; G *= 2)
-        if (kWalkFixedSmem + (uint64_t)(kWalkThreads / G) * P.group_smem <= max_smem) geo.G = G;
+        if (walk_dyn_smem(G, P.group_smem, k) <= max_smem) geo.G = G;
     if (!geo.G) return false;
-    geo.walk_dyn = kWalkFixedSmem + (kWalkThreads / geo.G) * P.group_smem;
+    geo.walk_dyn = (uint32_t)walk_dyn_smem(geo.G, P.group_smem, k);
     const uint32_t hs = (2 * P.KS + 64 + 15) & ~15u;
     P.ks_stage = hs < 2048 ? 2048u : hs;
     // k_emit per warp: an output assembly buffer (at least one block, normally 8 KB = a batch of ~28 entries), the key-stream
@@ -608,7 +618,7 @@ PGS_DEV unsigned long long adj_head_to(unsigned long long a, uint32_t pos, uint3
 // executed by all 32 lanes; `act` marks the groups that still have records.
 template <uint32_t G>
 PGS_DEV void walk_segment(const MergeParams &P, const RunDev *runs, const Grp<G> &g, bool seg_en, uint32_t q, CurState *cs, uint32_t *rows,
-                          const unsigned long long *crc, WalkAcc &acc, WalkCtaStats *cta)
+                          uint8_t *wins, const unsigned long long *crc, WalkAcc &acc, WalkCtaStats *cta)
 {
     const uint32_t k = P.k, KS = P.KS, KSW = P.KSW, RI = P.restart_interval, BS = P.block_size;
     uint32_t *rowA = rows + k * KSW, *rowB = rowA + KSW, *rowLO = rowB + KSW, *rowHI = rowLO + KSW;
@@ -645,7 +655,7 @@ PGS_DEV void walk_segment(const MergeParams &P, const RunDev *runs, const Grp<G>
         if (en && !seg_slice(P, q, j, lo, hi_ex, chk)) err = PGS_ABORTED;
         CurState *C = &cs[j];
         uint32_t *row = rows + j * KSW;
-        const uint32_t e1 = cur_open(g, en && !err, runs[j], C, row, KS, lo, hi_ex, chk);
+        const uint32_t e1 = cur_open<G, true>(g, en && !err, runs[j], C, row, KS, lo, hi_ex, chk, wins + j * kHeadWin);
         if (en && !err) err = e1;
 #pragma unroll 1
         for (;;) { // records at or below U_lo belong to the previous segment
@@ -653,7 +663,7 @@ PGS_DEV void walk_segment(const MergeParams &P, const RunDev *runs, const Grp<G>
             const int c = row_cmp(g, sk, row, sk ? C->klen - 8 : 0u, rowLO, ulo_len, dpos);
             const bool more = sk && c <= 0;
             if (!g.any(more)) break;
-            const uint32_t e2 = cur_next(g, more, runs[j], C, row, KS);
+            const uint32_t e2 = cur_next<G, true>(g, more, runs[j], C, row, KS, wins + j * kHeadWin);
             if (more) err = e2;
         }
         const bool hi = seg_en && !err && C->live && !last && C->b >= C->chk_from;
@@ -844,7 +854,7 @@ PGS_DEV void walk_segment(const MergeParams &P, const RunDev *runs, const Grp<G>
         last_run = c;
         g.sync();
         // (4) advance the cursor and restore the merge order
-        const uint32_t e3 = cur_next(g, act && !err, runs[c], C, row, KS);
+        const uint32_t e3 = cur_next<G, true>(g, act && !err, runs[c], C, row, KS, wins + c * kHeadWin);
         if (act && !err) err = e3;
         const bool adv = act && !err;
         bool alive = adv && C->live != 0;
@@ -945,9 +955,11 @@ __global__ void __launch_bounds__(kWalkThreads, 4) k_walk(const __grid_constant_
     for (uint32_t i = threadIdx.x; i < kMaxRuns; i += blockDim.x) runs[i] = P.runs[i < P.k ? i : 0];
     for (uint32_t i = threadIdx.x; i < sizeof(WalkCtaStats) / 4; i += blockDim.x) ((uint32_t *)cta)[i] = 0;
     if (__syncthreads_or(P.stats->error != 0)) return; // the planner rejected the layout: the output is discarded
-    uint8_t *gs = dyn + kWalkFixedSmem + (size_t)(warp * NGW + g.shift / G) * P.group_smem;
+    const uint32_t gi = warp * NGW + g.shift / G; // the group inside the CTA
+    uint8_t *gs = dyn + kWalkFixedSmem + (size_t)gi * P.group_smem;
     CurState *cs = (CurState *)gs;
     uint32_t *rows = (uint32_t *)(gs + (size_t)P.k * sizeof(CurState));
+    uint8_t *wins = dyn + walk_win_off(G, P.group_smem) + (size_t)gi * walk_win_stride(P.k);
     WalkAcc acc;
     acc.e0 = acc.e1 = acc.e2 = acc.n = 0;
     acc.b_in = acc.b_key = acc.b_val = 0;
@@ -960,7 +972,7 @@ __global__ void __launch_bounds__(kWalkThreads, 4) k_walk(const __grid_constant_
         t0 = __shfl_sync(kFull, t0, 0);
         if (t0 >= P.Q) break;
         const uint32_t q = t0 + g.shift / G;
-        walk_segment<G>(P, runs, g, q < P.Q, q < P.Q ? q : 0u, cs, rows, crc, acc, cta);
+        walk_segment<G>(P, runs, g, q < P.Q, q < P.Q ? q : 0u, cs, rows, wins, crc, acc, cta);
     }
     // statistics: group -> CTA (shared-memory atomics) -> MergeStats
     acc_flush_events(acc, cta, g.gl == 0);

@@ -85,9 +85,10 @@ PGS_DEV int row_cmp(const Grp<G> &g, bool en, const uint32_t *a, uint32_t la, co
 }
 
 // ---- sequential cursor over the blocks of one HBM-resident run ------------------------------------------------------------
-// Group-uniform state of one cursor, in shared memory.  The cursor reads entries straight from global memory: one
-// dependent round trip per entry (the header), everything else of the entry's head lies in the same or the next cache line.
-// Latency is hidden by the number of groups in flight, not by staging.
+// Group-uniform state of one cursor, in shared memory.  The read kernels' cursors read entries straight from global memory:
+// one dependent round trip per entry (the header), everything else of the entry's head lies in the same or the next cache
+// line; latency is hidden by the number of groups in flight.  The compaction walker stages each next entry's whole head in
+// a window instead (kHeadWin below).
 struct CurState { // 32-bit fields only: any 4-byte-aligned stride between the states of neighbouring groups works
     uint32_t base_lo, base_hi; // blk_off[b]
     uint32_t nb_lo, nb_hi;     // blk_off[b + 1], fetched asynchronously when block b was entered
@@ -107,6 +108,7 @@ struct CurState { // 32-bit fields only: any 4-byte-aligned stride between the s
     uint32_t hi_lcp;           // compaction walker: bytes the key shares with the range's upper bound (0x80000000: not known)
     uint32_t hw0, hw1, hw2;    // the aligned words that hold the NEXT entry's first eight bytes (its header), fetched
     uint32_t hvalid;           // asynchronously when this entry was decoded; hvalid = there is such an entry and it was fetched
+                               // (the compaction walker leaves hw0..hw2 unused: hvalid = its head window holds the next entry)
 };
 PGS_DEV unsigned long long cur_trailer(const CurState *c) { return ((unsigned long long)c->tr_hi << 32) | c->tr_lo; }
 PGS_DEV unsigned long long cur_base(const CurState *c) { return ((unsigned long long)c->base_hi << 32) | c->base_lo; }
@@ -146,12 +148,22 @@ PGS_DEV void ld_2x32_any(const uint8_t *p, uint32_t &lo, uint32_t &hi)
     hi = __funnelshift_r(w1, w2, sh);
 }
 
+// The compaction walker's head window (Win = true below): one 16-aligned window of kHeadWin bytes per cursor in shared memory.
+// When an entry is decoded, the window starting at the 16-byte boundary in front of the NEXT entry of the cursor -- in the same
+// block, or the first entry of the next block once that block's metadata is in -- is fetched with 16-byte asynchronous copies
+// spread over the group's lanes.  The next decode then reads the header, the key delta, the trailer and the first four value
+// bytes from shared memory whenever they lie inside the window, so a merge step waits for no global load of its own: restart
+// points with keys of up to ~60 bytes fit, longer heads and multi-byte varint headers take the global path.  A window reaches
+// at most kHeadWin - 1 bytes past the start of an entry that lies inside a block, which stays inside a run's 256 bytes of slack.
+constexpr uint32_t kHeadWin = 96;
+
 // decode the entry at (base, p) of the current block into the state and the key row (groups with en).  prev_klen = internal-
 // key length of the previous entry of the block (0 at a block start: the entry must then be a restart point).
-// Executed by the whole warp (two warp barriers inside).  Returns 0 or a status.
-template <uint32_t G>
+// Win: win = the cursor's head window; stashed = it holds this entry's head.  Otherwise stashed = hw0..hw2 hold its header.
+// Executed by the whole warp (two warp barriers inside, three with Win).  Returns 0 or a status.
+template <uint32_t G, bool Win = false>
 PGS_DEV uint32_t cur_decode(const Grp<G> &g, bool en, const RunDev &r, CurState *c, uint32_t *row, uint32_t KS, unsigned long long base,
-                            uint32_t p, uint32_t blk_size, uint32_t prev_klen, uint32_t rem_new, bool stashed = false)
+                            uint32_t p, uint32_t blk_size, uint32_t prev_klen, uint32_t rem_new, bool stashed = false, uint8_t *win = nullptr)
 {
     uint32_t err = 0, sh = 0, ns = 0, vl = 0, h = 0, klen = 0;
     const uint8_t *src = nullptr;
@@ -159,7 +171,11 @@ PGS_DEV uint32_t cur_decode(const Grp<G> &g, bool en, const RunDev &r, CurState 
     if (en) {
         A = r.data + base + p;
         uint32_t h_lo, h_hi;
-        if (stashed) { // the header words arrived while the previous entry was being handled
+        const uint8_t *S = A; // where the head's bytes are read: global memory, or the same bytes in the window
+        if constexpr (Win) {
+            if (stashed) S = win + ((uintptr_t)A & 15);
+            ld_2x32_any(S, h_lo, h_hi);
+        } else if (stashed) { // the header words arrived while the previous entry was being handled
             const uint32_t s8 = (uint32_t)((uintptr_t)A & 3) * 8, w0 = c->hw0, w1 = c->hw1, w2 = c->hw2;
             h_lo = __funnelshift_r(w0, w1, s8);
             h_hi = __funnelshift_r(w1, w2, s8);
@@ -174,6 +190,8 @@ PGS_DEV uint32_t cur_decode(const Grp<G> &g, bool en, const RunDev &r, CurState 
         if (!err) {
             // key bytes [sh, sh + ns) <- the entry's delta; lane L owns the words L, L + G, ... of the row
             src = A + h;
+            // from the window when every word read below (delta, trailer, expire_ts) ends inside it
+            if constexpr (Win) if (S != A && ((uint32_t)((uintptr_t)A & 15) + h + ns + 8 <= kHeadWin)) src = S + h;
             const uint32_t end = sh + ns;
 #pragma unroll 1
             for (uint32_t w = (sh >> 2) + g.gl; 4 * w < end; w += G) {
@@ -187,6 +205,16 @@ PGS_DEV uint32_t cur_decode(const Grp<G> &g, bool en, const RunDev &r, CurState 
         }
     }
     g.sync();
+    // Win: where the next entry of the cursor starts (nullptr: no window is fetched for it).  Past the last entry of the block it
+    // is the next block's first entry, when that block is in the cursor's range and its metadata arrived (it was requested
+    // when this block was entered, so not yet when this is the block's first entry).
+    const uint8_t *nx = nullptr;
+    if constexpr (Win) {
+        if (en && !err) {
+            if (rem_new >= 2) nx = A + h + ns + vl;
+            else if (p != 0 && c->b + 1 < c->b_end && c->b + 1 < r.nb) nx = r.data + (((unsigned long long)c->nb_hi << 32) | c->nb_lo);
+        }
+    }
     if (en && !err) {
         uint32_t tr_lo, tr_hi;
         if (ns >= 8) ld_2x32_any(src + ns - 8, tr_lo, tr_hi);
@@ -195,7 +223,8 @@ PGS_DEV uint32_t cur_decode(const Grp<G> &g, bool en, const RunDev &r, CurState 
         if (g.gl == 0) {
             c->p = p; c->elen = h + ns + vl; c->klen = klen; c->vlen = vl; c->voff = p + h + ns; c->shared = sh; c->ets_le = ets;
             c->rem = rem_new;
-            c->hvalid = rem_new >= 2 ? 1u : 0u;
+            if constexpr (Win) c->hvalid = nx ? 1u : 0u;
+            else c->hvalid = rem_new >= 2 ? 1u : 0u;
             c->tr_lo = tr_lo; c->tr_hi = tr_hi;
             if (sh < 8) { // the leading bytes changed
                 const uint32_t ul = klen - 8;
@@ -205,10 +234,18 @@ PGS_DEV uint32_t cur_decode(const Grp<G> &g, bool en, const RunDev &r, CurState 
                 c->kp_hi = __byte_perm(w0, 0, 0x0123); c->kp_lo = __byte_perm(w1, 0, 0x0123);
             }
         }
-        if (rem_new >= 2) { // the next entry of the block: start fetching its header words (consumed by the next cur_next)
+        if (!Win && rem_new >= 2) { // the next entry of the block: start fetching its header words (consumed by the next cur_next)
             const uint32_t *nw = reinterpret_cast<const uint32_t *>((uintptr_t)(A + h + ns + vl) & ~(uintptr_t)3);
 #pragma unroll
             for (uint32_t i = g.gl; i < 3; i += G) async_copy4(i == 0 ? &c->hw0 : i == 1 ? &c->hw1 : &c->hw2, nw + i);
+        }
+    }
+    if constexpr (Win) {
+        g.sync(); // every lane has read this entry's head from the window
+        if (nx) {
+            const uint8_t *w0 = (const uint8_t *)((uintptr_t)nx & ~(uintptr_t)15);
+#pragma unroll
+            for (uint32_t i = g.gl; i < kHeadWin / 16; i += G) async_copy16(win + 16 * i, w0 + 16 * i);
         }
     }
     async_copy_commit();
@@ -217,9 +254,11 @@ PGS_DEV uint32_t cur_decode(const Grp<G> &g, bool en, const RunDev &r, CurState 
 }
 
 // position the cursor on the first entry of block b (or leave it exhausted when b >= b_end); synchronous metadata loads
-template <uint32_t G>
-PGS_DEV uint32_t cur_open(const Grp<G> &g, bool en, const RunDev &r, CurState *c, uint32_t *row, uint32_t KS, uint32_t b, uint32_t b_end, uint32_t chk_from)
+template <uint32_t G, bool Win = false>
+PGS_DEV uint32_t cur_open(const Grp<G> &g, bool en, const RunDev &r, CurState *c, uint32_t *row, uint32_t KS, uint32_t b, uint32_t b_end, uint32_t chk_from,
+                          uint8_t *win = nullptr)
 {
+    if constexpr (Win) async_copy_wait_all(); // a window or metadata fetched for the cursor's previous range lands before the new ones start
     const bool some = en && b < b_end && b < r.nb;
     unsigned long long base = 0;
     uint32_t r0 = 0, r1 = 0, bsize = 0;
@@ -231,14 +270,15 @@ PGS_DEV uint32_t cur_open(const Grp<G> &g, bool en, const RunDev &r, CurState *c
     g.sync();
     cur_prefetch_next(g, some, r, c, b);
     const uint32_t err = some && r1 <= r0 ? (uint32_t)PGS_CORRUPTION : 0u; // a block holds at least one entry
-    const uint32_t e2 = cur_decode(g, some && !err, r, c, row, KS, base, 0, bsize, 0, r1 - r0);
+    const uint32_t e2 = cur_decode<G, Win>(g, some && !err, r, c, row, KS, base, 0, bsize, 0, r1 - r0, false, win);
     return err ? err : e2;
 }
 
 // advance to the next entry (groups with en); crossing into the next block uses the metadata fetched when the current block
 // was entered.  Leaves live = 0 when the range is exhausted.  Executed by the whole warp.  Returns 0 or a status.
-template <uint32_t G>
-PGS_DEV uint32_t cur_next(const Grp<G> &g, bool en, const RunDev &r, CurState *c, uint32_t *row, uint32_t KS)
+// Win: win = the cursor's head window (see kHeadWin), which then also serves the first entry of the next block.
+template <uint32_t G, bool Win = false>
+PGS_DEV uint32_t cur_next(const Grp<G> &g, bool en, const RunDev &r, CurState *c, uint32_t *row, uint32_t KS, uint8_t *win = nullptr)
 {
     uint32_t rem = 0, b = 0, p = 0, prev_klen = 0, bsize = 0;
     unsigned long long base = 0;
@@ -248,9 +288,9 @@ PGS_DEV uint32_t cur_next(const Grp<G> &g, bool en, const RunDev &r, CurState *c
         in_block = rem > 1;
         if (in_block) { base = cur_base(c); p = c->p + c->elen; prev_klen = c->klen; bsize = c->bsize; stashed = c->hvalid != 0; }
         else if (b + 1 >= c->b_end || b + 1 >= r.nb) done = true;
-        else cross = true;
+        else { cross = true; stashed = Win && c->hvalid != 0; }
     }
-    async_copy_wait_all(); // the header words fetched when the current entry was decoded (and, long ago, the next block's metadata)
+    async_copy_wait_all(); // the header words or head window fetched when the current entry was decoded (and, long ago, the next block's metadata)
     g.sync(); // every lane is done with the old key row and state, and sees the fetched words
     uint32_t r0 = 0, r1 = 0;
     if (g.any(cross || done)) { // a block boundary (about one step in thirteen)
@@ -264,7 +304,8 @@ PGS_DEV uint32_t cur_next(const Grp<G> &g, bool en, const RunDev &r, CurState *c
         cur_prefetch_next(g, cross, r, c, b + 1);
     }
     const uint32_t err = cross && r1 <= r0 ? (uint32_t)PGS_CORRUPTION : 0u;
-    const uint32_t e2 = cur_decode(g, (in_block || cross) && !err, r, c, row, KS, base, p, bsize, prev_klen, in_block ? rem - 1 : r1 - r0, stashed);
+    const uint32_t e2 = cur_decode<G, Win>(g, (in_block || cross) && !err, r, c, row, KS, base, p, bsize, prev_klen, in_block ? rem - 1 : r1 - r0,
+                                           stashed, win);
     return err ? err : e2;
 }
 
