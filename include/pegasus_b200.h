@@ -393,6 +393,11 @@ typedef struct {
     uint8_t prefix_filter;                         /* rocksdb_filter_type == "prefix" (default 1) */
     uint8_t cluster_id;                            /* timetag cluster id, default 1           */
     uint8_t reserved[6];
+    /* hot-key detection (hotkey_collector.cpp:38-75); pgs_rrdb_start rejects a bucket count that is not a prime >= 3 */
+    uint32_t hotkey_buckets_num;                   /* 0 -> 37                                 */
+    uint32_t hot_bucket_variance_threshold;        /* 0 -> 7                                  */
+    uint32_t hot_key_variance_threshold;           /* 0 -> 5                                  */
+    uint32_t max_seconds_to_detect_hotkey;         /* 0 -> 150                                */
 } pgs_server_options;
 
 /* replication_app_base::open/start: creates the partition on `e`, data version 1
@@ -578,6 +583,25 @@ PGS_API int32_t pgs_rrdb_apply_checkpoint(pgs_server *s, const char *checkpoint_
 /* drops scan contexts older than 5 minutes (pegasus_server_impl.cpp:1377-1385 schedules the same expiry per context);
  * also runs implicitly on every scanner call. Returns the number of contexts dropped. */
 PGS_API uint32_t pgs_rrdb_gc(pgs_server *s, uint32_t now);
+
+/* on_detect_hotkey (pegasus_server_impl.cpp:3544-3566, hotkey_collector.cpp): the READ and WRITE hot-key collectors of the
+ * replica.  START moves a STOPPED collector to COARSE_DETECTING; STOP clears it; QUERY returns the hot hash key once the
+ * collector is FINISHED.  Returns a PGS_HOTKEY_ outcome; result_buf receives up to cap bytes of the hint, or of the hot hash
+ * key of a successful QUERY, and *result_len its whole length.  Captures follow capacity_unit_calculator.cpp:158-403: reads
+ * answered by the memtable and the handlers' own weights on the host, the misses of batched gets on the device
+ * (k_hotkey_capture, next to k_get, only while the READ collector is active); scans capture nothing.  The collectors live on
+ * the replica's partition, so pgs_get_batch / pgs_get_batch_multi / pgs_batcher_get on pgs_rrdb_partition(s) capture too. */
+enum { PGS_HOTKEY_READ = 0, PGS_HOTKEY_WRITE = 1 };
+enum { PGS_HOTKEY_START = 0, PGS_HOTKEY_STOP = 1, PGS_HOTKEY_QUERY = 2 };
+enum { PGS_HOTKEY_OK = 0, PGS_HOTKEY_BUSY = 1, PGS_HOTKEY_INVALID_STATE = 2, PGS_HOTKEY_INVALID_PARAMETERS = 3 };
+enum { PGS_HOTKEY_STOPPED = 0, PGS_HOTKEY_COARSE_DETECTING = 1, PGS_HOTKEY_FINE_DETECTING = 2, PGS_HOTKEY_FINISHED = 3 };
+PGS_API int32_t pgs_rrdb_detect_hotkey(pgs_server *s, int32_t type, int32_t action, uint32_t now_s, char *result_buf,
+                                       uint32_t cap, uint32_t *result_len);
+/* one analysis step of both collectors at now_s (hotkey_collector::analyse_data); the library owns no threads, so the
+ * binding calls it every hotkey_analyse_time_interval_s (10 s), like pgs_rrdb_gc.  Returns a status code. */
+PGS_API int32_t pgs_rrdb_hotkey_analyse(pgs_server *s, uint32_t now_s);
+/* a collector's PGS_HOTKEY_ state (-1: invalid type) */
+PGS_API int32_t pgs_rrdb_hotkey_state(pgs_server *s, int32_t type);
 
 /* ============================================================================================
  * 7. box-level placement: one engine per visible GPU

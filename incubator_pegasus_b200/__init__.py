@@ -111,7 +111,8 @@ class ServerOptions(C.Structure):
                 ("rocksdb_multi_get_max_iteration_count", C.c_uint32),
                 ("rocksdb_multi_get_max_iteration_size", C.c_uint64), ("l0_compaction_trigger", C.c_uint32),
                 ("memtable_bytes", C.c_uint64), ("prefix_filter", C.c_uint8), ("cluster_id", C.c_uint8),
-                ("reserved", C.c_uint8 * 6)]
+                ("reserved", C.c_uint8 * 6), ("hotkey_buckets_num", C.c_uint32), ("hot_bucket_variance_threshold", C.c_uint32),
+                ("hot_key_variance_threshold", C.c_uint32), ("max_seconds_to_detect_hotkey", C.c_uint32)]
 
 
 class Response(C.Structure):
@@ -234,6 +235,9 @@ def lib() -> C.CDLL:
         "pgs_rrdb_multi_remove": [vp, Blob, C.POINTER(Blob), C.c_uint32, C.c_int64, C.POINTER(C.c_int64), C.c_uint32],
         "pgs_rrdb_flush": [vp, C.c_uint32],
         "pgs_rrdb_manual_compact": [vp, C.c_uint32, C.POINTER(CompactResult)],
+        "pgs_rrdb_detect_hotkey": [vp, C.c_int32, C.c_int32, C.c_uint32, C.c_char_p, C.c_uint32, u32p],
+        "pgs_rrdb_hotkey_analyse": [vp, C.c_uint32],
+        "pgs_rrdb_hotkey_state": [vp, C.c_int32],
     }.items():
         if hasattr(L, name):
             getattr(L, name).argtypes = args
@@ -513,6 +517,33 @@ def manual_compact_state_check(now_ms: int, last_finish_ms: int, min_interval_s:
     f.argtypes = [C.c_uint64, C.c_uint64, C.c_int32, C.POINTER(C.c_uint64)]
     ok = f(now_ms, last_finish_ms, min_interval_s, C.byref(e))
     return bool(ok), e.value
+
+
+HOTKEY_READ, HOTKEY_WRITE = 0, 1
+HOTKEY_START, HOTKEY_STOP, HOTKEY_QUERY = 0, 1, 2
+HOTKEY_OK, HOTKEY_BUSY, HOTKEY_INVALID_STATE, HOTKEY_INVALID_PARAMETERS = 0, 1, 2, 3
+HOTKEY_STOPPED, HOTKEY_COARSE_DETECTING, HOTKEY_FINE_DETECTING, HOTKEY_FINISHED = 0, 1, 2, 3
+
+
+def detect_hotkey(server, hotkey_type: int, action: int, now_s: int):
+    """pgs_rrdb_detect_hotkey on a pgs_server handle -> (outcome, hint or hot hash key as bytes)"""
+    L = lib()
+    n = C.c_uint32(0)
+    buf = C.create_string_buffer(4096)
+    out = L.pgs_rrdb_detect_hotkey(server, hotkey_type, action, now_s, buf, len(buf), C.byref(n))
+    if n.value > len(buf):
+        buf = C.create_string_buffer(n.value)
+        out = L.pgs_rrdb_detect_hotkey(server, hotkey_type, HOTKEY_QUERY, now_s, buf, len(buf), C.byref(n)) if action == HOTKEY_QUERY else out
+    return int(out), buf.raw[:n.value]
+
+
+def hotkey_analyse(server, now_s: int) -> None:
+    """pgs_rrdb_hotkey_analyse: one analysis step of both collectors of a pgs_server handle (the binding's 10 s timer)"""
+    _check(lib().pgs_rrdb_hotkey_analyse(server, now_s), "rrdb_hotkey_analyse")
+
+
+def hotkey_state(server, hotkey_type: int) -> int:
+    return int(lib().pgs_rrdb_hotkey_state(server, hotkey_type))
 
 
 def partition_index(hash_key: bytes, sort_key: bytes, partition_count: int) -> int:

@@ -6,11 +6,13 @@
 #include <cstdint>
 #include <memory>
 #include <mutex>
+#include <shared_mutex>
 #include <string>
 #include <type_traits>
 #include <vector>
 
 #include "../../include/pegasus_b200.h"
+#include "../host/hotkey.h"
 #include "format.h"
 
 namespace pgs {
@@ -88,7 +90,23 @@ struct Partition {
     std::vector<std::shared_ptr<Run>> runs; // read order: L0 newest first, then L1, L2 ...
     std::shared_ptr<Run> find(uint64_t id);
     void insert(std::shared_ptr<Run> r);
+    // hot-key collectors of the replica (host/hotkey.h).  The READ collector's coarse counters of batched gets live in HBM
+    // (hk_dev_buckets, hk_dev_n of them, allocated at the first capturing launch); a capturing launch holds hk_dev_mu shared
+    // from its launch to the hand-over of its fine captures, analysis and STOP hold it exclusively, so no capture is lost
+    // between reading the counters and zeroing them.
+    HotkeyCollector hk_read{HOTKEY_READ}, hk_write{HOTKEY_WRITE};
+    std::shared_mutex hk_dev_mu;
+    unsigned long long *hk_dev_buckets = nullptr;
+    uint32_t hk_dev_n = 0;
+    ~Partition();
 };
+
+// the device half of the READ collector (lookup.cu): analysis and STOP of a partition's collectors, with its HBM counters
+int32_t hotkey_analyse(Partition &p, uint32_t now);
+int32_t hotkey_control(Partition &p, int32_t type, int32_t action, uint32_t now, std::string &text);
+// pgs_get_batch; capture = false leaves the READ collector to the caller
+int32_t get_batch(pgs_partition *ph, const uint8_t *keys, const uint32_t *key_off, uint32_t n, uint32_t now, uint8_t *arena,
+                  uint64_t arena_cap, pgs_get_result *results, uint64_t *arena_used, bool capture);
 
 void set_error(const char *fmt, ...);
 int32_t cuda_fail(cudaError_t e, const char *what);

@@ -65,6 +65,33 @@ PGS_HD uint64_t pegasus_key_hash(const T *table, const uint8_t *key, uint32_t le
     return ~c;
 }
 
+// Bucket hash of the hot-key collectors (host/hotkey.h, hotkey_kernels.cuh): it only decides which hash keys share a coarse
+// bucket, never which key is reported.  Not crc64: every key of a partition has the same crc64 % partition_count, so crc64
+// buckets would be correlated with the partition.  The hash is a sum of independently mixed 32-bit words (word j = bytes
+// 4j..4j+3 little endian, zero padded past the end, mixed with its index), so that the lanes of a group can each hash some
+// words of a long key and add their partial sums.
+PGS_HD uint32_t hotkey_word(const uint8_t *p, uint32_t len, uint32_t j)
+{
+    uint32_t w = 0;
+    for (uint32_t b = 0; b < 4 && 4 * j + b < len; b++) w |= (uint32_t)p[4 * j + b] << (8 * b);
+    return w;
+}
+PGS_HD uint64_t hotkey_mix(uint64_t x)
+{
+    x ^= x >> 30; x *= 0xBF58476D1CE4E5B9ull;
+    x ^= x >> 27; x *= 0x94D049BB133111EBull;
+    return x ^ (x >> 31);
+}
+PGS_HD uint64_t hotkey_word_hash(uint32_t w, uint32_t j) { return hotkey_mix(((uint64_t)j << 32 | w) + 0x9E3779B97F4A7C15ull); }
+PGS_HD uint64_t hotkey_finish(uint64_t sum, uint32_t len) { return hotkey_mix(sum ^ ((uint64_t)len * 0xD6E8FEB86659FD93ull)); }
+PGS_HD uint64_t hotkey_hash(const uint8_t *p, uint32_t len)
+{
+    uint64_t s = 0;
+    for (uint32_t j = 0; 4 * j < len; j++) s += hotkey_word_hash(hotkey_word(p, len, j), j);
+    return hotkey_finish(s, len);
+}
+PGS_HD uint32_t hotkey_bucket(const uint8_t *hash_key, uint32_t len, uint32_t n_buckets) { return (uint32_t)(hotkey_hash(hash_key, len) % n_buckets); }
+
 // crc64 table (host): reflected CRC-64, table driven; polynomial bits from utils/crc.cpp:289-295
 inline void crc64_make_table(uint64_t tab[256])
 {

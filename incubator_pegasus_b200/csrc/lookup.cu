@@ -7,6 +7,7 @@
 #include <cstring>
 
 #include "engine.h"
+#include "hotkey_kernels.cuh"
 #include "read_kernels.cuh"
 #include "scan_kernel.cuh"
 
@@ -314,13 +315,112 @@ static int32_t scan_launch(Partition &part, const std::vector<std::shared_ptr<Ru
     return PGS_OK;
 }
 
+// ---- hot-key capture of batched gets (hotkey_kernels.cuh) ------------------------------------------------------------------
+Partition::~Partition()
+{
+    if (hk_dev_buckets) { cudaSetDevice(eng->device); cudaFree(hk_dev_buckets); }
+}
+
+int32_t hotkey_control(Partition &p, int32_t type, int32_t action, uint32_t now, std::string &text)
+{
+    if (action != HOTKEY_START && action != HOTKEY_STOP && action != HOTKEY_QUERY) { text = "invalid detect_action"; return HOTKEY_INVALID_PARAMETERS; }
+    if (type != HOTKEY_READ && type != HOTKEY_WRITE) { text = "invalid hotkey_type"; return HOTKEY_INVALID_PARAMETERS; }
+    if (type == HOTKEY_WRITE) return p.hk_write.control(action, now, text);
+    std::unique_lock<std::shared_mutex> g(p.hk_dev_mu);
+    if (action == HOTKEY_START && p.hk_read.state() == HOTKEY_STOPPED) { // the device counters start from zero
+        const uint32_t nb = p.hk_read.config().buckets;
+        cudaError_t e = cudaSetDevice(p.eng->device);
+        if (e == cudaSuccess && p.hk_dev_buckets && p.hk_dev_n != nb) { cudaFree(p.hk_dev_buckets); p.hk_dev_buckets = nullptr; }
+        if (e == cudaSuccess && !p.hk_dev_buckets) e = cudaMalloc((void **)&p.hk_dev_buckets, sizeof(unsigned long long) * nb);
+        if (e == cudaSuccess) { p.hk_dev_n = nb; e = cudaMemset(p.hk_dev_buckets, 0, sizeof(unsigned long long) * nb); }
+        if (e == cudaSuccess) e = cudaDeviceSynchronize();
+        if (e != cudaSuccess) { cuda_fail(e, "hotkey counters"); text = std::string("hotkey counters: ") + cudaGetErrorString(e); return HOTKEY_INVALID_STATE; }
+    }
+    return p.hk_read.control(action, now, text);
+}
+
+int32_t hotkey_analyse(Partition &p, uint32_t now)
+{
+    p.hk_write.analyse(now);
+    std::unique_lock<std::shared_mutex> g(p.hk_dev_mu); // no capturing launch is in flight
+    std::vector<uint64_t> dev;
+    if (p.hk_dev_buckets && p.hk_read.state() == HOTKEY_COARSE) { // read and zero the counters with one small copy each way
+        PGS_CUDA(cudaSetDevice(p.eng->device));
+        dev.resize(p.hk_dev_n);
+        PGS_CUDA(cudaMemcpy(dev.data(), p.hk_dev_buckets, sizeof(unsigned long long) * p.hk_dev_n, cudaMemcpyDeviceToHost));
+        PGS_CUDA(cudaMemset(p.hk_dev_buckets, 0, sizeof(unsigned long long) * p.hk_dev_n));
+        PGS_CUDA(cudaDeviceSynchronize());
+    }
+    p.hk_read.analyse(now, &dev);
+    return PGS_OK;
+}
+
+// The READ collectors a get launch captures into: the distinct partitions of the call with an active collector, locked
+// shared (hk_dev_mu) until the fine captures are handed over, and one slot descriptor per partition slot of the launch.
+struct HotkeyCapture {
+    std::vector<std::shared_lock<std::shared_mutex>> locks;
+    std::vector<HotkeySlotDev> slots;
+    std::vector<Partition *> slot_part;
+    uint32_t total_room = 0;
+    bool any = false;
+    uint32_t n_buckets = 0;
+
+    void open(pgs_partition *const *parts, uint32_t n_parts)
+    {
+        bool active = false;
+        for (uint32_t s = 0; s < n_parts; s++) active |= parts[s]->p.hk_read.active();
+        if (!active) return; // no detection: nothing is locked, uploaded or launched
+        std::vector<Partition *> locked;
+        slots.assign(n_parts, HotkeySlotDev{nullptr, 0, 0, 0, 0});
+        slot_part.assign(n_parts, nullptr);
+        for (uint32_t s = 0; s < n_parts; s++) {
+            Partition &pp = parts[s]->p;
+            if (!pp.hk_read.active()) continue;
+            if (std::find(locked.begin(), locked.end(), &pp) == locked.end()) { locks.emplace_back(pp.hk_dev_mu); locked.push_back(&pp); }
+            const HotkeyCollector::Phase ph = pp.hk_read.device_phase();
+            // every collector of one engine shares the bucket count of its options; a slot with another count is left out
+            if (ph.state == HOTKEY_STOPPED || !pp.hk_dev_buckets || (n_buckets && pp.hk_dev_n != n_buckets)) continue;
+            n_buckets = pp.hk_dev_n;
+            HotkeySlotDev &d = slots[s];
+            d.state = ph.state;
+            if (ph.state == HOTKEY_COARSE) d.buckets = pp.hk_dev_buckets;
+            else { d.target = ph.target; d.room = ph.room; d.idx_base = total_room; total_room += ph.room; }
+            slot_part[s] = &pp;
+            any = true;
+        }
+    }
+    // keys the memtable-less shortcut answers without a launch (a partition with no runs): captured on the host
+    void capture_on_host(const uint8_t *keys, const uint32_t *key_off, const uint32_t *key_part, uint32_t n)
+    {
+        for (uint32_t i = 0; any && i < n; i++)
+            if (Partition *pp = slot_part[key_part ? key_part[i] : 0])
+                pp->hk_read.capture_raw_key(std::string_view((const char *)keys + key_off[i], key_off[i + 1] - key_off[i]), 1);
+    }
+    // the fine captures of a finished launch: the first min(ticket, room) admitted keys of every fine slot
+    void hand_over(const uint8_t *keys, const uint32_t *key_off, const std::vector<uint32_t> &tickets, const std::vector<uint32_t> &idx)
+    {
+        for (uint32_t s = 0; s < slots.size(); s++) {
+            if (slots[s].state != HOTKEY_FINE) continue;
+            const uint32_t m = std::min(tickets[s], slots[s].room);
+            std::vector<std::string> hks;
+            for (uint32_t j = 0; j < m; j++) {
+                const uint32_t q = idx[slots[s].idx_base + j];
+                const KeyParts k = split_key(keys + key_off[q], key_off[q + 1] - key_off[q]);
+                hks.emplace_back((const char *)k.hk, k.hkl);
+            }
+            slot_part[s]->hk_read.add_fine_keys(hks);
+        }
+    }
+};
+
 } // namespace pgs
 
 using namespace pgs;
 
 // one get launch over the keys of one partition (parts[0], key_part null) or of several partitions of one engine
 static int32_t get_batch_impl(pgs_partition *const *parts, uint32_t n_parts, const uint8_t *keys, const uint32_t *key_off, const uint32_t *key_part,
-                              uint32_t n, uint32_t now, uint8_t *arena, uint64_t arena_cap, pgs_get_result *results, uint64_t *arena_used)
+                              uint32_t n, uint32_t now, uint8_t *arena, uint64_t arena_cap, pgs_get_result *results, uint64_t *arena_used,
+                              bool capture = true)
 {
     Partition &part = parts[0]->p;
     Engine *e = part.eng;
@@ -336,8 +436,11 @@ static int32_t get_batch_impl(pgs_partition *const *parts, uint32_t n_parts, con
     if (rc != PGS_OK) return rc;
     for (uint32_t i = 0; key_part && i < n; i++)
         if (key_part[i] >= n_parts) { set_error("get_batch_multi: key %u names partition slot %u of %u", i, key_part[i], n_parts); return PGS_INVALID_ARGUMENT; }
+    HotkeyCapture hk;
+    if (capture) hk.open(parts, key_part ? n_parts : 1);
     if (key_part ? M.packed.empty() : P.rr.n == 0) {
         for (uint32_t i = 0; i < n; i++) { memset(&results[i], 0, sizeof results[i]); results[i].status = PGS_NOT_FOUND; }
+        hk.capture_on_host(keys, key_off, key_part, n);
         return PGS_OK;
     }
     const ReadGeometry geo = get_geometry(P.KS);
@@ -376,12 +479,33 @@ static int32_t get_batch_impl(pgs_partition *const *parts, uint32_t n_parts, con
     kern<<<grid, kReadThreads, geo.dyn, st>>>(P);
     PGS_CUDA(cudaEventRecord(ev_b, st));
     e->launches++;
+    // hot-key capture (only while a slot's READ collector is active): its fine tickets and indices come back with the results
+    std::vector<uint32_t> hk_tickets, hk_idx;
+    if (hk.any) {
+        HotkeyParams H{};
+        H.keys = d_keys; H.key_off = P.key_off; H.key_part = key_part ? P.key_part : nullptr; H.n = n; H.n_buckets = hk.n_buckets;
+        const uint32_t n_slots = (uint32_t)hk.slots.size();
+        PGS_CUDA(S.upload(H.slots, hk.slots.data(), n_slots));
+        PGS_CUDA(S.alloc(H.tickets, sizeof(uint32_t) * (n_slots + (size_t)hk.total_room)));
+        PGS_CUDA(cudaMemsetAsync(H.tickets, 0, sizeof(uint32_t) * n_slots, st));
+        H.idx = H.tickets + n_slots;
+        const uint32_t hgrid = std::min<uint32_t>((n + kHotkeyThreads - 1) / kHotkeyThreads, 8u * e->sm_count);
+        k_hotkey_capture<<<hgrid, kHotkeyThreads, 0, st>>>(H);
+        e->launches++;
+        hk_tickets.resize(n_slots + (size_t)hk.total_room);
+        PGS_CUDA(cudaMemcpyAsync(hk_tickets.data(), H.tickets, sizeof(uint32_t) * hk_tickets.size(), cudaMemcpyDeviceToHost, st));
+    }
     uint32_t herr = 0;
     unsigned long long cur3[3] = {0, 0, 0};
     PGS_CUDA(cudaMemcpyAsync(results, P.results, sizeof(pgs_get_result) * n, cudaMemcpyDeviceToHost, st));
     PGS_CUDA(cudaMemcpyAsync(cur3, P.arena_cursor, 24, cudaMemcpyDeviceToHost, st));
     PGS_CUDA(cudaMemcpyAsync(&herr, P.error, 4, cudaMemcpyDeviceToHost, st));
     PGS_CUDA(cudaStreamSynchronize(st));
+    if (hk.any && hk.total_room) {
+        hk_idx.assign(hk_tickets.begin() + hk.slots.size(), hk_tickets.end());
+        hk_tickets.resize(hk.slots.size());
+        hk.hand_over(keys, key_off, hk_tickets, hk_idx);
+    }
     float ms = 0.f;
     cudaEventElapsedTime(&ms, ev_a, ev_b);
     set_last_read_stats(ms, cur3[1], cur3[2]);
@@ -395,7 +519,15 @@ static int32_t get_batch_impl(pgs_partition *const *parts, uint32_t n_parts, con
     return used > arena_cap ? PGS_INCOMPLETE : PGS_OK;
 }
 
-extern "C" int32_t pgs_get_batch(pgs_partition *ph, const uint8_t *keys, const uint32_t *key_off, uint32_t n, uint32_t now, uint8_t *arena,
+// pgs_get_batch, with the READ collector's capture switched on or off (handlers that capture with their own weights)
+int32_t pgs::get_batch(pgs_partition *ph, const uint8_t *keys, const uint32_t *key_off, uint32_t n, uint32_t now, uint8_t *arena,
+                       uint64_t arena_cap, pgs_get_result *results, uint64_t *arena_used, bool capture)
+{
+    if (!ph || (n && (!keys || !key_off || !results))) return PGS_INVALID_ARGUMENT;
+    return get_batch_impl(&ph, 1, keys, key_off, nullptr, n, now, arena, arena_cap, results, arena_used, capture);
+}
+
+extern "C" int32_t pgs_get_batch(pgs_partition *ph,const uint8_t *keys, const uint32_t *key_off, uint32_t n, uint32_t now, uint8_t *arena,
                                  uint64_t arena_cap, pgs_get_result *results, uint64_t *arena_used)
 {
     if (!ph || (n && (!keys || !key_off || !results))) return PGS_INVALID_ARGUMENT;

@@ -304,8 +304,10 @@ static int32_t ensure_range_ready(Server &s, RLock &lk, uint32_t now, bool rever
 
 // Point lookups of n raw keys: the memtable answers what it holds (newest version wins over every run), the rest goes to
 // the GPU in one pgs_get_batch.  res[i].value_off/value_len index `arena` (grown as needed).
+// capture: every key is captured once by the READ hot-key collector with weight 1 -- here when the memtable answers it, on
+// the device (k_hotkey_capture) when it goes to the GPU; handlers with weights of their own pass false.
 static int32_t point_lookup(Server &s, const std::vector<std::string> &keys, uint32_t now, std::vector<pgs_get_result> &res,
-                            std::vector<uint8_t> &arena)
+                            std::vector<uint8_t> &arena, bool capture = true)
 {
     const uint32_t n = (uint32_t)keys.size();
     res.assign(n, pgs_get_result{});
@@ -316,6 +318,7 @@ static int32_t point_lookup(Server &s, const std::vector<std::string> &keys, uin
         std::string_view v;
         const int m = s.mem_get(keys[i], &v);
         if (m == 0) { miss.push_back(i); continue; }
+        if (capture) s.part->p.hk_read.capture_raw_key(keys[i], 1);
         pgs_get_result &r = res[i];
         r.status = PGS_NOT_FOUND;
         if (m == 2) continue; // tombstone
@@ -335,7 +338,8 @@ static int32_t point_lookup(Server &s, const std::vector<std::string> &keys, uin
     uint64_t used = 0;
     int32_t st;
     for (;;) {
-        st = pgs_get_batch(s.part, (const uint8_t *)flat.data(), off.data(), (uint32_t)miss.size(), now, dev.data(), dev.size(), gr.data(), &used);
+        st = get_batch(s.part, (const uint8_t *)flat.data(), off.data(), (uint32_t)miss.size(), now, dev.data(), dev.size(), gr.data(), &used,
+                       capture && !used); // a retry with a larger arena captures nothing again
         if (st == PGS_INCOMPLETE && used > dev.size()) { dev.resize(used + 64); continue; }
         break;
     }
@@ -435,7 +439,7 @@ static int32_t do_multi_get(Server &s, RLock &lk, const pgs_multi_get_request &q
     for (uint32_t i = 0; i < q.n_sort_keys; i++) keys.push_back(make_key(hash_key, bsv(q.sort_keys[i])));
     std::vector<pgs_get_result> gr;
     std::vector<uint8_t> arena;
-    st = point_lookup(s, keys, now, gr, arena);
+    st = point_lookup(s, keys, now, gr, arena, false);
     if (st != PGS_OK) return read_fail(r, st);
     int32_t count = 0;
     int64_t size = 0;
@@ -461,7 +465,7 @@ static int32_t do_batch_get(Server &s, const pgs_full_key *fk, uint32_t n, uint3
     for (uint32_t i = 0; i < n; i++) keys.push_back(make_key(bsv(fk[i].hash_key), bsv(fk[i].sort_key)));
     std::vector<pgs_get_result> gr;
     std::vector<uint8_t> arena;
-    int32_t st = point_lookup(s, keys, now, gr, arena);
+    int32_t st = point_lookup(s, keys, now, gr, arena, false);
     if (st != PGS_OK) return read_fail(r, st);
     for (uint32_t i = 0; i < n; i++) {
         if (gr[i].expired) { r.view.expire_count++; continue; }
@@ -694,8 +698,17 @@ int32_t pgs_rrdb_start(pgs_engine *e, int32_t app_id, int32_t pidx, const pgs_se
     s.pidx = pidx;
     if (opt) s.opt = *opt; else s.opt.prefix_filter = 1;
     if (!s.opt.cluster_id) s.opt.cluster_id = 1;
+    HotkeyConfig hc;
+    if (!hotkey_config(s.opt.hotkey_buckets_num, s.opt.hot_bucket_variance_threshold, s.opt.hot_key_variance_threshold,
+                       s.opt.max_seconds_to_detect_hotkey, hc)) {
+        set_error("rrdb_start: hotkey_buckets_num %u is not a prime >= 3", s.opt.hotkey_buckets_num);
+        delete h;
+        return PGS_INVALID_ARGUMENT;
+    }
     int32_t st = pgs_partition_create(e, app_id, pidx, s.data_version, &s.part);
     if (st != PGS_OK) { delete h; return st; }
+    s.part->p.hk_read.set_config(hc);
+    s.part->p.hk_write.set_config(hc);
     std::mt19937_64 rng(std::random_device{}());
     s.ctx_counter = (int64_t)(rng() % (1ull << 31)) << 32; // pegasus_scan_context.h:113-114, kept non-negative
     if (envs && n_envs) pgs_rrdb_update_app_envs(h, envs, n_envs, 0);
@@ -716,13 +729,50 @@ void pgs_rrdb_set_partition_version(pgs_server *h, int32_t pv) { h->s.partition_
 #define WLOCKED(h) std::unique_lock<std::shared_mutex> _g((h)->s.mu)
 int32_t pgs_rrdb_get(pgs_server *h, pgs_blob key, uint32_t now, pgs_response_buf *r) { RLOCKED(h); return do_get(h->s, bsv(key), now, r->r, false); }
 int32_t pgs_rrdb_ttl(pgs_server *h, pgs_blob key, uint32_t now, pgs_response_buf *r) { RLOCKED(h); return do_get(h->s, bsv(key), now, r->r, true); }
-int32_t pgs_rrdb_multi_get(pgs_server *h, const pgs_multi_get_request *q, uint32_t now, pgs_response_buf *r) { RLOCKED(h); return do_multi_get(h->s, _g, *q, now, r->r); }
-int32_t pgs_rrdb_batch_get(pgs_server *h, const pgs_full_key *k, uint32_t n, uint32_t now, pgs_response_buf *r) { RLOCKED(h); return do_batch_get(h->s, k, n, now, r->r); }
-int32_t pgs_rrdb_sortkey_count(pgs_server *h, pgs_blob hk, uint32_t now, pgs_response_buf *r) { RLOCKED(h); return do_sortkey_count(h->s, _g, bsv(hk), now, r->r); }
+// the READ collector's captures of these handlers (capacity_unit_calculator.cpp:179-269) follow their responses
+int32_t pgs_rrdb_multi_get(pgs_server *h, const pgs_multi_get_request *q, uint32_t now, pgs_response_buf *r)
+{
+    RLOCKED(h);
+    const int32_t st = do_multi_get(h->s, _g, *q, now, r->r);
+    if (st == PGS_OK || st == PGS_NOT_FOUND || st == PGS_INCOMPLETE || st == PGS_INVALID_ARGUMENT)
+        h->s.part->p.hk_read.capture_hash_key(bsv(q->hash_key), r->r.view.n_kvs); // weight = kvs returned
+    return st;
+}
+int32_t pgs_rrdb_batch_get(pgs_server *h, const pgs_full_key *k, uint32_t n, uint32_t now, pgs_response_buf *r)
+{
+    RLOCKED(h);
+    const int32_t st = do_batch_get(h->s, k, n, now, r->r);
+    for (uint32_t i = 0; i < r->r.view.n_kvs; i++) // the hash key of every returned record, weight 1
+        h->s.part->p.hk_read.capture_hash_key(std::string_view(r->r.arena.data() + r->r.kvs[i].key_off, r->r.hk_len[i]), 1);
+    return st;
+}
+int32_t pgs_rrdb_sortkey_count(pgs_server *h, pgs_blob hk, uint32_t now, pgs_response_buf *r)
+{
+    RLOCKED(h);
+    const int32_t st = do_sortkey_count(h->s, _g, bsv(hk), now, r->r);
+    if (st == PGS_OK || st == PGS_NOT_FOUND) h->s.part->p.hk_read.capture_hash_key(bsv(hk), 1);
+    return st;
+}
 int32_t pgs_rrdb_get_scanner(pgs_server *h, const pgs_get_scanner_request *q, uint32_t now, pgs_response_buf *r) { RLOCKED(h); return do_get_scanner(h->s, _g, *q, now, r->r); }
 int32_t pgs_rrdb_scan(pgs_server *h, int64_t context_id, uint32_t now, pgs_response_buf *r) { RLOCKED(h); return do_scan(h->s, context_id, now, r->r); }
 void pgs_rrdb_clear_scanner(pgs_server *h, int64_t context_id) { std::lock_guard<std::mutex> g(h->s.ctx_mu); h->s.ctx.erase(context_id); }
 uint32_t pgs_rrdb_gc(pgs_server *h, uint32_t now) { return h->s.gc_contexts(now); }
+
+int32_t pgs_rrdb_detect_hotkey(pgs_server *h, int32_t type, int32_t action, uint32_t now_s, char *result_buf, uint32_t cap, uint32_t *result_len)
+{
+    if (!h) return PGS_HOTKEY_INVALID_PARAMETERS;
+    std::string text;
+    const int32_t out = hotkey_control(h->s.part->p, type, action, now_s, text);
+    if (result_buf && cap) memcpy(result_buf, text.data(), std::min<size_t>(cap, text.size()));
+    if (result_len) *result_len = (uint32_t)text.size();
+    return out;
+}
+int32_t pgs_rrdb_hotkey_analyse(pgs_server *h, uint32_t now_s) { return h ? hotkey_analyse(h->s.part->p, now_s) : PGS_INVALID_ARGUMENT; }
+int32_t pgs_rrdb_hotkey_state(pgs_server *h, int32_t type)
+{
+    if (!h || (type != PGS_HOTKEY_READ && type != PGS_HOTKEY_WRITE)) return -1;
+    return (int32_t)(type == PGS_HOTKEY_READ ? h->s.part->p.hk_read : h->s.part->p.hk_write).state();
+}
 
 int32_t pgs_rrdb_get_many(pgs_server *h, const uint8_t *keys, const uint32_t *key_off, uint32_t n, uint32_t now,
                           uint8_t *arena, uint64_t arena_cap, pgs_get_result *results, uint64_t *arena_used)
@@ -750,6 +800,7 @@ int32_t pgs_rrdb_put(pgs_server *h, pgs_blob key, pgs_blob value, uint32_t expir
     WLOCKED(h);
     h->s.last_committed_decree = decree;
     h->s.put_one(bsv(key), bsv(value), expire_ts, timestamp_us, now);
+    h->s.part->p.hk_write.capture_raw_key(bsv(key), 1);
     return PGS_OK;
 }
 int32_t pgs_rrdb_remove(pgs_server *h, pgs_blob key, int64_t decree, uint32_t now)
@@ -757,6 +808,7 @@ int32_t pgs_rrdb_remove(pgs_server *h, pgs_blob key, int64_t decree, uint32_t no
     WLOCKED(h);
     h->s.last_committed_decree = decree;
     h->s.mem_write(std::string(bsv(key)), PGS_TYPE_DELETION, std::string(), now);
+    h->s.part->p.hk_write.capture_raw_key(bsv(key), 1);
     return PGS_OK;
 }
 int32_t pgs_rrdb_on_batched_writes(pgs_server *h, const pgs_write_request *reqs, uint32_t count, int64_t decree, uint64_t timestamp_us,
@@ -772,6 +824,7 @@ int32_t pgs_rrdb_on_batched_writes(pgs_server *h, const pgs_write_request *reqs,
     for (uint32_t i = 0; i < count; i++) {
         if (reqs[i].op == 0) s.put_one(bsv(reqs[i].raw_key), bsv(reqs[i].value), reqs[i].expire_ts_seconds, timestamp_us, now);
         else s.mem_write(std::string(bsv(reqs[i].raw_key)), PGS_TYPE_DELETION, std::string(), now);
+        s.part->p.hk_write.capture_raw_key(bsv(reqs[i].raw_key), 1);
         if (resp_errors) resp_errors[i] = PGS_OK;
     }
     return PGS_OK;
@@ -828,6 +881,7 @@ int32_t pgs_rrdb_incr(pgs_server *h, pgs_blob key, int64_t increment, int32_t ex
         new_ets = expire_ts_seconds == 0 ? gr[0].expire_ts : expire_ts_seconds < 0 ? 0u : (uint32_t)expire_ts_seconds;
     }
     s.put_one(bsv(key), std::to_string(nv), new_ets, timestamp_us, now);
+    s.part->p.hk_write.capture_raw_key(bsv(key), 1);
     *resp_error = PGS_OK;
     *new_value = nv;
     return PGS_OK;
@@ -869,8 +923,9 @@ static bool cas_validate(int32_t type, std::string_view operand, bool exist, std
     return false;
 }
 
+// write_weight: the WRITE collector's weight of a successful call (check_and_set 1, check_and_mutate the mutation count)
 static int32_t check_and_mutate(Server &s, const pgs_check_and_mutate_request &q, int64_t decree, uint64_t timestamp_us, uint32_t now,
-                                pgs_cas_result *res, uint8_t *cv_out, uint32_t cv_cap)
+                                pgs_cas_result *res, uint8_t *cv_out, uint32_t cv_cap, int64_t write_weight)
 {
     s.last_committed_decree = decree;
     pgs_cas_result dummy;
@@ -881,6 +936,7 @@ static int32_t check_and_mutate(Server &s, const pgs_check_and_mutate_request &q
     if (bad) {
         res->error = PGS_INVALID_ARGUMENT;
         s.put_one({}, {}, 0, timestamp_us, now); // empty_put: the decree still advances
+        s.part->p.hk_read.capture_hash_key(bsv(q.hash_key), 1);
         return PGS_OK;
     }
     std::vector<pgs_get_result> gr;
@@ -907,6 +963,7 @@ static int32_t check_and_mutate(Server &s, const pgs_check_and_mutate_request &q
             else s.mem_write(key, PGS_TYPE_DELETION, std::string(), now);
         }
         res->error = PGS_OK;
+        s.part->p.hk_write.capture_hash_key(bsv(q.hash_key), write_weight); // the read was captured by point_lookup
     } else {
         s.put_one({}, {}, 0, timestamp_us, now);
         res->error = invalid ? PGS_INVALID_ARGUMENT : PGS_TRY_AGAIN;
@@ -918,7 +975,7 @@ int32_t pgs_rrdb_check_and_mutate(pgs_server *h, const pgs_check_and_mutate_requ
 {
     if (!h || !q) return PGS_INVALID_ARGUMENT;
     WLOCKED(h);
-    return check_and_mutate(h->s, *q, decree, timestamp_us, now, res, cv_out, cv_cap);
+    return check_and_mutate(h->s, *q, decree, timestamp_us, now, res, cv_out, cv_cap, q->n_mutate);
 }
 int32_t pgs_rrdb_check_and_set(pgs_server *h, const pgs_check_and_set_request *q, int64_t decree, uint64_t timestamp_us, uint32_t now,
                                pgs_cas_result *res, uint8_t *cv_out, uint32_t cv_cap)
@@ -927,7 +984,7 @@ int32_t pgs_rrdb_check_and_set(pgs_server *h, const pgs_check_and_set_request *q
     WLOCKED(h);
     pgs_mutate m{0, q->set_diff_sort_key ? q->set_sort_key : q->check_sort_key, q->set_value, q->set_expire_ts_seconds};
     pgs_check_and_mutate_request r{q->hash_key, q->check_sort_key, q->check_type, q->check_operand, &m, 1, q->return_check_value};
-    return check_and_mutate(h->s, r, decree, timestamp_us, now, res, cv_out, cv_cap);
+    return check_and_mutate(h->s, r, decree, timestamp_us, now, res, cv_out, cv_cap, 1);
 }
 int32_t pgs_rrdb_multi_put(pgs_server *h, pgs_blob hash_key, const pgs_blob *sort_keys, const pgs_blob *values,
                            uint32_t n, uint32_t expire_ts, int64_t decree, uint64_t timestamp_us, uint32_t now)
@@ -937,9 +994,11 @@ int32_t pgs_rrdb_multi_put(pgs_server *h, pgs_blob hash_key, const pgs_blob *sor
     s.last_committed_decree = decree;
     if (n == 0) { // request.kvs is empty: kInvalidArgument, but an empty record still advances the decree
         s.put_one({}, {}, 0, timestamp_us, now); // empty_put (pegasus_write_service_impl.h:90-99,112-119)
+        s.part->p.hk_write.capture_hash_key(bsv(hash_key), 0); // multi_put captures whatever its status (a weight of 0 counts 1)
         return PGS_INVALID_ARGUMENT;
     }
     for (uint32_t i = 0; i < n; i++) s.put_one(make_key(bsv(hash_key), bsv(sort_keys[i])), bsv(values[i]), expire_ts, timestamp_us, now);
+    s.part->p.hk_write.capture_hash_key(bsv(hash_key), n);
     return PGS_OK;
 }
 int32_t pgs_rrdb_multi_remove(pgs_server *h, pgs_blob hash_key, const pgs_blob *sort_keys, uint32_t n, int64_t decree,
@@ -954,6 +1013,7 @@ int32_t pgs_rrdb_multi_remove(pgs_server *h, pgs_blob hash_key, const pgs_blob *
         return PGS_INVALID_ARGUMENT;
     }
     for (uint32_t i = 0; i < n; i++) s.mem_write(make_key(bsv(hash_key), bsv(sort_keys[i])), PGS_TYPE_DELETION, std::string(), now);
+    s.part->p.hk_write.capture_hash_key(bsv(hash_key), n);
     if (count) *count = n;
     return PGS_OK;
 }

@@ -5,6 +5,7 @@
 
 #define PGS_SIM 1
 #include "../../incubator_pegasus_b200/csrc/compact_kernels.cuh"
+#include "../../incubator_pegasus_b200/csrc/hotkey_kernels.cuh"
 #include "../../incubator_pegasus_b200/csrc/index_kernel.cuh"
 #include "../../incubator_pegasus_b200/csrc/read_kernels.cuh"
 #include "../../incubator_pegasus_b200/csrc/scan_kernel.cuh"
@@ -314,5 +315,42 @@ int32_t sim_scan(uint32_t k, const uint8_t **data, const uint64_t *data_bytes, c
     PGS_LAUNCH(scan_fwd_kernel(geo.G, multi), 2, kReadThreads, geo.dyn, 0, P);
     return err[0] ? (int32_t)err[0] : PGS_OK;
 }
+
+// k_hotkey_capture over n keys of n_slots partition slots (key_part null: every key is slot 0).  Per slot: state (0 off,
+// 1 coarse, 2 fine), target bucket and queue room; buckets = n_slots * n_buckets counters, accumulated into; tickets[n_slots];
+// idx = the admitted fine indices, slot s at the sum of the rooms of the slots before it.  Returns the number of idx entries.
+uint32_t sim_hotkey_capture(const uint8_t *keys, const uint32_t *key_off, const uint32_t *key_part, uint32_t n, uint32_t n_buckets,
+                            uint32_t n_slots, const uint32_t *state, const uint32_t *target, const uint32_t *room,
+                            unsigned long long *buckets, uint32_t *tickets, uint32_t *idx, uint32_t grid)
+{
+    HostMem mem;
+    HotkeyParams P{};
+    uint8_t *k;
+    uint32_t *ko, *kp = nullptr, *t, *ix;
+    memcpy(host_alloc(mem, k, key_off[n] + 16, 0), keys, key_off[n]); // the slack of the product's key buffer
+    memcpy(host_alloc(mem, ko, n + 1, 0), key_off, 4 * (size_t)(n + 1));
+    if (key_part) memcpy(host_alloc(mem, kp, n, 0), key_part, 4 * (size_t)n);
+    HotkeySlotDev *sd;
+    host_alloc(mem, sd, n_slots, 0);
+    std::vector<unsigned long long *> bk(n_slots, nullptr);
+    uint32_t total = 0;
+    for (uint32_t s = 0; s < n_slots; s++) {
+        if (state[s] == 1) memcpy(host_alloc(mem, bk[s], n_buckets, 0), buckets + (size_t)s * n_buckets, 8 * (size_t)n_buckets);
+        sd[s] = HotkeySlotDev{bk[s], state[s], target[s], state[s] == 2 ? room[s] : 0u, total};
+        total += sd[s].room;
+    }
+    host_alloc(mem, t, n_slots, 0);
+    host_alloc(mem, ix, total, 0xEE);
+    P.keys = k; P.key_off = ko; P.key_part = kp; P.n = n; P.n_buckets = n_buckets; P.slots = sd; P.tickets = t; P.idx = ix;
+    if (n) PGS_LAUNCH(k_hotkey_capture, grid, kHotkeyThreads, 0, 0, P);
+    for (uint32_t s = 0; s < n_slots; s++)
+        if (bk[s]) memcpy(buckets + (size_t)s * n_buckets, bk[s], 8 * (size_t)n_buckets);
+    memcpy(tickets, t, 4 * (size_t)n_slots);
+    memcpy(idx, ix, 4 * (size_t)total);
+    return total;
+}
+
+// the bucket hash of format.h, for the tests' model
+uint64_t sim_hotkey_hash(const uint8_t *p, uint32_t len) { return hotkey_hash(p, len); }
 
 } // extern "C"

@@ -249,6 +249,18 @@ inline uint32_t __ballot_sync(uint32_t mask, int pred)
         return (uint64_t)b;
     });
 }
+template <class T>
+inline uint32_t __match_any_sync(uint32_t mask, T v)
+{
+    static_assert(sizeof(T) <= 8, "match");
+    uint64_t raw = 0;
+    memcpy(&raw, &v, sizeof(T));
+    return (uint32_t)simt::exchange(mask, raw, [&](uint64_t *w) {
+        uint32_t b = 0;
+        for (uint32_t l = 0; l < 32; l++) if ((mask >> l & 1) && w[l] == raw) b |= 1u << l;
+        return (uint64_t)b;
+    });
+}
 inline int __any_sync(uint32_t mask, int pred) { return __ballot_sync(mask, pred) != 0; }
 inline int __all_sync(uint32_t mask, int pred) { return __ballot_sync(mask, pred) == mask; }
 inline uint32_t __activemask() { return 0xffffffffu; }
@@ -314,4 +326,5 @@ typedef struct simt_stream_ *cudaStream_t; // launches run synchronously, in ord
 #define __shfl_xor_sync(...) (simt::cur_site() = __LINE__, __shfl_xor_sync(__VA_ARGS__))
 #define __ballot_sync(...) (simt::cur_site() = __LINE__, __ballot_sync(__VA_ARGS__))
 #define __any_sync(...) (simt::cur_site() = __LINE__, __any_sync(__VA_ARGS__))
+#define __match_any_sync(...) (simt::cur_site() = __LINE__, __match_any_sync(__VA_ARGS__))
 #define __all_sync(...) (simt::cur_site() = __LINE__, __all_sync(__VA_ARGS__))
