@@ -328,7 +328,6 @@ inline uint32_t compact_filter(MergeParams &P, const pgs_filter_params *fp)
 // Every buffer of one launch: buf(pointer, elements, fill, out) allocates the elements and, unless fill is kNoFill, sets each
 // byte to fill before the first kernel.  The scratch (out = false) lives as long as the launch; the merged run's buffers
 // (out = true) are fields of `run` (the library's Run, or the simulator's host copy), which outlives it.  P points at all of them.
-constexpr int kNoFill = -1;
 template <class R, class F>
 inline void compact_buffers(MergeParams &P, const CompactGeometry &geo, const CompactTotals &T, R &run, F &&buf)
 {

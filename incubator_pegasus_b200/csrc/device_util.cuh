@@ -23,6 +23,7 @@ namespace pgs {
 
 constexpr uint32_t kWarp = 32;
 constexpr uint32_t kFull = 0xffffffffu;
+constexpr int kNoFill = -1; // a launch buffer the host leaves unset (compact_buffers, get_buffers, scan_buffers)
 
 // ---- shared-memory addressing / mbarrier / TMA bulk (cp.async.bulk) ----------------------------
 #ifdef PGS_SIM

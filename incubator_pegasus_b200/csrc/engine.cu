@@ -137,7 +137,7 @@ cudaStream_t Engine::read_stream()
 static thread_local float t_last_ms = 0.f;
 static thread_local uint64_t t_last_probed = 0, t_last_skipped = 0;
 void set_last_read_stats(float ms, uint64_t probed, uint64_t skipped) { t_last_ms = ms; t_last_probed = probed; t_last_skipped = skipped; }
-int32_t lookup_init_kernels(int max_smem);
+int32_t lookup_init_kernels(Engine &e);
 int32_t compact_init_kernels(int max_smem);
 
 void *Engine::pinned(size_t bytes)
@@ -396,7 +396,7 @@ int32_t pgs_engine_open(const pgs_engine_config *cfg, pgs_engine **out)
         err = cudaMalloc(&e.d_crc, sizeof tab);
         if (err == cudaSuccess) err = cudaMemcpy(e.d_crc, tab, sizeof tab, cudaMemcpyHostToDevice);
     }
-    if (err == cudaSuccess && (lookup_init_kernels(e.max_smem_optin) != PGS_OK || compact_init_kernels(e.max_smem_optin) != PGS_OK ||
+    if (err == cudaSuccess && (lookup_init_kernels(e) != PGS_OK || compact_init_kernels(e.max_smem_optin) != PGS_OK ||
                                index_init_kernels() != PGS_OK)) {
         delete h; // the failing call left its description in pgs_last_error()
         return PGS_IO_ERROR;

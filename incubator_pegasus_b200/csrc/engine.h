@@ -49,6 +49,7 @@ struct Engine {
     pgs_engine_config cfg{};
     int sm_count = 0;
     int max_smem_optin = 0;
+    uint32_t scan_static_smem = 0; // k_scan's static shared memory (lookup_init_kernels)
     uint64_t *d_crc = nullptr; // the crc64 table (2 KB) of partition-hash validation in reads and compactions
     std::atomic<uint64_t> launches{0};
     std::atomic<uint64_t> next_run_id{1};
@@ -107,6 +108,28 @@ int32_t hotkey_control(Partition &p, int32_t type, int32_t action, uint32_t now,
 // pgs_get_batch; capture = false leaves the READ collector to the caller
 int32_t get_batch(pgs_partition *ph, const uint8_t *keys, const uint32_t *key_off, uint32_t n, uint32_t now, uint8_t *arena,
                   uint64_t arena_cap, pgs_get_result *results, uint64_t *arena_used, bool capture);
+// Where a scan call's answers go.  One request: its records and their bytes at kvs and arena, its resume key at resume.
+// Several: the launch gives request i arena_stride bytes, kv_stride records and a resume slot of resume_stride bytes, and
+// the answers come back packed -- request i's records at kvs + kv_base[i], their bytes at arena + arena_base[i] (n + 1
+// entries each, may be null), its resume key at resume + i * resume_stride.  arena_cap / kv_cap bound the whole answer.
+struct ScanOut {
+    uint8_t *arena;
+    uint64_t arena_stride, arena_cap;
+    pgs_kv *kvs;
+    uint32_t kv_stride;
+    uint64_t kv_cap;
+    uint8_t *resume;
+    uint32_t resume_stride;
+    uint64_t *arena_base;
+    uint32_t *kv_base;
+};
+// range scans over parts[0] (req_part null), or forward scans over several partitions of one engine in one launch: request i
+// reads partition slot req_part[i].  pinned = the runs to read instead of the partition's current ones (a parked scan context)
+int32_t scan_many(pgs_partition *const *parts, uint32_t n_parts, const uint32_t *req_part, const pgs_scan_request *reqs, uint32_t n,
+                  uint32_t now, pgs_scan_result *results, const ScanOut &out, const std::vector<std::shared_ptr<Run>> *pinned = nullptr);
+// true when k_scan can stage one block of every current run of the partition in one request's launch; a batch with a reverse
+// request gets PGS_NOT_SUPPORTED otherwise (the server folds L0 first, server.cpp)
+bool scan_stages_every_run(pgs_partition *ph);
 
 void set_error(const char *fmt, ...);
 int32_t cuda_fail(cudaError_t e, const char *what);

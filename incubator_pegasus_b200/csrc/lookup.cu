@@ -1,8 +1,13 @@
-// lookup.cu — host side of the read path (pgs_get_batch, pgs_range_scan, pgs_range_scan_many).
+// lookup.cu — host side of the read path (pgs_get_batch[_multi], pgs_range_scan, pgs_range_scan_many[_multi]).
 //
 //   k_get / k_scan_fwd (read_kernels.cuh)  point lookups and forward range scans: lane-group iterators straight over HBM.
 //   k_scan (scan_kernel.cuh)  REVERSE range scans, every request of a batch that mixes directions, and forward scans
 //           whose user keys are too long for k_scan_fwd: one CTA per request stages chunks of blocks of every run in shared memory.
+//
+// A read is planned and launched by the functions next to its kernels, which the simulator (tools/simt) calls too, as a
+// compaction is: read_run_set (the partition slots' runs), get_plan / scan_plan (kernel and shared memory), get_buffers /
+// scan_buffers (every device buffer with its size and initial content) and read_launch.  This file adds what is the library's
+// own: the run snapshot, the occupancy cap, device scratch, events, the read-back and the hot-key capture.
 #include <algorithm>
 #include <cstring>
 
@@ -52,85 +57,36 @@ __global__ void k_pack_copy(const pgs_scan_result *__restrict__ res, uint32_t n,
 
 void set_last_read_stats(float ms, uint64_t probed, uint64_t skipped);
 
-static int32_t snapshot_runs(Partition &part, std::vector<std::shared_ptr<Run>> &runs, ReadRuns &rr, uint32_t &KS,
+// The runs of a read call's partition slots (parts[0 .. n_slots)), each kept alive in `slots` until the launch is done, as the
+// launch plan's run set.  pinned = the runs to read instead of parts[0]'s current ones.  what: the ABI call, for the message.
+using SlotRuns = std::vector<std::vector<std::shared_ptr<Run>>>;
+static int32_t snapshot_runs(pgs_partition *const *parts, uint32_t n_slots, bool multi, const char *what, SlotRuns &slots, ReadRunSet &R,
                              const std::vector<std::shared_ptr<Run>> *pinned = nullptr)
 {
-    if (pinned) {
-        runs = *pinned;
-    } else {
-        std::lock_guard<std::mutex> g(part.mu);
-        runs = part.runs;
-    }
-    if (runs.size() > kMaxReadRuns) {
-        set_error("read: %zu runs > %u (compact first)", runs.size(), kMaxReadRuns);
-        return PGS_NOT_SUPPORTED;
-    }
-    rr.n = (uint32_t)runs.size();
-    uint32_t mk = 0;
-    for (uint32_t i = 0; i < rr.n; i++) { rr.runs[i] = runs[i]->dev(); mk = std::max(mk, runs[i]->info.max_ukey_len); }
-    if (mk > kMaxUkeyLen) return PGS_NOT_SUPPORTED;
-    KS = read_key_slot(mk);
-    return PGS_OK;
-}
-
-// the runs of several partitions of one engine, packed for one launch: partition slot s reads packed[begin[s] .. begin[s + 1])
-struct MultiRuns {
-    std::vector<std::shared_ptr<Run>> runs; // every run a request may touch stays alive until the launch is done
-    std::vector<RunDev> packed;
-    std::vector<uint32_t> begin{0};
-};
-// what: the ABI call, for the error message
-static int32_t snapshot_multi(pgs_partition *const *parts, uint32_t n_parts, const char *what, MultiRuns &M, ReadRuns &rr, uint32_t &KS)
-{
     const Partition &part = parts[0]->p;
-    KS = 8;
-    for (uint32_t p = 0; p < n_parts; p++) {
-        Partition &pp = parts[p]->p;
+    slots.resize(n_slots);
+    for (uint32_t s = 0; s < n_slots; s++) {
+        Partition &pp = parts[s]->p;
         if (pp.eng != part.eng || pp.data_version != part.data_version) { set_error("%s: partitions of different engines / data versions", what); return PGS_INVALID_ARGUMENT; }
-        std::vector<std::shared_ptr<Run>> rs;
-        ReadRuns one;
-        uint32_t ks = 0;
-        int32_t rc = snapshot_runs(pp, rs, one, ks);
-        if (rc != PGS_OK) return rc;
-        M.packed.insert(M.packed.end(), one.runs, one.runs + one.n);
-        M.begin.push_back((uint32_t)M.packed.size());
-        M.runs.insert(M.runs.end(), rs.begin(), rs.end());
-        KS = std::max(KS, ks);
+        if (pinned) {
+            slots[s] = *pinned;
+        } else {
+            std::lock_guard<std::mutex> g(pp.mu);
+            slots[s] = pp.runs;
+        }
     }
-    multi_read_runs(M.packed, M.begin, rr);
-    return PGS_OK;
+    return read_run_set(slots, multi, R);
 }
 
-// the dynamic shared memory of a k_scan launch of n_req requests over these runs on the current device (scan_dyn_bytes: 0 when
-// one block of every run does not fit); *pool = its staging pool
-static cudaError_t scan_launch_dyn(const Engine &e, const std::vector<std::shared_ptr<Run>> &runs, uint32_t KS, uint32_t n_req,
-                                   uint64_t &dyn, uint32_t *pool)
+bool scan_stages_every_run(pgs_partition *ph)
 {
-    cudaFuncAttributes attr;
-    const cudaError_t rc = cudaFuncGetAttributes(&attr, k_scan);
-    if (rc != cudaSuccess) return rc;
-    ScanBlockBound bb;
-    for (auto &r : runs) bb.add(r->info);
-    dyn = scan_dyn_bytes((uint32_t)runs.size(), KS, bb.max_blk, bb.max_rec, n_req, scan_max_dyn(e.max_smem_optin, attr.sharedSizeBytes), pool);
-    return cudaSuccess;
-}
-
-// true when k_scan can stage one block of every current run of the partition in one request's launch; scan_launch answers
-// a batch with a reverse request with PGS_NOT_SUPPORTED otherwise (the server folds L0 first, server.cpp)
-bool scan_stages_every_run(Partition &part)
-{
-    std::vector<std::shared_ptr<Run>> runs;
-    {
-        std::lock_guard<std::mutex> g(part.mu);
-        runs = part.runs;
-    }
-    if (runs.size() > kMaxReadRuns) return false;
-    uint32_t mk = 0;
-    for (auto &r : runs) mk = std::max(mk, r->info.max_ukey_len);
-    uint64_t dyn = 0; uint32_t pool = 0;
-    if (cudaSetDevice(part.eng->device) != cudaSuccess || scan_launch_dyn(*part.eng, runs, read_key_slot(mk), 1, dyn, &pool) != cudaSuccess)
-        return true; // the launch reports it
-    return dyn != 0;
+    SlotRuns slots;
+    ReadRunSet R;
+    if (snapshot_runs(&ph, 1, false, "", slots, R) != PGS_OK) return false;
+    ScanParams P{};
+    P.n = 1;
+    ReadLaunch<ScanParams> L;
+    return scan_plan(P, R, true, ph->p.eng->max_smem_optin, ph->p.eng->scan_static_smem, L) == PGS_OK;
 }
 
 // kernels of this file take their dynamic shared-memory size per launch; the opt-in maximum is set once per device here
@@ -143,8 +99,12 @@ static cudaError_t allow_max_smem(K kernel, int max_smem)
     if (e != cudaSuccess) return e;
     return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem - (int)a.sharedSizeBytes);
 }
-int32_t lookup_init_kernels(int max_smem)
+int32_t lookup_init_kernels(Engine &e)
 {
+    const int max_smem = e.max_smem_optin;
+    cudaFuncAttributes a;
+    PGS_CUDA(cudaFuncGetAttributes(&a, k_scan));
+    e.scan_static_smem = (uint32_t)a.sharedSizeBytes;
     PGS_CUDA(allow_max_smem(k_scan, max_smem));
     PGS_CUDA(cudaFuncSetAttribute(k_scan, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
     PGS_CUDA(allow_max_smem(k_get<8, false>, max_smem)); PGS_CUDA(allow_max_smem(k_get<8, true>, max_smem));
@@ -153,111 +113,70 @@ int32_t lookup_init_kernels(int max_smem)
     return PGS_OK;
 }
 
-static int32_t scan_launch(Partition &part, const std::vector<std::shared_ptr<Run>> &runs, ScanParams &P, const MultiRuns *multi,
-                           const uint32_t *req_part, const pgs_scan_request *reqs, uint32_t n, uint32_t now, unsigned long long arena_stride,
-                           uint32_t kv_stride, uint8_t *arena, uint64_t arena_cap, pgs_kv *kvs, uint64_t kv_cap, uint8_t *resume,
-                           uint32_t resume_stride, pgs_scan_result *results, uint64_t *arena_base, uint32_t *kv_base);
-
-int32_t scan_many(Partition &part, const pgs_scan_request *reqs, uint32_t n, uint32_t now, unsigned long long arena_stride,
-                  uint32_t kv_stride, uint8_t *arena, uint64_t arena_cap, pgs_kv *kvs, uint64_t kv_cap, uint8_t *resume,
-                  uint32_t resume_stride, pgs_scan_result *results, uint64_t *arena_base, uint32_t *kv_base,
-                  const std::vector<std::shared_ptr<Run>> *pinned)
+// the buffers of a read launch (get_buffers, scan_buffers) in its device scratch, on its stream; ce = the first failure
+static auto device_buffers(LaunchScratch &S, cudaError_t &ce)
 {
-    std::vector<std::shared_ptr<Run>> runs;
-    ScanParams P{};
-    int32_t rc = snapshot_runs(part, runs, P.rr, P.KS, pinned);
-    if (rc != PGS_OK) return rc;
-    if (n == 0) return PGS_OK;
-    return scan_launch(part, runs, P, nullptr, nullptr, reqs, n, now, arena_stride, kv_stride, arena, arena_cap, kvs, kv_cap, resume,
-                       resume_stride, results, arena_base, kv_base);
+    return [&S, &ce](auto *&p, uint64_t bytes, ReadInit in) {
+        if (ce == cudaSuccess) ce = S.alloc(p, bytes);
+        if (ce == cudaSuccess && in.src) ce = cudaMemcpyAsync((void *)p, in.src, in.src_bytes, cudaMemcpyHostToDevice, S.st);
+        if (ce == cudaSuccess && in.fill != kNoFill) ce = cudaMemsetAsync((void *)p, in.fill, bytes, S.st);
+    };
 }
 
-// forward scans over several partitions of one engine in one launch: request i reads partition slot req_part[i]
-static int32_t scan_many_multi(pgs_partition *const *parts, uint32_t n_parts, const pgs_scan_request *reqs, const uint32_t *req_part, uint32_t n,
-                               uint32_t now, unsigned long long arena_stride, uint32_t kv_stride, uint8_t *arena, uint64_t arena_cap, pgs_kv *kvs,
-                               uint64_t kv_cap, uint8_t *resume, uint32_t resume_stride, pgs_scan_result *results, uint64_t *arena_base,
-                               uint32_t *kv_base)
+// the CTAs of L the device holds at once (resident CTAs per SM for its dynamic shared memory; registers count too)
+template <class Params>
+static cudaError_t resident_ctas(const Engine &e, const ReadLaunch<Params> &L, uint64_t &ctas)
 {
-    ScanParams P{};
-    MultiRuns M;
-    int32_t rc = snapshot_multi(parts, n_parts, "range_scan_many_multi", M, P.rr, P.KS);
+    int occ = 0;
+    const cudaError_t rc = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, L.kernel, (int)L.threads, (size_t)L.dyn);
+    ctas = (uint64_t)std::max(1, occ) * e.sm_count;
+    return rc;
+}
+
+int32_t scan_many(pgs_partition *const *parts, uint32_t n_parts, const uint32_t *req_part, const pgs_scan_request *reqs, uint32_t n,
+                  uint32_t now, pgs_scan_result *results, const ScanOut &out, const std::vector<std::shared_ptr<Run>> *pinned)
+{
+    Partition &part = parts[0]->p;
+    Engine *e = part.eng;
+    SlotRuns slots;
+    ReadRunSet R;
+    int32_t rc = snapshot_runs(parts, n_parts, req_part != nullptr, "range_scan_many_multi", slots, R, pinned);
     if (rc != PGS_OK) return rc;
-    for (uint32_t i = 0; i < n; i++) {
+    for (uint32_t i = 0; req_part && i < n; i++) {
         if (req_part[i] >= n_parts) { set_error("range_scan_many_multi: request %u names partition slot %u of %u", i, req_part[i], n_parts); return PGS_INVALID_ARGUMENT; }
         if (reqs[i].reverse) { set_error("range_scan_many_multi: reverse scans go through pgs_range_scan_many"); return PGS_NOT_SUPPORTED; }
     }
     if (n == 0) return PGS_OK;
-    return scan_launch(parts[0]->p, M.runs, P, &M, req_part, reqs, n, now, arena_stride, kv_stride, arena, arena_cap, kvs, kv_cap, resume,
-                       resume_stride, results, arena_base, kv_base);
-}
-
-static int32_t scan_launch(Partition &part, const std::vector<std::shared_ptr<Run>> &runs, ScanParams &P, const MultiRuns *multi,
-                           const uint32_t *req_part, const pgs_scan_request *reqs, uint32_t n, uint32_t now, unsigned long long arena_stride,
-                           uint32_t kv_stride, uint8_t *arena, uint64_t arena_cap, pgs_kv *kvs, uint64_t kv_cap, uint8_t *resume,
-                           uint32_t resume_stride, pgs_scan_result *results, uint64_t *arena_base, uint32_t *kv_base)
-{
-    Engine *e = part.eng;
+    if (R.empty()) { // empty DB: every iterator is invalid from the start
+        memset(results, 0, sizeof(pgs_scan_result) * n);
+        if (out.arena_base) for (uint32_t i = 0; i <= n; i++) out.arena_base[i] = 0;
+        if (out.kv_base) for (uint32_t i = 0; i <= n; i++) out.kv_base[i] = 0;
+        return PGS_OK;
+    }
     PGS_CUDA(cudaSetDevice(e->device));
     cudaStream_t st = e->read_stream();
     const ScanBatch B = flatten_scan_requests(reqs, n);
-    if (!scan_output_strides(P, arena_stride, kv_stride, resume_stride)) resume_stride = 0; // caller gave no room for resume keys
+    ScanParams P{};
     P.n = n; P.now = now; P.data_version = part.data_version;
-    if (multi ? multi->packed.empty() : P.rr.n == 0) { // empty DB: every iterator is invalid from the start
-        memset(results, 0, sizeof(pgs_scan_result) * n);
-        if (arena_base) for (uint32_t i = 0; i <= n; i++) arena_base[i] = 0;
-        if (kv_base) for (uint32_t i = 0; i <= n; i++) kv_base[i] = 0;
-        return PGS_OK;
-    }
+    if (B.need_crc) P.crc_table = (const unsigned long long *)e->d_crc;
+    ReadLaunch<ScanParams> L;
+    rc = scan_plan(P, R, B.any_reverse, e->max_smem_optin, e->scan_static_smem, L);
+    if (rc != PGS_OK) return rc;
 
     LaunchScratch S(st);
     cudaEvent_t ev_a, ev_b;
     PGS_CUDA(S.event(ev_a));
     PGS_CUDA(S.event(ev_b));
-    PGS_CUDA(S.upload(P.reqs, B.reqs.data(), n));
-    PGS_CUDA(S.upload(P.blob, (const uint8_t *)B.blob.data(), B.blob.size()));
-    PGS_CUDA(S.alloc(P.arena, P.arena_stride * n + 16));
-    PGS_CUDA(S.alloc(P.kvs, sizeof(pgs_kv) * (size_t)kv_stride * n + 16));
-    PGS_CUDA(S.alloc(P.resume, (size_t)P.resume_stride * n + 16));
-    PGS_CUDA(S.alloc(P.results, sizeof(pgs_scan_result) * n));
-    PGS_CUDA(S.alloc(P.error, 16));
-    PGS_CUDA(cudaMemsetAsync(P.error, 0, 16, st));
-    if (multi) {
-        PGS_CUDA(S.upload(P.multi_runs, multi->packed.data(), multi->packed.size()));
-        PGS_CUDA(S.upload(P.multi_begin, multi->begin.data(), multi->begin.size()));
-        PGS_CUDA(S.upload(P.req_part, req_part, n));
-    }
-    if (B.need_crc) P.crc_table = (const unsigned long long *)e->d_crc;
-    P.ticket = P.error + 1;
-    // forward scans: lane-group merging iterators (read_kernels.cuh), unless the groups' key rows do not fit shared memory
-    // (user keys of a few KB): then k_scan, which stages records instead of keeping one key row per run and group
-    const ReadGeometry fwd = scan_fwd_geometry(P.rr.n, P.KS);
-    const bool fwd_fits = fwd.dyn <= (uint32_t)e->max_smem_optin;
-    if (!fwd_fits && multi) { set_error("scan: %u runs with keys of %u bytes do not fit shared memory", P.rr.n, P.KS); return PGS_NOT_SUPPORTED; }
-    if (!B.any_reverse && fwd_fits) {
-        fwd.apply(P);
-        const scan_fwd_kernel_t kern = scan_fwd_kernel(fwd.G, multi != nullptr);
-        int occ = 0;
-        PGS_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, (int)kReadThreads, (size_t)fwd.dyn));
-        const uint32_t per_cta = kReadThreads / fwd.G;
-        const uint32_t grid = std::min<uint32_t>((n + per_cta - 1) / per_cta, (uint32_t)std::max(1, occ) * e->sm_count);
-        PGS_CUDA(cudaEventRecord(ev_a, st));
-        kern<<<grid, kReadThreads, fwd.dyn, st>>>(P);
-        PGS_CUDA(cudaEventRecord(ev_b, st));
-    } else {
-        // ---- reverse scans (and forward ones with long keys): the block-staging kernel ---------------------------------
-        uint64_t dyn = 0;
-        PGS_CUDA(scan_launch_dyn(*e, runs, P.KS, n, dyn, &P.pool_bytes));
-        if (!dyn) {
-            set_error("scan: blocks too large for shared memory");
-            return PGS_NOT_SUPPORTED;
-        }
-        int occ = 0; // resident CTAs per SM for this dynamic shared-memory size (registers count too)
-        PGS_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_scan, (int)kScanThreads, (size_t)dyn));
-        uint32_t grid = std::min<uint32_t>(n, (uint32_t)std::max(1, occ) * e->sm_count);
-        PGS_CUDA(cudaEventRecord(ev_a, st));
-        k_scan<<<grid, kScanThreads, dyn, st>>>(P);
-        PGS_CUDA(cudaEventRecord(ev_b, st));
-    }
+    cudaError_t ce = cudaSuccess;
+    // resume_stride 0: the caller gave no room for resume keys
+    const uint32_t resume_stride = scan_buffers(P, R, B, req_part, out.arena_stride, out.kv_stride, out.resume_stride, device_buffers(S, ce))
+                                       ? out.resume_stride : 0;
+    PGS_CUDA(ce);
+    uint64_t ctas = 0;
+    PGS_CUDA(resident_ctas(*e, L, ctas));
+    PGS_CUDA(cudaEventRecord(ev_a, st));
+    read_launch(L, P, ctas, st);
+    PGS_CUDA(cudaEventRecord(ev_b, st));
     e->launches++;
     uint32_t herr = 0;
     if (n == 1) {
@@ -265,14 +184,14 @@ static int32_t scan_launch(Partition &part, const std::vector<std::shared_ptr<Ru
         PGS_CUDA(cudaMemcpyAsync(&herr, P.error, 4, cudaMemcpyDeviceToHost, st));
         PGS_CUDA(cudaStreamSynchronize(st));
         if (!herr) {
-            if (results[0].arena_used > arena_cap || results[0].n_kvs > kv_cap) return PGS_INCOMPLETE;
-            if (results[0].arena_used) PGS_CUDA(cudaMemcpyAsync(arena, P.arena, results[0].arena_used, cudaMemcpyDeviceToHost, st));
-            if (results[0].n_kvs) PGS_CUDA(cudaMemcpyAsync(kvs, P.kvs, sizeof(pgs_kv) * results[0].n_kvs, cudaMemcpyDeviceToHost, st));
-            if (results[0].iter_valid && resume && resume_stride) PGS_CUDA(cudaMemcpyAsync(resume, P.resume, results[0].resume_len, cudaMemcpyDeviceToHost, st));
+            if (results[0].arena_used > out.arena_cap || results[0].n_kvs > out.kv_cap) return PGS_INCOMPLETE;
+            if (results[0].arena_used) PGS_CUDA(cudaMemcpyAsync(out.arena, P.arena, results[0].arena_used, cudaMemcpyDeviceToHost, st));
+            if (results[0].n_kvs) PGS_CUDA(cudaMemcpyAsync(out.kvs, P.kvs, sizeof(pgs_kv) * results[0].n_kvs, cudaMemcpyDeviceToHost, st));
+            if (results[0].iter_valid && out.resume && resume_stride) PGS_CUDA(cudaMemcpyAsync(out.resume, P.resume, results[0].resume_len, cudaMemcpyDeviceToHost, st));
             PGS_CUDA(cudaStreamSynchronize(st));
         }
-        if (arena_base) { arena_base[0] = 0; arena_base[1] = results[0].arena_used; }
-        if (kv_base) { kv_base[0] = 0; kv_base[1] = results[0].n_kvs; }
+        if (out.arena_base) { out.arena_base[0] = 0; out.arena_base[1] = results[0].arena_used; }
+        if (out.kv_base) { out.kv_base[0] = 0; out.kv_base[1] = results[0].n_kvs; }
     } else {
         unsigned long long *d_abase = nullptr;
         uint32_t *d_kbase = nullptr;
@@ -288,21 +207,21 @@ static int32_t scan_launch(Partition &part, const std::vector<std::shared_ptr<Ru
         PGS_CUDA(cudaStreamSynchronize(st));
         e->launches++;
         if (!herr) {
-            if (ab[n] > arena_cap || kb[n] > kv_cap) { set_error("scan_many: output arena too small"); return PGS_INCOMPLETE; }
+            if (ab[n] > out.arena_cap || kb[n] > out.kv_cap) { set_error("scan_many: output arena too small"); return PGS_INCOMPLETE; }
             uint8_t *d_parena = nullptr;
             pgs_kv *d_pkvs = nullptr;
             PGS_CUDA(S.alloc(d_parena, ab[n] + 16));
             PGS_CUDA(S.alloc(d_pkvs, sizeof(pgs_kv) * ((size_t)kb[n] + 1)));
-            k_pack_copy<<<std::min<uint32_t>(n, 8 * e->sm_count), 128, 0, st>>>(P.results, n, P.arena, P.arena_stride, P.kvs, kv_stride, d_abase,
+            k_pack_copy<<<std::min<uint32_t>(n, 8 * e->sm_count), 128, 0, st>>>(P.results, n, P.arena, P.arena_stride, P.kvs, P.kv_stride, d_abase,
                                                                               d_kbase, d_parena, d_pkvs);
             e->launches++;
-            if (ab[n]) PGS_CUDA(cudaMemcpyAsync(arena, d_parena, ab[n], cudaMemcpyDeviceToHost, st));
-            if (kb[n]) PGS_CUDA(cudaMemcpyAsync(kvs, d_pkvs, sizeof(pgs_kv) * kb[n], cudaMemcpyDeviceToHost, st));
-            if (resume && resume_stride) PGS_CUDA(cudaMemcpyAsync(resume, P.resume, (size_t)P.resume_stride * n, cudaMemcpyDeviceToHost, st));
+            if (ab[n]) PGS_CUDA(cudaMemcpyAsync(out.arena, d_parena, ab[n], cudaMemcpyDeviceToHost, st));
+            if (kb[n]) PGS_CUDA(cudaMemcpyAsync(out.kvs, d_pkvs, sizeof(pgs_kv) * kb[n], cudaMemcpyDeviceToHost, st));
+            if (out.resume && resume_stride) PGS_CUDA(cudaMemcpyAsync(out.resume, P.resume, (size_t)P.resume_stride * n, cudaMemcpyDeviceToHost, st));
             PGS_CUDA(cudaStreamSynchronize(st));
         }
-        if (arena_base) for (uint32_t i = 0; i <= n; i++) arena_base[i] = ab[i];
-        if (kv_base) for (uint32_t i = 0; i <= n; i++) kv_base[i] = kb[i];
+        if (out.arena_base) for (uint32_t i = 0; i <= n; i++) out.arena_base[i] = ab[i];
+        if (out.kv_base) for (uint32_t i = 0; i <= n; i++) out.kv_base[i] = kb[i];
     }
     float ms = 0.f;
     cudaEventElapsedTime(&ms, ev_a, ev_b);
@@ -314,7 +233,6 @@ static int32_t scan_launch(Partition &part, const std::vector<std::shared_ptr<Ru
     }
     return PGS_OK;
 }
-
 // ---- hot-key capture of batched gets (hotkey_kernels.cuh) ------------------------------------------------------------------
 Partition::~Partition()
 {
@@ -426,64 +344,43 @@ static int32_t get_batch_impl(pgs_partition *const *parts, uint32_t n_parts, con
     Engine *e = part.eng;
     if (arena_used) *arena_used = 0;
     if (n == 0) return PGS_OK;
-    // pgs_get_result::value_off is 32-bit: a call uses at most the first 4 GiB - 1 of the arena.  A value that would end
-    // beyond that gets PGS_INCOMPLETE like any value that does not fit, and *arena_used still reports the whole need.
-    arena_cap = std::min<uint64_t>(arena_cap, UINT32_MAX);
-    std::vector<std::shared_ptr<Run>> runs; // every run a key may touch stays alive until the launch is done
-    GetParams P{};
-    MultiRuns M;
-    int32_t rc = key_part ? snapshot_multi(parts, n_parts, "get_batch_multi", M, P.rr, P.KS) : snapshot_runs(part, runs, P.rr, P.KS);
+    SlotRuns slots;
+    ReadRunSet R;
+    int32_t rc = snapshot_runs(parts, key_part ? n_parts : 1, key_part != nullptr, "get_batch_multi", slots, R);
     if (rc != PGS_OK) return rc;
     for (uint32_t i = 0; key_part && i < n; i++)
         if (key_part[i] >= n_parts) { set_error("get_batch_multi: key %u names partition slot %u of %u", i, key_part[i], n_parts); return PGS_INVALID_ARGUMENT; }
     HotkeyCapture hk;
     if (capture) hk.open(parts, key_part ? n_parts : 1);
-    if (key_part ? M.packed.empty() : P.rr.n == 0) {
+    if (R.empty()) {
         for (uint32_t i = 0; i < n; i++) { memset(&results[i], 0, sizeof results[i]); results[i].status = PGS_NOT_FOUND; }
         hk.capture_on_host(keys, key_off, key_part, n);
         return PGS_OK;
     }
-    const ReadGeometry geo = get_geometry(P.KS);
-    if (geo.dyn > (uint32_t)e->max_smem_optin) return PGS_NOT_SUPPORTED;
-    geo.apply(P);
+    GetParams P{};
+    P.n = n; P.now = now; P.data_version = part.data_version;
+    ReadLaunch<GetParams> L;
+    if ((rc = get_plan(P, R, e->max_smem_optin, L)) != PGS_OK) return rc;
     PGS_CUDA(cudaSetDevice(e->device));
     cudaStream_t st = e->read_stream();
-    const uint64_t key_bytes = key_off[n];
     LaunchScratch S(st);
     cudaEvent_t ev_a, ev_b;
-    uint8_t *d_keys = nullptr;
     PGS_CUDA(S.event(ev_a));
     PGS_CUDA(S.event(ev_b));
-    PGS_CUDA(S.alloc(d_keys, key_bytes + 16));
-    PGS_CUDA(cudaMemcpyAsync(d_keys, keys, key_bytes, cudaMemcpyHostToDevice, st));
-    PGS_CUDA(S.upload(P.key_off, key_off, n + 1));
-    PGS_CUDA(S.alloc(P.results, sizeof(pgs_get_result) * n));
-    PGS_CUDA(S.alloc(P.arena, arena_cap + 16));
-    PGS_CUDA(S.alloc(P.arena_cursor, 32));
-    PGS_CUDA(S.alloc(P.error, 16));
-    PGS_CUDA(cudaMemsetAsync(P.arena_cursor, 0, 32, st));
-    PGS_CUDA(cudaMemsetAsync(P.error, 0, 16, st));
-    if (key_part) {
-        PGS_CUDA(S.upload(P.multi_runs, M.packed.data(), M.packed.size()));
-        PGS_CUDA(S.upload(P.multi_begin, M.begin.data(), M.begin.size()));
-        PGS_CUDA(S.upload(P.key_part, key_part, n));
-    }
-    P.keys = d_keys; P.n = n; P.now = now; P.data_version = part.data_version;
-    P.arena_cap = arena_cap; P.ticket = P.error + 1;
-    int occ = 0;
-    auto kern = key_part ? k_get<8, true> : k_get<8, false>;
-    PGS_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, (int)kReadThreads, (size_t)geo.dyn));
-    const uint32_t per_cta = kReadThreads / geo.G;
-    const uint32_t grid = std::min<uint32_t>((n + per_cta - 1) / per_cta, (uint32_t)std::max(1, occ) * e->sm_count);
+    cudaError_t ce = cudaSuccess;
+    get_buffers(P, R, keys, key_off, key_part, arena_cap, device_buffers(S, ce));
+    PGS_CUDA(ce);
+    uint64_t ctas = 0;
+    PGS_CUDA(resident_ctas(*e, L, ctas));
     PGS_CUDA(cudaEventRecord(ev_a, st));
-    kern<<<grid, kReadThreads, geo.dyn, st>>>(P);
+    read_launch(L, P, ctas, st);
     PGS_CUDA(cudaEventRecord(ev_b, st));
     e->launches++;
     // hot-key capture (only while a slot's READ collector is active): its fine tickets and indices come back with the results
     std::vector<uint32_t> hk_tickets, hk_idx;
     if (hk.any) {
         HotkeyParams H{};
-        H.keys = d_keys; H.key_off = P.key_off; H.key_part = key_part ? P.key_part : nullptr; H.n = n; H.n_buckets = hk.n_buckets;
+        H.keys = P.keys; H.key_off = P.key_off; H.key_part = P.key_part; H.n = n; H.n_buckets = hk.n_buckets;
         const uint32_t n_slots = (uint32_t)hk.slots.size();
         PGS_CUDA(S.upload(H.slots, hk.slots.data(), n_slots));
         PGS_CUDA(S.alloc(H.tickets, sizeof(uint32_t) * (n_slots + (size_t)hk.total_room)));
@@ -512,11 +409,11 @@ static int32_t get_batch_impl(pgs_partition *const *parts, uint32_t n_parts, con
     const unsigned long long used = cur3[0];
     if (arena_used) *arena_used = used;
     if (!herr && used) {
-        PGS_CUDA(cudaMemcpyAsync(arena, P.arena, std::min<unsigned long long>(used, arena_cap), cudaMemcpyDeviceToHost, st));
+        PGS_CUDA(cudaMemcpyAsync(arena, P.arena, std::min<unsigned long long>(used, P.arena_cap), cudaMemcpyDeviceToHost, st));
         PGS_CUDA(cudaStreamSynchronize(st));
     }
     if (herr) { set_error("get kernel failed with status %u", herr); return herr == PGS_CORRUPTION ? PGS_CORRUPTION : PGS_IO_ERROR; }
-    return used > arena_cap ? PGS_INCOMPLETE : PGS_OK;
+    return used > P.arena_cap ? PGS_INCOMPLETE : PGS_OK;
 }
 
 // pgs_get_batch, with the READ collector's capture switched on or off (handlers that capture with their own weights)
@@ -549,7 +446,7 @@ extern "C" int32_t pgs_range_scan(pgs_partition *ph, const pgs_scan_request *req
                                   uint32_t resume_cap, pgs_scan_result *out)
 {
     if (!ph || !req || !out) return PGS_INVALID_ARGUMENT;
-    return scan_many(ph->p, req, 1, now, arena_cap, kv_cap, arena, arena_cap, kvs, kv_cap, resume_key, resume_cap, out, nullptr, nullptr, nullptr);
+    return scan_many(&ph, 1, nullptr, req, 1, now, out, ScanOut{arena, arena_cap, arena_cap, kvs, kv_cap, kv_cap, resume_key, resume_cap, nullptr, nullptr});
 }
 
 extern "C" int32_t pgs_range_scan_many(pgs_partition *ph, const pgs_scan_request *reqs, uint32_t n, uint32_t now,
@@ -558,8 +455,8 @@ extern "C" int32_t pgs_range_scan_many(pgs_partition *ph, const pgs_scan_request
                                        pgs_scan_result *results, uint64_t *arena_base, uint32_t *kv_base)
 {
     if (!ph || (n && (!reqs || !results))) return PGS_INVALID_ARGUMENT;
-    return scan_many(ph->p, reqs, n, now, arena_stride, kv_stride, arena, arena_cap, kvs, kv_cap, resume_keys, resume_stride, results,
-                     arena_base, kv_base, nullptr);
+    return scan_many(&ph, 1, nullptr, reqs, n, now, results,
+                     ScanOut{arena, arena_stride, arena_cap, kvs, kv_stride, kv_cap, resume_keys, resume_stride, arena_base, kv_base});
 }
 
 extern "C" int32_t pgs_range_scan_many_multi(pgs_partition *const *parts, uint32_t n_parts, const pgs_scan_request *reqs, const uint32_t *req_part,
@@ -570,6 +467,6 @@ extern "C" int32_t pgs_range_scan_many_multi(pgs_partition *const *parts, uint32
     if (!parts || !n_parts || (n && (!reqs || !req_part || !results))) return PGS_INVALID_ARGUMENT;
     for (uint32_t p = 0; p < n_parts; p++)
         if (!parts[p]) return PGS_INVALID_ARGUMENT;
-    return scan_many_multi(parts, n_parts, reqs, req_part, n, now, arena_stride, kv_stride, arena, arena_cap, kvs, kv_cap, resume_keys,
-                           resume_stride, results, arena_base, kv_base);
+    return scan_many(parts, n_parts, req_part, reqs, n, now, results,
+                     ScanOut{arena, arena_stride, arena_cap, kvs, kv_stride, kv_cap, resume_keys, resume_stride, arena_base, kv_base});
 }

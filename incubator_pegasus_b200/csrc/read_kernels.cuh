@@ -636,4 +636,138 @@ inline scan_fwd_kernel_t scan_fwd_kernel(uint32_t G, bool multi)
     return k[G == 8 ? 0 : G == 16 ? 1 : 2][multi ? 1 : 0];
 }
 
+// ---- the read launch plan: what the library (lookup.cu) and the simulator (tools/simt) both launch ------------------------------
+void set_error(const char *fmt, ...); // the message of a refused call (engine.cu; the simulator prints it)
+
+// the largest block of a launch's runs, in bytes and in records (k_scan's staging pool, scan_kernel.cuh)
+struct ScanBlockBound {
+    uint32_t max_blk = 0, max_rec = 0;
+    void add(const pgs_run_info &i) { max_blk = std::max(max_blk, i.max_block_size); max_rec = std::max(max_rec, i.max_block_records); }
+};
+
+// The runs of one read launch.  A call with a key / request slot index (multi) uses the MULTI instantiations, even with one
+// slot: slot s reads packed[begin[s] .. begin[s + 1]) and rr holds dummies (multi_read_runs).  Any other call reads its one
+// slot's runs from the kernels' shared-memory table rr.  KS = the launch's key slot, bb = the largest block of its runs.
+struct ReadRunSet {
+    bool multi = false;
+    ReadRuns rr{};
+    uint32_t KS = 8;
+    ScanBlockBound bb;
+    std::vector<RunDev> packed;
+    std::vector<uint32_t> begin{0};
+    bool empty() const { return packed.empty(); } // every iterator is invalid from the start: no launch
+};
+// slots = one run list (newest first) per partition slot, of runs with dev() and info (the library's Run, the simulator's
+// HostRun).  PGS_NOT_SUPPORTED when a slot has more than kMaxReadRuns runs or a user key longer than kMaxUkeyLen.
+template <class Slots>
+inline int32_t read_run_set(const Slots &slots, bool multi, ReadRunSet &R)
+{
+    R.multi = multi;
+    uint32_t mk = 0;
+    for (const auto &runs : slots) {
+        if (runs.size() > kMaxReadRuns) {
+            set_error("read: %zu runs > %u (compact first)", runs.size(), kMaxReadRuns);
+            return PGS_NOT_SUPPORTED;
+        }
+        uint32_t slot_mk = 0;
+        for (const auto &r : runs) {
+            R.packed.push_back(r->dev());
+            R.bb.add(r->info);
+            slot_mk = std::max(slot_mk, r->info.max_ukey_len);
+        }
+        if (slot_mk > kMaxUkeyLen) return PGS_NOT_SUPPORTED;
+        mk = std::max(mk, slot_mk);
+        R.begin.push_back((uint32_t)R.packed.size());
+    }
+    R.KS = read_key_slot(mk);
+    if (multi) multi_read_runs(R.packed, R.begin, R.rr);
+    else { R.rr.n = (uint32_t)R.packed.size(); std::copy(R.packed.begin(), R.packed.end(), R.rr.runs); }
+    return PGS_OK;
+}
+
+// the kernel of a read launch, its block size and dynamic shared memory, and how many requests one CTA takes
+template <class Params>
+struct ReadLaunch {
+    void (*kernel)(const Params);
+    uint32_t threads, dyn, per_cta;
+};
+// launches L over P.n requests on at most max_ctas CTAs (the library: as many as the device holds at once)
+template <class Params>
+inline void read_launch(const ReadLaunch<Params> &L, const Params &P, uint64_t max_ctas, cudaStream_t st)
+{
+    const uint32_t grid = (uint32_t)std::min<uint64_t>((P.n + L.per_cta - 1) / L.per_cta, max_ctas);
+    PGS_LAUNCH(L.kernel, grid, L.threads, L.dyn, st, P);
+}
+
+// k_get over the runs R: P's runs and key rows; PGS_NOT_SUPPORTED when the key rows do not fit the device's shared memory
+inline int32_t get_plan(GetParams &P, const ReadRunSet &R, uint32_t max_smem_optin, ReadLaunch<GetParams> &L)
+{
+    const ReadGeometry geo = get_geometry(R.KS);
+    if (geo.dyn > max_smem_optin) return PGS_NOT_SUPPORTED;
+    P.rr = R.rr;
+    geo.apply(P);
+    L = {R.multi ? k_get<8, true> : k_get<8, false>, kReadThreads, geo.dyn, kReadThreads / geo.G};
+    return PGS_OK;
+}
+
+// the initial content of a launch buffer: src_bytes copied from the host, or every byte set to fill, or none
+struct ReadInit {
+    const void *src = nullptr;
+    uint64_t src_bytes = 0;
+    int fill = kNoFill;
+};
+constexpr ReadInit kZero{nullptr, 0, 0};
+
+// the buffers of a multi-partition launch: its packed runs, their slot bounds, and the slot of each of its n requests
+template <class F>
+inline void multi_buffers(const ReadRunSet &R, const RunDev *&runs, const uint32_t *&begin, const uint32_t *&part, const uint32_t *req_part,
+                          uint64_t n, F &&buf)
+{
+    if (!R.multi) return;
+    buf(runs, sizeof(RunDev) * R.packed.size(), ReadInit{R.packed.data(), sizeof(RunDev) * R.packed.size()});
+    buf(begin, 4 * R.begin.size(), ReadInit{R.begin.data(), 4 * R.begin.size()});
+    buf(part, 4 * n, ReadInit{req_part, 4 * n});
+}
+
+// Every device buffer of a k_get launch (P.n set): buf(pointer, bytes, init) allocates the bytes and gives them their content.
+// The keys and the arena carry 16 bytes of slack; error[0] is the launch's status and error[1] its ticket counter.
+// pgs_get_result::value_off is 32-bit: a call uses at most the first 4 GiB - 1 of the arena.  A value that would end beyond
+// that gets PGS_INCOMPLETE like any value that does not fit, and arena_cursor[0] still reports the whole need.
+template <class F>
+inline void get_buffers(GetParams &P, const ReadRunSet &R, const uint8_t *keys, const uint32_t *key_off, const uint32_t *key_part,
+                        uint64_t arena_cap, F &&buf)
+{
+    const uint64_t n = P.n;
+    P.arena_cap = std::min<uint64_t>(arena_cap, UINT32_MAX);
+    buf(P.keys, key_off[n] + 16, ReadInit{keys, key_off[n]});
+    buf(P.key_off, 4 * (n + 1), ReadInit{key_off, 4 * (n + 1)});
+    buf(P.results, sizeof(pgs_get_result) * n, ReadInit{});
+    buf(P.arena, P.arena_cap + 16, ReadInit{});
+    buf(P.arena_cursor, 32, kZero);
+    buf(P.error, 16, kZero);
+    P.ticket = P.error + 1;
+    multi_buffers(R, P.multi_runs, P.multi_begin, P.key_part, key_part, n, buf);
+}
+
+// Every device buffer of a scan launch of the batch B (P.n and P.KS set), as get_buffers: the requests, and per request an
+// output slice of arena_stride bytes, kv_stride records and a resume slot (scan_output_strides), each array with 16 bytes of
+// slack.  Returns false when the resume slots are too short to report resume keys.
+template <class F>
+inline bool scan_buffers(ScanParams &P, const ReadRunSet &R, const ScanBatch &B, const uint32_t *req_part, unsigned long long arena_stride,
+                         uint32_t kv_stride, uint32_t resume_stride, F &&buf)
+{
+    const uint64_t n = P.n;
+    const bool report_resume = scan_output_strides(P, arena_stride, kv_stride, resume_stride);
+    buf(P.reqs, sizeof(ScanReqDev) * n, ReadInit{B.reqs.data(), sizeof(ScanReqDev) * n});
+    buf(P.blob, B.blob.size(), ReadInit{B.blob.data(), B.blob.size()});
+    buf(P.arena, P.arena_stride * n + 16, ReadInit{});
+    buf(P.kvs, sizeof(pgs_kv) * P.kv_stride * n + 16, ReadInit{});
+    buf(P.resume, (uint64_t)P.resume_stride * n + 16, ReadInit{});
+    buf(P.results, sizeof(pgs_scan_result) * n, ReadInit{});
+    buf(P.error, 16, kZero);
+    P.ticket = P.error + 1;
+    multi_buffers(R, P.multi_runs, P.multi_begin, P.req_part, req_part, n, buf);
+    return report_resume;
+}
+
 } // namespace pgs

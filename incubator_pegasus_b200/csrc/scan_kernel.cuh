@@ -759,12 +759,6 @@ __global__ void __launch_bounds__(kScanThreads, 4) k_scan(const __grid_constant_
 }
 
 // Host side (shared with the CPU simulation driver under tools/simt).
-// the largest block of a launch's runs, in bytes and in records
-struct ScanBlockBound {
-    uint32_t max_blk = 0, max_rec = 0;
-    void add(const pgs_run_info &i) { max_blk = std::max(max_blk, i.max_block_size); max_rec = std::max(max_rec, i.max_block_records); }
-};
-
 // what the device leaves k_scan for dynamic shared memory, given its opt-in limit and the kernel's static shared memory
 inline uint64_t scan_max_dyn(uint64_t max_smem_optin, uint64_t static_smem) { return max_smem_optin - static_smem - 256; }
 
@@ -792,6 +786,43 @@ inline uint64_t scan_dyn_bytes(uint32_t n_runs, uint32_t KS, uint32_t max_blk, u
     dyn &= ~127ull;
     *pool = (uint32_t)(dyn - fixed_dyn);
     return dyn;
+}
+
+// The kernel of a scan launch over the runs R (P.n set).  Forward batches: k_scan_fwd<G, multi>, the lane-group iterators of
+// read_kernels.cuh, unless the groups' key rows do not fit shared memory (user keys of a few KB).  A batch with a reverse
+// request, and a single-partition forward batch whose key rows do not fit: k_scan, which stages records instead of keeping
+// a key row per run and group.  max_smem_optin = the device's opt-in shared memory per CTA, scan_static = k_scan's static
+// shared memory.  Test knobs: force_G = k_scan_fwd's lanes per group (at least the run count), pool_cap = an upper bound on
+// k_scan's staging pool, never below scan_min_pool.
+inline int32_t scan_plan(ScanParams &P, const ReadRunSet &R, bool any_reverse, uint32_t max_smem_optin, uint64_t scan_static,
+                         ReadLaunch<ScanParams> &L, uint32_t force_G = 0, uint32_t pool_cap = 0)
+{
+    P.rr = R.rr;
+    P.KS = R.KS;
+    const ReadGeometry fwd = scan_fwd_geometry(R.rr.n, R.KS, force_G);
+    const bool fwd_fits = fwd.dyn <= max_smem_optin;
+    if (!fwd_fits && R.multi) {
+        set_error("scan: %u runs with keys of %u bytes do not fit shared memory", R.rr.n, R.KS);
+        return PGS_NOT_SUPPORTED;
+    }
+    if (!any_reverse && fwd_fits) {
+        if (fwd.G < R.rr.n) return PGS_INVALID_ARGUMENT;
+        fwd.apply(P);
+        L = {scan_fwd_kernel(fwd.G, R.multi), kReadThreads, fwd.dyn, kReadThreads / fwd.G};
+        return PGS_OK;
+    }
+    uint64_t dyn = scan_dyn_bytes(R.rr.n, R.KS, R.bb.max_blk, R.bb.max_rec, P.n, scan_max_dyn(max_smem_optin, scan_static), &P.pool_bytes);
+    if (!dyn) {
+        set_error("scan: blocks too large for shared memory");
+        return PGS_NOT_SUPPORTED;
+    }
+    if (pool_cap) {
+        const uint64_t fixed_dyn = dyn - P.pool_bytes;
+        P.pool_bytes = std::max(std::min(P.pool_bytes, pool_cap), (uint32_t)scan_min_pool(R.rr.n, R.KS, R.bb.max_blk, R.bb.max_rec));
+        dyn = fixed_dyn + P.pool_bytes;
+    }
+    L = {k_scan, kScanThreads, (uint32_t)dyn, 1};
+    return PGS_OK;
 }
 
 } // namespace pgs

@@ -32,12 +32,6 @@
 
 namespace pgs {
 
-int32_t scan_many(Partition &part, const pgs_scan_request *reqs, uint32_t n, uint32_t now, unsigned long long arena_stride,
-                  uint32_t kv_stride, uint8_t *arena, uint64_t arena_cap, pgs_kv *kvs, uint64_t kv_cap, uint8_t *resume,
-                  uint32_t resume_stride, pgs_scan_result *results, uint64_t *arena_base, uint32_t *kv_base,
-                  const std::vector<std::shared_ptr<Run>> *pinned);
-bool scan_stages_every_run(Partition &part);
-
 constexpr size_t kReadMaxRuns = 12; // a read-triggered flush compacts L0 once the run list grows past this
 
 struct Resp {
@@ -172,7 +166,7 @@ struct Server {
     }
     // range reads: the memtable becomes an L0 run, and L0 is folded once the run list grows past kReadMaxRuns, or when the
     // reverse-scan kernel could not stage one block of every run (many L0 runs of small records, such as tombstones)
-    bool needs_fold(bool reverse) { return runs().size() > kReadMaxRuns || (reverse && !scan_stages_every_run(part->p)); }
+    bool needs_fold(bool reverse) { return runs().size() > kReadMaxRuns || (reverse && !scan_stages_every_run(part)); }
     bool range_read_needs_prepare(bool reverse) { return !mem.empty() || needs_fold(reverse); }
     int32_t prepare_read(uint32_t now, bool reverse)
     {
@@ -232,8 +226,8 @@ struct Server {
             arena.resize(cap);
             kvs.resize(kv_cap);
             resume.assign(kMaxUkeyLen + 8, '\0');
-            int32_t st = scan_many(part->p, &rq, 1, now, cap, kv_cap, arena.data(), cap, kvs.data(), kv_cap, (uint8_t *)&resume[0],
-                                   (uint32_t)resume.size(), &res, nullptr, nullptr, pinned);
+            const ScanOut out{arena.data(), cap, cap, kvs.data(), kv_cap, kv_cap, (uint8_t *)&resume[0], (uint32_t)resume.size(), nullptr, nullptr};
+            int32_t st = scan_many(&part, 1, nullptr, &rq, 1, now, &res, out, pinned);
             if (st == PGS_ABORTED && cap < (4ull << 30)) { // the result did not fit the arena or the record table: grow both
                 cap *= 8;
                 if (!rq.count_only && kv_cap < rq.max_count) kv_cap = (uint32_t)std::min<uint64_t>((uint64_t)kv_cap * 8, rq.max_count);

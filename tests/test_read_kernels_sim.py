@@ -106,11 +106,11 @@ def test_sim_get_multi_partition(pgs, sim):
     assert hits > 30
 
 
-def do_scans(pgs, sim, args, reqs, lanes=0, pool=0):
+def do_scans(pgs, sim, args, reqs, lanes=0, pool=0, rstride=512):
     n = len(reqs)
     keep = []
     arr = scan_requests(pgs, reqs, keep)
-    astride, kstride, rstride = 1 << 16, 512, 512
+    astride, kstride = 1 << 16, 512
     arena = np.zeros(astride * n, np.uint8)
     kvs = (pgs.KV * (kstride * n))()
     resume = np.zeros(rstride * n, np.uint8)
@@ -131,16 +131,20 @@ def check_scans(vis, reqs, got):
 SCAN_HKS = [b"h%d" % i for i in range(7)] + [b"", b"h1x", bytes([0xff, 0xff])]
 
 
-@pytest.mark.parametrize("n_runs,lanes", [(4, 0), (1, 0), (6, 16), (3, 32)])
-def test_sim_scan_forward(pgs, sim, n_runs, lanes):
+@pytest.mark.parametrize("n_runs,lanes,long_keys", [(4, 0, False), (1, 0, False), (6, 16, False), (3, 32, False), (2, 0, True)],
+                         ids=["4-0", "1-0", "6-16", "3-32", "2-0-3k_keys"])
+def test_sim_scan_forward(pgs, sim, n_runs, lanes, long_keys):
+    """long_keys: a hash key of 3000 bytes, whose key rows do not fit k_scan_fwd's shared memory: the forward batch runs
+    through k_scan, as in the library"""
     rng = np.random.default_rng(100 + n_runs)
-    runs, items = make_db(pgs, rng, n_runs, SCAN_HKS, 30)
+    hks = SCAN_HKS[:3] + [b"L" * 3000] if long_keys else SCAN_HKS
+    runs, items = make_db(pgs, rng, n_runs, hks, 12 if long_keys else 30)
     vis, best = visible(items)
     args, keep = run_args(pgs, runs, block_size=512, ri=4)
     full = dict(start=b"", stop=b"\xff" * 4, start_inclusive=True, stop_inclusive=True, key_mode=0, max_count=1000, max_iter_count=1000,
                 max_iter_size=0)
-    reqs = scan_list(SCAN_HKS) + filter_list(full)
-    check_scans(vis, reqs, do_scans(pgs, sim, args, reqs, lanes))
+    reqs = scan_list(hks) + filter_list(full)
+    check_scans(vis, reqs, do_scans(pgs, sim, args, reqs, lanes, rstride=4096 if long_keys else 512))
 
 
 @pytest.mark.parametrize("pool", ["product", "minimal"])

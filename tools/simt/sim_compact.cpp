@@ -10,12 +10,24 @@
 #include "../../incubator_pegasus_b200/csrc/read_kernels.cuh"
 #include "../../incubator_pegasus_b200/csrc/scan_kernel.cuh"
 
+#include <cstdarg>
 #include <memory>
 #include <new>
 #include <string>
 #include <vector>
 
 using namespace pgs;
+
+// the message of a call the read launch plan refuses (the library keeps it for pgs_last_error)
+void pgs::set_error(const char *fmt, ...)
+{
+    va_list ap;
+    va_start(ap, fmt);
+    fputs("sim: ", stderr);
+    vfprintf(stderr, fmt, ap);
+    fputc('\n', stderr);
+    va_end(ap);
+}
 
 namespace {
 
@@ -211,109 +223,118 @@ uint32_t sim_run_bloom(const uint8_t *data, uint64_t data_bytes, const uint64_t 
 }
 
 static bool load_runs(uint32_t k, const uint8_t **data, const uint64_t *data_bytes, const uint64_t **blk_off, const uint32_t **blk_size,
-                      const uint32_t *n_blocks, std::vector<HostRun> &runs, ReadRuns &rr, uint32_t &max_ukey)
+                      const uint32_t *n_blocks, std::vector<HostRun> &runs)
 {
     runs.resize(k);
-    rr.n = k;
-    max_ukey = 0;
-    for (uint32_t i = 0; i < k; i++) {
+    for (uint32_t i = 0; i < k; i++)
         if (!load_run(runs[i], data[i], data_bytes[i], blk_off[i], blk_size[i], n_blocks[i])) return false;
-        rr.runs[i] = runs[i].dev();
-        max_ukey = std::max(max_ukey, runs[i].info.max_ukey_len);
-    }
     return true;
 }
 
+// The run set of a read launch over the loaded runs (newest first), as the library's snapshot builds it.  compacted: the run
+// of the last sim_compact call joins as the oldest run, with the index and filter k_emit wrote.  multi: the multi-partition
+// shape -- slot 0 owns the runs [0, k/2), slot 1 the rest, slot 2 is an empty partition.  bloom = false: the runs' filters
+// are left out.
+static int32_t read_slots(const std::vector<HostRun> &runs, bool compacted, bool multi, bool bloom, ReadRunSet &R)
+{
+    std::vector<const HostRun *> all;
+    for (const HostRun &r : runs) all.push_back(&r);
+    if (compacted) {
+        if (all.size() >= kMaxReadRuns || !g_res.st.tot_blocks) return PGS_INVALID_ARGUMENT;
+        all.push_back(&g_res.run);
+    }
+    const auto half = all.begin() + all.size() / 2;
+    const std::vector<std::vector<const HostRun *>> slots =
+        multi ? std::vector<std::vector<const HostRun *>>{{all.begin(), half}, {half, all.end()}, {}} : std::vector<std::vector<const HostRun *>>{all};
+    const int32_t rc = read_run_set(slots, multi, R);
+    auto no_bloom = [](RunDev &d) { d.bloom = nullptr; d.bloom_lines = 0; };
+    if (!bloom) {
+        for (RunDev &d : R.packed) no_bloom(d);
+        for (RunDev &d : R.rr.runs) no_bloom(d);
+    }
+    return rc;
+}
+
+// the buffers of a read launch (get_buffers, scan_buffers) in host memory at the library's sizes; what the library leaves
+// unset is poisoned until the kernels write it
+static auto host_buffers(HostMem &mem)
+{
+    return [&mem](auto *&p, uint64_t bytes, ReadInit in) {
+        uint8_t *b;
+        host_alloc(mem, b, bytes, in.fill == kNoFill ? 0xEE : in.fill);
+        if (in.src) memcpy(b, in.src, in.src_bytes);
+        p = (std::remove_reference_t<decltype(p)>)b;
+    };
+}
+
+// the slot of each of n requests in the multi-partition shape: request i belongs to slot i % 3
+static std::vector<uint32_t> slot_of_each(uint32_t n)
+{
+    std::vector<uint32_t> s(n);
+    for (uint32_t i = 0; i < n; i++) s[i] = i % 3;
+    return s;
+}
+
 // k_get over k runs (newest first); results / arena as pgs_get_batch.  stats[0] = arena bytes, [1] = blocks probed, [2] = runs skipped.
-// use_bloom: 1 = the runs' filters are used; 2 = the multi-partition shape (below); 4 = the last sim_compact output is the oldest run
+// use_bloom: 1 = the runs' filters are used; 2 = the multi-partition shape of pgs_get_batch_multi (read_slots; key i belongs to
+// slot i % 3); 4 = the last sim_compact output is the oldest run
 int32_t sim_get(uint32_t k, const uint8_t **data, const uint64_t *data_bytes, const uint64_t **blk_off, const uint32_t **blk_size,
                 const uint32_t *n_blocks, const uint8_t *keys, const uint32_t *key_off, uint32_t n, uint32_t now, uint8_t *arena,
                 uint64_t arena_cap, pgs_get_result *results, uint64_t *stats, uint32_t use_bloom)
 {
     std::vector<HostRun> runs;
+    if (!load_runs(k, data, data_bytes, blk_off, blk_size, n_blocks, runs)) return PGS_CORRUPTION;
+    ReadRunSet R;
+    if (const int32_t rc = read_slots(runs, use_bloom & 4, use_bloom & 2, use_bloom & 1, R)) return rc;
     GetParams P{};
-    uint32_t mk = 0;
-    if (!load_runs(k, data, data_bytes, blk_off, blk_size, n_blocks, runs, P.rr, mk)) return PGS_CORRUPTION;
-    if (use_bloom & 4) { // the run of the last sim_compact call joins as the oldest run, with the index and filter k_emit wrote
-        if (k >= kMaxReadRuns || !g_res.st.tot_blocks) return PGS_INVALID_ARGUMENT;
-        P.rr.runs[k] = g_res.run.dev();
-        mk = std::max(mk, g_res.run.info.max_ukey_len);
-        P.rr.n = ++k;
-    }
-    if (!(use_bloom & 1)) for (uint32_t i = 0; i < k; i++) { P.rr.runs[i].bloom = nullptr; P.rr.runs[i].bloom_lines = 0; }
-    std::vector<uint8_t> kcopy(keys, keys + key_off[n]);
-    kcopy.resize(kcopy.size() + 16); // the slack of the product's key buffer
-    unsigned long long cur[4] = {0, 0, 0, 0};
-    uint32_t err[4] = {0, 0, 0, 0};
-    P.keys = kcopy.data(); P.key_off = key_off; P.n = n; P.now = now; P.data_version = 1;
-    P.results = results; P.arena = arena; P.arena_cap = arena_cap; P.arena_cursor = cur; P.error = err; P.ticket = err + 1;
-    const ReadGeometry geo = get_geometry(read_key_slot(mk));
-    geo.apply(P);
-    // use_bloom & 2: the multi-partition shape of pgs_get_batch_multi -- slot 0 owns the runs [0, k/2), slot 1 the rest, slot 2
-    // is an empty partition; key i belongs to slot i % 3
-    std::vector<RunDev> packed(P.rr.runs, P.rr.runs + k);
-    std::vector<uint32_t> begin = {0, k / 2, k, k}, kp(n);
-    if (use_bloom & 2) {
-        for (uint32_t i = 0; i < n; i++) kp[i] = i % 3;
-        P.multi_runs = packed.data(); P.multi_begin = begin.data(); P.key_part = kp.data();
-        multi_read_runs(packed, begin, P.rr);
-    }
-    if (use_bloom & 2) PGS_LAUNCH((k_get<8, true>), 2, kReadThreads, geo.dyn, 0, P);
-    else PGS_LAUNCH((k_get<8, false>), 2, kReadThreads, geo.dyn, 0, P);
-    stats[0] = cur[0]; stats[1] = cur[1]; stats[2] = cur[2];
-    return err[0] ? (int32_t)err[0] : PGS_OK;
+    P.n = n; P.now = now; P.data_version = 1;
+    ReadLaunch<GetParams> L;
+    if (const int32_t rc = get_plan(P, R, kSimSmemOptin, L)) return rc;
+    HostMem mem;
+    get_buffers(P, R, keys, key_off, slot_of_each(n).data(), arena_cap, host_buffers(mem));
+    read_launch(L, P, 2, nullptr);
+    memcpy(results, P.results, sizeof(pgs_get_result) * n);
+    for (int i = 0; i < 3; i++) stats[i] = P.arena_cursor[i];
+    if (P.error[0]) return (int32_t)P.error[0];
+    memcpy(arena, P.arena, std::min<uint64_t>(P.arena_cursor[0], P.arena_cap));
+    return PGS_OK;
 }
 
-// range scans over k runs; outputs as the device side of scan_many (request i uses arena + i*arena_stride, kvs + i*kv_stride;
-// scan_output_strides rounds arena_stride up to a multiple of 16).
-// A batch without reverse requests runs k_scan_fwd, any other batch k_scan.  pool_bytes (k_scan only): 0 =
-// the pool the product gives a batch of n requests; otherwise at most pool_bytes, but never below the smallest pool
-// (scan_min_pool: one block of every run), so that a small value forces chunks of about one block.
+// range scans over k runs; outputs as the device side of scan_many: request i's answer at arena + i*arena_stride,
+// kvs + i*kv_stride and resume + i*resume_stride (scan_output_strides rounds arena_stride up to a multiple of 16; a resume
+// stride shorter than the key slot reports no resume key).  The kernel is scan_plan's choice.  lanes & 0xFF: k_scan_fwd's
+// lanes per group; lanes & 0x100: the multi-partition shape of pgs_range_scan_many_multi (read_slots; request i belongs to
+// slot i % 3).  pool_bytes (k_scan only): 0 = the pool the product gives a batch of n requests; otherwise at most pool_bytes,
+// but never below the smallest pool (scan_min_pool: one block of every run), so that a small value forces chunks of about
+// one block.
 int32_t sim_scan(uint32_t k, const uint8_t **data, const uint64_t *data_bytes, const uint64_t **blk_off, const uint32_t **blk_size,
                  const uint32_t *n_blocks, const pgs_scan_request *reqs, uint32_t n, uint32_t now, uint64_t arena_stride, uint32_t kv_stride,
                  uint8_t *arena, pgs_kv *kvs, uint8_t *resume, uint32_t resume_stride, pgs_scan_result *results, uint32_t lanes,
                  uint32_t pool_bytes)
 {
     std::vector<HostRun> runs;
-    ScanParams P{};
-    uint32_t mk = 0;
-    if (!load_runs(k, data, data_bytes, blk_off, blk_size, n_blocks, runs, P.rr, mk)) return PGS_CORRUPTION;
+    if (!load_runs(k, data, data_bytes, blk_off, blk_size, n_blocks, runs)) return PGS_CORRUPTION;
     const ScanBatch B = flatten_scan_requests(reqs, n);
-    uint32_t err[4] = {0, 0, 0, 0};
-    P.reqs = B.reqs.data(); P.blob = (const uint8_t *)B.blob.data(); P.n = n; P.now = now; P.data_version = 1;
-    P.results = results; P.kvs = kvs; P.arena = arena; P.resume = resume; P.error = err; P.ticket = err + 1;
-    P.KS = read_key_slot(mk);
-    scan_output_strides(P, arena_stride, kv_stride, resume_stride);
+    if (B.any_reverse && lanes) return PGS_INVALID_ARGUMENT; // k_scan has no lane groups and no multi-partition shape
+    ReadRunSet R;
+    if (const int32_t rc = read_slots(runs, false, lanes & 0x100, true, R)) return rc;
+    ScanParams P{};
+    P.n = n; P.now = now; P.data_version = 1;
     if (B.need_crc) { crc64_make_table(crc_tab); P.crc_table = (const unsigned long long *)crc_tab; }
-    if (B.any_reverse) {
-        if (lanes) return PGS_INVALID_ARGUMENT; // k_scan has no lane groups and no multi-partition shape
-        ScanBlockBound bb;
-        for (auto &r : runs) bb.add(r.info);
-        uint64_t dyn = scan_dyn_bytes(k, P.KS, bb.max_blk, bb.max_rec, n, scan_max_dyn(kSimSmemOptin, sizeof(ScanShared)), &P.pool_bytes);
-        if (!dyn) return PGS_NOT_SUPPORTED;
-        if (pool_bytes) {
-            const uint32_t fixed_dyn = (uint32_t)dyn - P.pool_bytes;
-            P.pool_bytes = std::max(std::min(P.pool_bytes, pool_bytes), (uint32_t)scan_min_pool(k, P.KS, bb.max_blk, bb.max_rec));
-            dyn = fixed_dyn + P.pool_bytes;
-        }
-        PGS_LAUNCH(k_scan, std::min(n, 3u), kScanThreads, dyn, 0, P);
-        return err[0] ? (int32_t)err[0] : PGS_OK;
+    ReadLaunch<ScanParams> L;
+    if (const int32_t rc = scan_plan(P, R, B.any_reverse, kSimSmemOptin, sizeof(ScanShared), L, lanes & 0xFF, pool_bytes)) return rc;
+    HostMem mem;
+    const bool report_resume = scan_buffers(P, R, B, slot_of_each(n).data(), arena_stride, kv_stride, resume_stride, host_buffers(mem));
+    read_launch(L, P, L.kernel == k_scan ? 3 : 2, nullptr);
+    memcpy(results, P.results, sizeof(pgs_scan_result) * n);
+    if (P.error[0]) return (int32_t)P.error[0];
+    for (uint64_t i = 0; i < n; i++) {
+        const pgs_scan_result &r = results[i];
+        memcpy(arena + i * P.arena_stride, P.arena + i * P.arena_stride, r.arena_used);
+        memcpy(kvs + i * kv_stride, P.kvs + i * kv_stride, sizeof(pgs_kv) * r.n_kvs);
+        if (report_resume && r.iter_valid) memcpy(resume + i * resume_stride, P.resume + i * P.resume_stride, r.resume_len);
     }
-    // lanes & 0x100: the multi-partition shape of pgs_range_scan_many_multi -- slot 0 owns the runs [0, k/2), slot 1 the rest,
-    // slot 2 is an empty partition; request i belongs to slot i % 3
-    const bool multi = (lanes & 0x100) != 0;
-    std::vector<RunDev> packed(P.rr.runs, P.rr.runs + k);
-    std::vector<uint32_t> begin = {0, k / 2, k, k}, rp(n);
-    if (multi) {
-        for (uint32_t i = 0; i < n; i++) rp[i] = i % 3;
-        P.multi_runs = packed.data(); P.multi_begin = begin.data(); P.req_part = rp.data();
-        multi_read_runs(packed, begin, P.rr);
-    }
-    const ReadGeometry geo = scan_fwd_geometry(P.rr.n, P.KS, lanes & 0xFF);
-    if (geo.G < P.rr.n) return PGS_INVALID_ARGUMENT;
-    geo.apply(P);
-    PGS_LAUNCH(scan_fwd_kernel(geo.G, multi), 2, kReadThreads, geo.dyn, 0, P);
-    return err[0] ? (int32_t)err[0] : PGS_OK;
+    return PGS_OK;
 }
 
 // k_hotkey_capture over n keys of n_slots partition slots (key_part null: every key is slot 0).  Per slot: state (0 off,
