@@ -25,10 +25,10 @@
 //                 32/G groups share a warp in lock step; there is no block-wide barrier anywhere.
 //   k_seg_scan    exclusive prefix of the per-segment output sizes (bytes, blocks, records, index-key bytes).
 //   k_emit        one warp per segment builds the output blocks in batches of up to 32 entries, one thread per entry:
-//                 entry heads (from the key-stream records) and values are gathered into a shared-memory buffer
-//                 (16-byte global loads, byte-exact placement) together with the restart arrays and padding of the
-//                 blocks that close, and each batch leaves with one bulk TMA store; the new run's index and Bloom filter
-//                 are written alongside.
+//                 a batch's key-stream records and values arrive in shared-memory stages by bulk TMA copies (one wait per
+//                 batch), entry heads and values are assembled byte-exact in an output buffer together with the restart
+//                 arrays and padding of the blocks that close, and each batch leaves with one bulk TMA store; the new
+//                 run's index and Bloom filter are written alongside.
 //   Output blocks stay contiguous and in key order; every segment starts a new block.
 #pragma once
 #include <algorithm>
@@ -155,6 +155,7 @@ struct MergeParams {
     uint32_t *out_bloom; // the new run's Bloom filter (zeroed by the host), out_bloom_lines lines of 64 bytes
     uint32_t out_bloom_lines;
     MergeStats *stats;
+    uint32_t emit_vstage; // k_emit's value stage per warp (bytes)
 };
 
 // ---- launch geometry and buffer bounds (host side; shared with the CPU simulation driver under tools/simt) -----------------
@@ -219,6 +220,21 @@ PGS_HD uint64_t walk_dyn_smem(uint32_t G, uint32_t group_smem, uint32_t k)
 {
     return walk_win_off(G, group_smem) + (uint64_t)(kWalkThreads / G) * walk_win_stride(k);
 }
+// k_emit's shared memory per warp, every part 16-aligned: output buffer (ob) | key-stream stage (ks) | value stage (vs) | the
+// stages' mbarrier | restart offsets.  The 32 bytes behind each buffer take the whole 16-byte chunks read or written past its end.
+PGS_HD uint32_t emit_vs_off(uint32_t ob, uint32_t ks) { return ob + 32 + ks + 32; }
+PGS_HD uint32_t emit_bar_off(uint32_t ob, uint32_t ks, uint32_t vs) { return emit_vs_off(ob, ks) + vs + 32; }
+PGS_HD uint32_t emit_rst_off(uint32_t ob, uint32_t ks, uint32_t vs) { return emit_bar_off(ob, ks, vs) + 16; }
+// The output buffer for a block buffer of bb bytes: at least one entry + the restart array of the block it closes, normally
+// 8 KB (a batch of ~28 entries).  The value stage is as large: it holds the 16-byte span of any entry's value (at most bb + 30
+// bytes) and rarely ends a batch before the output buffer does.  Returns k_emit's shared memory per warp (bb, ks < 2^24).
+PGS_HD uint32_t emit_warp_layout(uint32_t bb, uint32_t RI, uint32_t ks, uint32_t &ob)
+{
+    const uint32_t rst = 4 * (bb / (11 * RI) + 4); // the restart offsets of an open block (entries of at least 11 bytes)
+    const uint32_t ob_min = bb + rst + 256;
+    ob = ob_min < 8192 ? 8192u : ((ob_min + 15) & ~15u);
+    return (emit_rst_off(ob, ks, ob) + rst + 15) & ~15u;
+}
 // fills the derived fields of P (P.k, P.block_size, P.restart_interval must be set); false = not supported
 constexpr uint32_t kWalkMinG = 4; // default lanes per merge group (see group.cuh)
 // walk_groups = merge groups the device runs at the same time (0: not known yet, the default segment budget is used)
@@ -245,22 +261,29 @@ inline bool compact_geometry(MergeParams &P, const CompactTotals &T, uint32_t ma
     geo.walk_dyn = (uint32_t)walk_dyn_smem(geo.G, P.group_smem, k);
     const uint32_t hs = (2 * P.KS + 64 + 15) & ~15u;
     P.ks_stage = hs < 2048 ? 2048u : hs;
-    // k_emit per warp: an output assembly buffer (at least one block, normally 8 KB = a batch of ~28 entries), the key-stream
-    // stage, the restart offsets of the open block.  An entry that does not fit a block buffer gets a block of its own, written
-    // in place.
+    // k_emit per warp (emit_warp_layout): output buffer, key-stream stage, value stage, the stages' mbarrier, the restart offsets
+    // of the open block.  An entry that does not fit a block buffer gets a block of its own, written in place.
     const uint32_t RI = P.restart_interval;
-    uint32_t blk_buf = (P.block_size + 24 + 15) & ~15u;
-    if (blk_buf + 1024ull + P.ks_stage + 8ull * (blk_buf / (11 * RI) + 4) > max_smem) { // huge block_size: cut smaller blocks
-        if (max_smem < P.ks_stage + 8192) return false;
-        blk_buf = (uint32_t)(((max_smem - P.ks_stage - 1024) * 11ull / 20)) & ~15u;
+    uint32_t blk_buf = (uint32_t)std::min<uint64_t>((P.block_size + 24ull + 15) & ~15ull, max_smem & ~15u), ob = 0;
+    if (P.ks_stage > max_smem || emit_warp_layout(blk_buf, RI, P.ks_stage, ob) > max_smem) {
+        // huge block_size: cut smaller blocks, to the largest block buffer whose warp fits shared memory
+        uint32_t lo = 0, hi = blk_buf / 16; // lo * 16 fits (or is 0), hi * 16 does not
+        while (hi - lo > 1) {
+            const uint32_t mid = lo + (hi - lo) / 2;
+            if (emit_warp_layout(mid * 16, RI, P.ks_stage, ob) <= max_smem) lo = mid; else hi = mid;
+        }
+        if (lo * 16 < 1024) return false;
+        blk_buf = lo * 16;
         if (P.block_size > blk_buf - 24) P.block_size = blk_buf - 24;
     }
     P.blk_buf = blk_buf;
-    const uint32_t ob_min = blk_buf + 4 * (blk_buf / (11 * RI) + 4) + 256; // an entry + the restart array of the block it closes
-    P.emit_obuf = ob_min < 8192 ? 8192u : ((ob_min + 15) & ~15u);
-    P.emit_warp_smem = (uint32_t)((P.emit_obuf + 32ull + P.ks_stage + 32 + 4ull * (blk_buf / (11 * RI) + 4) + 15) & ~15ull);
-    geo.emit_warps = max_smem / P.emit_warp_smem;
-    if (geo.emit_warps > kEmitThreads / 32) geo.emit_warps = kEmitThreads / 32;
+    P.emit_warp_smem = emit_warp_layout(blk_buf, RI, P.ks_stage, P.emit_obuf);
+    P.emit_vstage = P.emit_obuf;
+    // warps per CTA: the most (up to 4) that fit shared memory once, unless CTAs that fit twice per SM run more warps in all
+    // (large blocks: two CTAs of 3 warps rather than one of 4)
+    const uint32_t w_once = std::min(max_smem / P.emit_warp_smem, kEmitThreads / 32);
+    const uint32_t w_twice = std::min((max_smem / 2) / P.emit_warp_smem, kEmitThreads / 32);
+    geo.emit_warps = 2 * w_twice > w_once ? w_twice : w_once;
     if (geo.emit_warps == 0) return false;
     geo.emit_dyn = geo.emit_warps * P.emit_warp_smem;
     // segments
@@ -1053,9 +1076,9 @@ PGS_DEV void store_chunk_part(uint8_t *dst16, uint4 v, uint32_t lo, uint32_t hi)
         }
     }
 }
-// one THREAD copies n bytes from global memory (any alignment, readable in whole 16-byte chunks inside [lim_lo, ...)) to shared
-// memory at dst (any alignment): 16-byte loads and stores, byte-exact at both ends.  Four loads are in flight per round trip.
-PGS_DEV void thread_copy_g2s(uint8_t *obuf16, uint32_t doff, const uint8_t *src, uint32_t n, const uint8_t *lim_lo)
+// one THREAD copies n bytes inside shared memory, from src (any alignment, readable in whole 16-byte chunks from the chunk before
+// the one src lies in) to obuf16 + doff (any alignment): 16-byte loads and stores, byte-exact at both ends, four loads at a time.
+PGS_DEV void thread_copy_s2s(uint8_t *obuf16, uint32_t doff, const uint8_t *src, uint32_t n)
 {
     if (n == 0) return;
     const uint32_t x0 = doff & ~15u;                   // first destination chunk
@@ -1063,11 +1086,11 @@ PGS_DEV void thread_copy_g2s(uint8_t *obuf16, uint32_t doff, const uint8_t *src,
     const uint32_t a = (uint32_t)((uintptr_t)A & 15);
     const uint4 *sp = reinterpret_cast<const uint4 *>(A - a);
     const uint4 zero = make_uint4(0u, 0u, 0u, 0u);
-    uint4 Pc = (const uint8_t *)sp >= lim_lo ? sp[0] : zero; // only its bytes before src could lie outside the run's buffer
+    uint4 Pc = sp[0];
     const uint32_t end = doff + n;
 #pragma unroll 1
     for (uint32_t x = x0; x < end; x += 64) {
-        uint4 nx[4];                                   // (reads at most 31 bytes past the value: run buffers carry slack)
+        uint4 nx[4];                                   // (reads at most the chunk after the one of src's last byte)
 #pragma unroll
         for (uint32_t j = 0; j < 4; j++) nx[j] = x + 16 * j < end ? sp[j + 1] : zero;
         sp += 4;
@@ -1119,20 +1142,25 @@ PGS_DEV void copy_bytes_s2s(uint8_t *dst, const uint8_t *src, uint32_t n)
 }
 
 // k_emit: one warp per segment, one THREAD per entry.  A batch of up to 32 descriptors is laid out with warp scans (block
-// membership, restart points, entry sizes, offsets inside the block, block starts); every thread builds its entry's head from
-// its key-stream record (varints | key bytes after the shared prefix | trailer), copies the value into the warp's output
-// buffer and adds the key (and a new hash-key prefix) to the run's Bloom filter; the threads standing on a block boundary
-// finish the previous block (restart array, padding, index entry); the batch's bytes leave with one bulk TMA store.  Blocks
-// of a segment are adjacent in the output run, so a batch's bytes are one contiguous range; the partial 16-byte chunk at its
-// end is carried into the next batch.
+// membership, restart points, entry sizes, offsets inside the block, block starts, places in the stages).  As soon as the batch
+// is fixed its key-stream records and values are brought into the stages by bulk copies that complete on one mbarrier, so the
+// batch waits for global memory once.  Then every thread builds its entry's head from its key-stream record (varints | key
+// bytes after the shared prefix | trailer), copies the value from the value stage into the warp's output buffer and adds the
+// key (and a new hash-key prefix) to the run's Bloom filter; the threads standing on a block boundary finish the previous
+// block (restart array, padding, index entry); the batch's bytes leave with one bulk TMA store, which the next batch waits
+// for only when it writes the output buffer after its own stages have landed.  Blocks of a segment are adjacent in the output
+// run, so a batch's bytes are one contiguous range; the partial 16-byte chunk at its end is carried into the next batch.
 
 // a warp's shared memory, its lane, and what it added to the filter (counted by lane 0)
 struct EmitWarp {
-    uint8_t *obuf;  // emit_obuf + 32 bytes: the output buffer
-    uint8_t *stage; // ks_stage + 32 bytes: the key-stream records of a batch
-    uint32_t *rst;  // restart offsets of the open block (it may span batches)
+    uint8_t *obuf;   // emit_obuf + 32 bytes: the output buffer
+    uint8_t *stage;  // ks_stage + 32 bytes: the key-stream records of a batch
+    uint8_t *vstage; // emit_vstage + 32 bytes: the values of a batch, each in the 16-byte-aligned span that covers it
+    uint64_t *bar;   // the mbarrier the bulk copies into both stages complete on
+    uint32_t *rst;   // restart offsets of the open block (it may span batches)
     uint32_t lane, lt; // lt: the lanes before mine
-    uint32_t RI, OB;   // restart interval, output buffer bytes
+    uint32_t RI, OB, VS; // restart interval, output buffer bytes, value stage bytes
+    uint32_t phase;  // the barrier's phase the next batch waits for
     uint32_t n_bloom_keys, n_bloom_prefixes;
 };
 PGS_DEV void emit_warp(EmitWarp &W, const MergeParams &P, uint8_t *ws, uint32_t lane)
@@ -1140,14 +1168,20 @@ PGS_DEV void emit_warp(EmitWarp &W, const MergeParams &P, uint8_t *ws, uint32_t 
     W.obuf = ws;
     W.RI = P.restart_interval;
     W.OB = P.emit_obuf;
+    W.VS = P.emit_vstage;
     W.stage = ws + W.OB + 32;
-    W.rst = (uint32_t *)(W.stage + P.ks_stage + 32);
+    W.vstage = ws + emit_vs_off(W.OB, P.ks_stage);
+    W.bar = (uint64_t *)(ws + emit_bar_off(W.OB, P.ks_stage, W.VS));
+    W.rst = (uint32_t *)(ws + emit_rst_off(W.OB, P.ks_stage, W.VS));
     W.lane = lane;
     W.lt = (1u << lane) - 1u;
+    W.phase = 0;
     W.n_bloom_keys = W.n_bloom_prefixes = 0;
+    if (lane == 0) { mbar_init(W.bar, 1); mbar_fence_init(); }
+    __syncwarp();
 }
 
-// what a warp carries across the batches of a segment (warp-uniform)
+// what a warp carries across the batches of a segment (warp-uniform, except cv: each lane holds its own byte of the carry)
 struct EmitSeg {
     const Desc *desc;
     const uint8_t *ks;              // the segment's key stream
@@ -1156,7 +1190,8 @@ struct EmitSeg {
     uint32_t fill, blk_n, blk_rec0; // entry bytes / entries of the open block, its first record
     bool open;
     uint32_t blk_idx, rec_idx, keyb, kpos; // the next block, record and index-key byte; the next record in the key stream
-    uint32_t carry;                 // obuf[0, carry) = the bytes of the partial 16-byte chunk in front of the write position
+    uint32_t carry;                 // the bytes of the partial 16-byte chunk in front of the write position
+    uint8_t cv;                     // PER LANE: its byte number `lane` (lane < carry), which obuf_reclaim puts back at obuf[lane]
     uint32_t last_key_off, last_ulen; // the previous entry's user key in the key stream (the index key of a block it ends)
 };
 PGS_DEV void emit_seg(EmitSeg &S, const MergeParams &P, uint32_t q, const SegAgg &A, const SegBase &B)
@@ -1168,7 +1203,7 @@ PGS_DEV void emit_seg(EmitSeg &S, const MergeParams &P, uint32_t q, const SegAgg
     S.fill = 0; S.blk_n = 0; S.blk_rec0 = B.recs;
     S.open = false;
     S.blk_idx = B.blocks; S.rec_idx = B.recs; S.keyb = B.keyb; S.kpos = 0;
-    S.carry = 0;
+    S.carry = 0; S.cv = 0;
     S.last_key_off = 0; S.last_ulen = 0;
 }
 
@@ -1197,20 +1232,28 @@ PGS_DEV void close_open(const MergeParams &P, EmitSeg &S, const EmitWarp &W, con
     S.blk_start += asz;
     S.fill = 0; S.blk_n = 0; S.open = false;
 }
-// write obuf[0, bytes) to the run at the 16-aligned global offset gpos (bytes % 16 == 0), wait until it has been read
+// send obuf[0, bytes) to the run at the 16-aligned global offset gpos (bytes % 16 == 0) without waiting: obuf_reclaim waits
+// until the store has read it
 PGS_DEV void flush(const MergeParams &P, const EmitWarp &W, unsigned long long gpos, uint32_t bytes)
 {
     __syncwarp();
     if (bytes) {
         fence_proxy_async();
         __syncwarp();
-        if (W.lane == 0) { tma_store_1d(P.out_data + gpos, W.obuf, bytes); tma_store_commit(); tma_store_wait_read0(); }
-        __syncwarp();
+        if (W.lane == 0) { tma_store_1d(P.out_data + gpos, W.obuf, bytes); tma_store_commit(); }
     }
+}
+// before the next write into obuf: wait until the last store has read it (lane 0 issued it), put the carried bytes back in front
+PGS_DEV void obuf_reclaim(const EmitSeg &S, const EmitWarp &W)
+{
+    if (W.lane == 0) tma_store_wait_read0();
+    __syncwarp();
+    if (W.lane < S.carry) W.obuf[W.lane] = S.cv;
 }
 // close the open block and send what obuf still holds of it
 PGS_DEV void finish_open(const MergeParams &P, EmitSeg &S, const EmitWarp &W)
 {
+    obuf_reclaim(S, W);
     const unsigned long long obase = S.blk_start + S.fill - S.carry;
     close_open(P, S, W, S.ks + S.last_key_off, S.last_ulen, W.obuf + S.carry, restart_count(S.blk_n, W.RI));
     flush(P, W, obase, (uint32_t)(S.blk_start - obase));
@@ -1243,7 +1286,8 @@ struct EmitBatch {
     uint32_t hm_all, cnt;                 // the heads among the candidates; the entries of the batch (lanes 0..cnt-1)
     uint32_t n_i, sh_out, kd, hl, sz, sb; // my index in my block, shared / non-shared key bytes, head and entry bytes, record bytes
     uint32_t ps_incl, ss_incl;            // entry / record bytes of the lanes at or before me
-    // stage_records
+    uint32_t vs, vs_incl;                 // the 16-byte span that covers my value (0: no value); spans of the lanes at or before me
+    // stage_batch
     uint32_t total_s;                     // the batch's key-stream bytes
     const uint8_t *staged;                // the batch's first record in the stage
     // batch_offsets
@@ -1317,26 +1361,39 @@ PGS_DEV uint32_t batch_fit(const MergeParams &P, const EmitSeg &S, const EmitWar
     b.hl = entry_head_len(b.sh_out, b.kd, b.vl);
     b.sz = b.cand ? b.hl + b.vl : 0u;
     b.sb = b.cand ? ks_record(b.fl, b.ulen) : 0u;
+    const unsigned long long voff = desc_voff(b.loc);
+    b.vs = b.cand && b.vl ? (uint32_t)(((voff + b.vl + 15) & ~15ull) - (voff & ~15ull)) : 0u;
     b.ps_incl = warp_incl_scan(b.sz, lane);
     b.ss_incl = warp_incl_scan(b.sb, lane);
+    b.vs_incl = warp_incl_scan(b.vs, lane);
     // room: the entries, the restart arrays and paddings of the blocks that close here (the carried block brings its earlier
     // restart points along), the carried partial chunk
     const uint32_t room = S.carry + 32 * (lane + 1) + 64 + (S.open ? 4 * restart_count(S.blk_n, RI) : 0u);
-    const bool fits = b.cand && room + b.ps_incl <= W.OB && b.ss_incl <= P.ks_stage;
+    const bool fits = b.cand && room + b.ps_incl <= W.OB && b.ss_incl <= P.ks_stage && b.vs_incl <= W.VS;
     b.cnt = (uint32_t)__popc(__ballot_sync(kFull, fits)); // monotone: lanes 0..cnt-1
     b.mine = lane < b.cnt;
     return b.cnt;
 }
-// Fetch the next batch's descriptors, start staging this batch's key-stream records.
-PGS_DEV void stage_records(const EmitSeg &S, const EmitWarp &W, EmitBatch &b, uint32_t e0, uint4 &dn, uint32_t &dn_e0)
+// Fetch the next batch's descriptors; start the bulk copies of this batch into the stages, all completing on the warp's
+// barrier: lane 0 copies the 16-byte-aligned range that covers the batch's key-stream records, every lane of the batch the span
+// of its value (both read up to 15 bytes before and after what they cover, inside the allocation and its slack).  The barrier
+// expects the bytes of all of them before any is issued.
+PGS_DEV void stage_batch(const MergeParams &P, const EmitSeg &S, const EmitWarp &W, EmitBatch &b, uint32_t e0, uint4 &dn, uint32_t &dn_e0)
 {
     dn_e0 = e0 + b.cnt;
     dn = dn_e0 + W.lane < S.n ? *reinterpret_cast<const uint4 *>(&S.desc[dn_e0 + W.lane]) : make_uint4(0u, 0u, 0u, 0u);
     b.total_s = __shfl_sync(kFull, b.ss_incl, (int)b.cnt - 1);
+    const uint32_t total_v = __shfl_sync(kFull, b.vs_incl, (int)b.cnt - 1);
     const uint8_t *src = S.ks + S.kpos;
-    const uint32_t a = (uint32_t)((uintptr_t)src & 15);
-    for (uint32_t i = W.lane * 16; i < a + b.total_s; i += 512) async_copy16(W.stage + i, src - a + i);
-    async_copy_commit();
+    const uint32_t a = (uint32_t)((uintptr_t)src & 15), ks_bytes = (a + b.total_s + 15) & ~15u;
+    fence_proxy_async(); // the last batch's reads of the stages come before the copies that overwrite them
+    if (W.lane == 0) mbar_expect_tx(W.bar, ks_bytes + total_v);
+    __syncwarp();
+    if (W.lane == 0) tma_load_1d(W.stage, src - a, ks_bytes, W.bar);
+    if (b.mine && b.vs) {
+        const unsigned long long voff = desc_voff(b.loc);
+        tma_load_1d(W.vstage + (b.vs_incl - b.vs), P.runs[desc_run(b.loc)].data + (voff & ~15ull), b.vs, W.bar);
+    }
 }
 // Offsets and block starts: where my entry goes, the block a head closes, the index key of that block (the user key of the
 // entry before the head).
@@ -1394,8 +1451,8 @@ PGS_DEV void write_entries(const MergeParams &P, EmitWarp &W, const EmitBatch &b
         const uint32_t p = put_entry_varints(dst, b.sh_out, b.kd, b.vl);
         copy_bytes_s2s(dst + p, key + b.sh_out, b.kd);
         copy_bytes_s2s(dst + p + b.kd, rec, 8u);
-        const RunDev &r = P.runs[desc_run(b.loc)];
-        thread_copy_g2s(W.obuf, b.o_i + b.hl, r.data + desc_voff(b.loc), b.vl, r.data);
+        // from its span in the value stage (the chunk in front of a span is the one before it, or the key-stream stage's slack)
+        thread_copy_s2s(W.obuf, b.o_i + b.hl, W.vstage + (b.vs_incl - b.vs) + (uint32_t)(desc_voff(b.loc) & 15), b.vl);
         if ((b.fl & DF_REWRITE) && b.vl >= 4) { dst[b.hl] = rec[8]; dst[b.hl + 1] = rec[9]; dst[b.hl + 2] = rec[10]; dst[b.hl + 3] = rec[11]; }
         new_prefix = bloom_add(P, reinterpret_cast<const uint32_t *>(key), b.ulen, b.lcp);
     }
@@ -1437,7 +1494,7 @@ PGS_DEV void close_blocks(const MergeParams &P, const EmitSeg &S, const EmitWarp
         for (uint32_t x = lane; x < klen_b; x += 32) P.out_ikeys[ko_b + x] = pk[x];
     }
 }
-// Carry the state over to the next batch, send the batch's whole 16-byte chunks, move the partial one to the front of obuf.
+// Carry the state over to the next batch, send the batch's whole 16-byte chunks, keep the partial one in the lanes' cv.
 PGS_DEV void carry_over(const MergeParams &P, EmitSeg &S, const EmitWarp &W, const EmitBatch &b)
 {
     const uint32_t lane = W.lane;
@@ -1456,13 +1513,11 @@ PGS_DEV void carry_over(const MergeParams &P, EmitSeg &S, const EmitWarp &W, con
     const uint32_t used = (uint32_t)(wpos - b.obase), whole = used & ~15u;
     flush(P, W, b.obase, whole);
     S.carry = used - whole;
-    const uint8_t cv = lane < S.carry ? W.obuf[whole + lane] : (uint8_t)0;
-    __syncwarp();
-    if (lane < S.carry) W.obuf[lane] = cv;
-    __syncwarp();
+    S.cv = lane < S.carry ? W.obuf[whole + lane] : (uint8_t)0;
 }
 
-__global__ void __launch_bounds__(kEmitThreads, 5) k_emit(const __grid_constant__ MergeParams P)
+// three CTAs per SM: what shared memory allows with an 8 KB output buffer and an 8 KB value stage per warp
+__global__ void __launch_bounds__(kEmitThreads, 3) k_emit(const __grid_constant__ MergeParams P)
 {
     PGS_SMEM_DYN(dyn);
     const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -1488,11 +1543,12 @@ __global__ void __launch_bounds__(kEmitThreads, 5) k_emit(const __grid_constant_
             const uint32_t first_fl = __shfl_sync(kFull, b.fl, 0);
             if (first_fl & DF_BIG) { emit_big(P, S, W, b, first_fl); e0++; continue; }
             if (batch_fit(P, S, W, b) == 0) { err = PGS_ABORTED; break; }
-            stage_records(S, W, b, e0, dn, dn_e0);
+            stage_batch(P, S, W, b, e0, dn, dn_e0);
             batch_offsets(P, S, W, b);
-            async_copy_wait_upto(0);
-            __syncwarp();
+            mbar_wait(W.bar, W.phase); // the one wait of a batch for global memory
+            W.phase ^= 1;
             b.staged = W.stage + ((uintptr_t)(S.ks + S.kpos) & 15);
+            obuf_reclaim(S, W);
             restart_points(P, S, W, b);
             write_entries(P, W, b);
             __syncwarp();

@@ -27,13 +27,36 @@ constexpr int kNoFill = -1; // a launch buffer the host leaves unset (compact_bu
 
 // ---- shared-memory addressing / mbarrier / TMA bulk (cp.async.bulk) ----------------------------
 #ifdef PGS_SIM
+// The stand-ins check what the device would fault on or hang at: a bulk copy's addresses and size, and an mbarrier whose
+// expected bytes differ from the bytes its copies completed.  The barrier word holds the bytes expected and not yet arrived.
+#define PGS_SIM_CHECK(cond, ...) do { if (!(cond)) { fprintf(stderr, "sim: " __VA_ARGS__); fputc('\n', stderr); abort(); } } while (0)
+PGS_DEV void sim_check_bulk(const void *smem, const void *gmem, uint32_t bytes)
+{
+    PGS_SIM_CHECK(!((uintptr_t)smem & 15) && !((uintptr_t)gmem & 15) && !(bytes & 15) && bytes,
+                  "bulk copy of %u bytes between %p (shared) and %p (global): addresses must be 16-aligned, the size a multiple of 16",
+                  bytes, smem, gmem);
+}
 PGS_DEV void mbar_init(uint64_t *bar, uint32_t) { *bar = 0; }
 PGS_DEV void mbar_fence_init() {}
-PGS_DEV void mbar_expect_tx(uint64_t *, uint32_t) {}
-PGS_DEV bool mbar_try_wait(uint64_t *, uint32_t) { return true; }
-PGS_DEV void mbar_wait(uint64_t *, uint32_t) {}
-PGS_DEV void tma_load_1d(void *smem_dst, const void *gmem_src, uint32_t bytes, uint64_t *) { memcpy(smem_dst, gmem_src, bytes); }
-PGS_DEV void tma_store_1d(void *gmem_dst, const void *smem_src, uint32_t bytes) { memcpy(gmem_dst, smem_src, bytes); }
+PGS_DEV void mbar_expect_tx(uint64_t *bar, uint32_t bytes) { *bar += bytes; }
+PGS_DEV void mbar_wait(uint64_t *bar, uint32_t)
+{
+    PGS_SIM_CHECK(*bar == 0, "mbarrier wait with %lld expected bytes that no copy delivers", (long long)*bar);
+}
+PGS_DEV bool mbar_try_wait(uint64_t *bar, uint32_t parity) { mbar_wait(bar, parity); return true; }
+PGS_DEV void tma_load_1d(void *smem_dst, const void *gmem_src, uint32_t bytes, uint64_t *bar)
+{
+    sim_check_bulk(smem_dst, gmem_src, bytes);
+    PGS_SIM_CHECK((int64_t)(*bar - bytes) >= 0, "bulk copy of %u bytes completes on an mbarrier that expects %lld: expect_tx comes first",
+                  bytes, (long long)*bar);
+    memcpy(smem_dst, gmem_src, bytes);
+    *bar -= bytes;
+}
+PGS_DEV void tma_store_1d(void *gmem_dst, const void *smem_src, uint32_t bytes)
+{
+    sim_check_bulk(smem_src, gmem_dst, bytes);
+    memcpy(gmem_dst, smem_src, bytes);
+}
 PGS_DEV void tma_store_commit() {}
 PGS_DEV void tma_store_wait_read0() {}
 PGS_DEV void tma_store_wait_all() {}
