@@ -1424,10 +1424,20 @@ PGS_DEV void batch_offsets(const MergeParams &P, const EmitSeg &S, const EmitWar
     b.obase = S.blk_start + S.fill - S.carry;
     b.o_i = (uint32_t)(S.blk_start + b.base_i + b.fill_i - b.obase);
 }
-// Restart points: into obuf when my block closes in this batch, else into rst; my entry's offset into the index.
+// Restart points: into obuf when my block closes in this batch, else into rst; my entry's offset into the index.  When the
+// carried block closes here, its restart offsets from earlier batches leave rst first: the block that opens after it in this
+// batch puts its own into rst.
 PGS_DEV void restart_points(const MergeParams &P, const EmitSeg &S, const EmitWarp &W, const EmitBatch &b)
 {
     const uint32_t lane = W.lane, lt = W.lt, RI = W.RI;
+    const uint32_t first_close = __ffs((int)__ballot_sync(kFull, b.closes)) - 1; // lane of the first closing head (or ~0)
+    if (S.open && first_close < 32) {
+        const uint32_t Tc = __shfl_sync(kFull, b.T, (int)first_close);
+        const uint32_t have_r = restart_count(S.blk_n, RI); // restart points recorded before this batch
+        const uint32_t ro = (uint32_t)(S.blk_start - b.obase) + Tc;
+        for (uint32_t i = lane; i < 4 * have_r; i += 32) W.obuf[ro + i] = (uint8_t)(W.rst[i >> 2] >> (8 * (i & 3)));
+        __syncwarp();
+    }
     const uint32_t after = b.hm & ~(lt | (1u << lane));
     const int nh = after ? __ffs((int)after) - 1 : -1;                  // the head that closes my block inside this batch
     const uint32_t T_mine = __shfl_sync(kFull, b.T, nh >= 0 ? nh : 0); // my block's entry bytes, when it closes here
@@ -1459,19 +1469,11 @@ PGS_DEV void write_entries(const MergeParams &P, EmitWarp &W, const EmitBatch &b
     const uint32_t np = (uint32_t)__popc(__ballot_sync(kFull, new_prefix));
     if (P.out_bloom_lines) { W.n_bloom_keys += b.cnt; W.n_bloom_prefixes += np; }
 }
-// The heads finish the blocks that end in front of them: restart array, count, padding, index entry and index key.
+// The heads finish the blocks that end in front of them (their restart offsets are in place): count, padding, index entry
+// and index key.
 PGS_DEV void close_blocks(const MergeParams &P, const EmitSeg &S, const EmitWarp &W, const EmitBatch &b)
 {
     const uint32_t lane = W.lane;
-    const uint32_t first_close = __ffs((int)__ballot_sync(kFull, b.closes)) - 1; // lane of the first closing head (or ~0)
-    // the carried block's earlier restart offsets (from previous batches) go in front of this batch's
-    const bool carried_closes = S.open && first_close < 32;
-    if (carried_closes) {
-        const uint32_t Tc = __shfl_sync(kFull, b.T, (int)first_close);
-        const uint32_t have_r = restart_count(S.blk_n, W.RI); // restart points recorded before this batch
-        const uint32_t ro = (uint32_t)(S.blk_start - b.obase) + Tc;
-        for (uint32_t i = lane; i < 4 * have_r; i += 32) W.obuf[ro + i] = (uint8_t)(W.rst[i >> 2] >> (8 * (i & 3)));
-    }
     if (b.closes) {
         const uint32_t bstart = (uint32_t)(S.blk_start - b.obase) + (b.span_incl - b.asz_c); // obuf offset of the block I close
         uint32_t p = bstart + b.T + 4 * b.nrest_c;

@@ -124,6 +124,82 @@ def parse_blocks(br):
     return blocks
 
 
+def check_run_format(br, restart_interval, block_size):
+    """the block format of a merged run, which the decoders above do not read: for every block, its restart array (one
+    offset per restart_interval entries, each the offset of an entry that shares nothing with the one before, and their
+    count), the walker's cut rule (a block of more than one entry is at most block_size bytes: the effective, possibly cut,
+    size of emit_geometry), blocks 16-aligned and contiguous from offset 0, and zero padding between and behind them.
+    -> the entry count of every block"""
+    data = br.data.tobytes()
+    counts, pos = [], 0
+    for b, (off, size) in enumerate(zip(br.blk_off.tolist(), br.blk_size.tolist())):
+        assert off == pos, ("block not where the one before ends", b, off, pos)
+        assert off + size <= len(data) and size >= 4, (b, off, size)
+        blk = data[off:off + size]
+        nr = int.from_bytes(blk[-4:], "little")
+        limit = size - 4 - 4 * nr
+        assert limit >= 0, ("restart array larger than the block", b, nr, size)
+        rst = [int.from_bytes(blk[limit + 4 * i:limit + 4 * i + 4], "little") for i in range(nr)]
+        p, offs, shared = 0, [], []
+        while p < limit:
+            offs.append(p)
+            sh, p = _varint(blk, p)
+            ns, p = _varint(blk, p)
+            vl, p = _varint(blk, p)
+            shared.append(sh)
+            p += ns + vl
+        assert p == limit, ("entries overrun the restart array", b, p, limit)
+        n = len(offs)
+        assert n >= 1 and nr == (n + restart_interval - 1) // restart_interval, ("restart count", b, n, nr)
+        for i, r in enumerate(rst):
+            assert r == offs[i * restart_interval], ("restart offset", b, i, r, offs[i * restart_interval])
+            assert shared[i * restart_interval] == 0, ("restart point shares a prefix", b, i)
+        assert n == 1 or size <= block_size, ("block over the block size", b, n, size, block_size)
+        pos = (off + size + 15) & ~15
+        pad = data[off + size:min(pos, len(data))]
+        assert pad == bytes(len(pad)), ("padding not zero", b, pad.hex())
+        counts.append(n)
+    return counts
+
+
+def emit_warp_layout(bb, ri, ks):
+    """restates emit_warp_layout (compact_kernels.cuh): k_emit's shared memory per warp for a block buffer of bb bytes"""
+    rst = 4 * (bb // (11 * ri) + 4)
+    ob_min = bb + rst + 256
+    ob = 8192 if ob_min < 8192 else (ob_min + 15) & ~15
+    rst_off = ob + 32 + ks + 32 + ob + 32 + 16  # output buffer | key-stream stage | value stage (as large) | mbarrier
+    return (rst_off + rst + 15) & ~15
+
+
+def emit_geometry(block_size, ri, max_ukey, smem):
+    """restates the block-buffer rule of compact_geometry (compact_kernels.cuh) for a merge of user keys of at most max_ukey
+    bytes with `smem` bytes of shared memory per CTA (compact_smem_budget: the device's opt-in maximum less 1 KB).  A block
+    buffer holds a block and 24 bytes; when a warp's layout does not fit, the largest 16-byte multiple that fits is found by
+    bisection and the block size is cut to it.  -> dict(blk_buf, block_size: the effective one, warps: per CTA, twice: the
+    CTA fits an SM twice)"""
+    ks_row = 4 if max_ukey < 4 else (max_ukey + 3) & ~3
+    ks = max(2048, (2 * ks_row + 64 + 15) & ~15)
+    bb = min((block_size + 24 + 15) & ~15, smem & ~15)
+    bs = block_size
+    if ks > smem or emit_warp_layout(bb, ri, ks) > smem:
+        lo, hi = 0, bb // 16
+        while hi - lo > 1:
+            mid = lo + (hi - lo) // 2
+            if emit_warp_layout(mid * 16, ri, ks) <= smem:
+                lo = mid
+            else:
+                hi = mid
+        bb = lo * 16
+        bs = min(bs, bb - 24)
+    per_warp = emit_warp_layout(bb, ri, ks)
+    once, twice = min(smem // per_warp, 4), min((smem // 2) // per_warp, 4)
+    warps = twice if 2 * twice > once else once
+    return dict(blk_buf=bb, block_size=bs, warps=warps, twice=warps == twice)
+
+
+SIM_SMEM = 227 * 1024 - 1024  # the simulator's budget: an H100's opt-in shared memory per CTA less 1 KB
+
+
 class ModelRun:
     """one run as the lookup sees it: the newest version of every user key, the last user key, the filter"""
 

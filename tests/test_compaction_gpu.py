@@ -17,10 +17,13 @@ OPS_JSON = (
 
 
 def run_case(pgs, oracle, engine, runs, *, bottommost, now=synth.NOW, default_ttl=0, validate_hash=False, pidx=0,
-             partition_version=-1, ops_json=None, enabled=True):
+             partition_version=-1, ops_json=None, enabled=True, build=None, inspect=None):
+    """merge `runs` on the engine and compare with the oracle.  build = (block size, restart interval) of the input runs
+    (default: the host builder's); inspect(part, res, raw, want) runs on the merged run before the partition closes."""
     part = engine.partition()
     try:
-        ids = [part.upload_records(r) for r in runs]  # later upload = newer L0 run
+        ids = [part.upload(pgs.build_run(r, *build)) if build else part.upload_records(r) for r in runs]  # later upload = newer L0 run
+        part_bytes = [part.run_info(i).data_bytes for i in ids]
         ops_bin = pgs.parse_ops(ops_json) if ops_json else None
         res = part.compact(ids, out_level=1, bottommost=1 if bottommost else 0, now=now, enabled=enabled,
                            default_ttl=default_ttl, validate_hash=validate_hash, pidx=pidx,
@@ -45,7 +48,16 @@ def run_case(pgs, oracle, engine, runs, *, bottommost, now=synth.NOW, default_tt
             assert info.n_records == want.n
             assert info.raw_key_bytes == want.keys.shape[0]
             assert info.raw_value_bytes == want.vals.shape[0]
+            assert (info.level, info.n_tombstones) == (1, int(np.sum(want.type == 0)))
+            assert info.data_bytes == int(raw.blk_off[-1]) + ((int(raw.blk_size[-1]) + 15) & ~15)  # the last block, padded
+            assert info.max_ukey_len == int(np.diff(want.key_off.astype(np.int64)).max())
+            assert info.max_value_len == int(np.diff(want.val_off.astype(np.int64)).max())
+            assert info.max_block_size == int(raw.blk_size.max())
+            assert (info.smallest_seq, info.largest_seq) == (int(want.seq.min()), int(want.seq.max()))
+            assert res.out_block_bytes == raw.data.shape[0] and res.in_block_bytes == sum(part_bytes)
             assert part.runs() == [res.new_run_id]
+            if inspect:
+                inspect(part, res, raw, want)
         for f in ("in_records", "out_records", "in_bytes", "out_bytes", "dropped_shadowed", "dropped_tombstone",
                   "dropped_expired", "dropped_user", "dropped_stale", "ttl_rewritten"):
             assert getattr(res, f) == getattr(st, f), f

@@ -10,8 +10,9 @@ import subprocess
 import numpy as np
 import pytest
 
+import merge_inputs
+from get_model import SIM_SMEM, check_run_format, emit_geometry
 from incubator_pegasus_b200 import synth
-from scan_model import make_db
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 SIM_DIR = os.path.join(ROOT, "tools", "simt")
@@ -136,6 +137,11 @@ def check(pgs, oracle, sim, runs, *, bottommost, ops_json=None, **kw):
     for b in range(n):
         last = int(x["blk_rec"][b + 1]) - 1
         assert x["ikeys"][int(x["ikey_off"][b]):int(x["ikey_off"][b + 1])].tobytes() == want.key(last)
+    # restart arrays, the cut rule at the block size the geometry leaves, padding
+    max_ukey = max(int(np.diff(r.key_off.astype(np.int64)).max(initial=0)) for r in runs)
+    geo = emit_geometry(kw.get("block_size", 4096), kw.get("restart_interval", 16), max_ukey, SIM_SMEM)
+    counts = check_run_format(got_run, kw.get("restart_interval", 16), geo["block_size"])
+    assert counts == np.diff(x["blk_rec"][:n + 1].astype(np.int64)).tolist()
     # entry offsets: walking each block entry by entry must land on its rec_off entries
     for b in range(n):
         walk = entry_offsets(got_run.data, int(got_run.blk_off[b]), int(got_run.blk_size[b]))
@@ -185,27 +191,7 @@ def test_sim_filter_variants(pgs, oracle, sim):
 def test_sim_ragged_records(pgs, oracle, sim):
     """keys of 0..300 bytes, values of 0..9000 bytes (blocks of one entry, entries larger than the block buffer),
     several versions of a key inside one run, tombstones, restart interval 1 and 3, small blocks."""
-    rng = np.random.default_rng(11)
-    def mk(seq0, n):
-        items = {}
-        for i in range(n):
-            kl = int(rng.integers(0, 12)) if rng.random() < 0.8 else int(rng.integers(12, 300))
-            key = bytes(rng.integers(0, 3, kl, dtype=np.uint8) + (0 if rng.random() < 0.5 else 0xfe)) if kl else b""
-            for _ in range(int(rng.integers(1, 4))):
-                seq0 += 1
-                t = 0 if rng.random() < 0.15 else 1
-                vl = 0 if t == 0 else (int(rng.integers(4, 40)) if rng.random() < 0.9 else int(rng.integers(3000, 9000)))  # a value always carries its 4-byte header
-                val = bytes(rng.integers(0, 256, vl, dtype=np.uint8))
-                if t == 1 and vl >= 4 and rng.random() < 0.5:
-                    val = (0).to_bytes(4, "big") + val[4:]
-                items[(key, -seq0)] = (key, seq0, t, val)
-        return seq0, pgs.Records.from_list([items[k] for k in sorted(items)])
-    seq = 0
-    runs = []
-    for n in (150, 120, 90):
-        seq, r = mk(seq, n)
-        runs.append(r)
-    runs = runs[::-1]  # newest first is not required: the merge orders by (key, seq)
+    runs = merge_inputs.ragged_records(11)
     for ri, bs in ((1, 256), (3, 512), (16, 4096)):
         for bm in (True, False):
             check(pgs, oracle, sim, runs, bottommost=bm, restart_interval=ri, block_size=bs, seg_weight=8 * 1024, default_ttl=50)
@@ -215,22 +201,9 @@ def test_sim_long_restart_arrays_and_near_buffer_values(pgs, oracle, sim):
     """restart interval 1 with tiny entries: a 4 KB block holds ~270 entries and spans many emit batches, so its restart
     array is carried across batches; values just below / above the emit block buffer switch between the batch and the
     in-place path right after such a block."""
-    rng = np.random.default_rng(5)
-    def mk(seq0, n, big_every):
-        recs = []
-        for i in range(n):
-            key = b"k%05d" % (i * 3 + seq0 % 3)
-            seq0 += 1
-            if big_every and i % big_every == big_every - 1:
-                vl = int(rng.choice([4050, 4090, 4100, 4130, 4200, 8000]))
-            else:
-                vl = 4
-            recs.append((key, seq0, 1, bytes(rng.integers(0, 256, vl, dtype=np.uint8))))
-        return seq0, pgs.Records.from_list(sorted(recs, key=lambda r: (r[0], -r[1])))
-    seq, a = mk(0, 2000, 0)
-    seq, b = mk(seq, 1500, 301)
+    runs = merge_inputs.long_restart_arrays(5)
     for ri in (1, 2, 16):
-        check(pgs, oracle, sim, [b, a], bottommost=True, restart_interval=ri, block_size=4096, seg_weight=64 * 1024)
+        check(pgs, oracle, sim, runs, bottommost=True, restart_interval=ri, block_size=4096, seg_weight=64 * 1024)
 
 
 def test_sim_single_run_and_empty_output(pgs, oracle, sim):
@@ -242,26 +215,23 @@ def test_sim_single_run_and_empty_output(pgs, oracle, sim):
 
 def test_sim_long_keys_widen_the_groups(pgs, oracle, sim):
     """2 KB user keys: a narrow group's key rows no longer fit shared memory, the geometry falls back to wider groups"""
-    rng = np.random.default_rng(3)
-    runs, seq = [], 1
-    for i in range(3):
-        items = {}
-        for j in range(120):
-            hk = b"h%03d" % rng.integers(0, 20)
-            sk = bytes(rng.integers(97, 100, int(rng.integers(1500, 2000))).astype(np.uint8))
-            key = len(hk).to_bytes(2, "big") + hk + sk
-            items[key] = (key, seq, 1, (0).to_bytes(4, "big") + bytes(8) + b"v%d" % j)
-            seq += 1
-        runs.append(pgs.Records.from_list([items[k] for k in sorted(items)]))
+    runs = merge_inputs.long_keys(3)
     check(pgs, oracle, sim, runs, bottommost=True, lanes=0, seg_weight=64 * 1024)
 
 
 def test_sim_anywhere_rule_and_empty_hash_keys(pgs, oracle, sim):
     """a delete rule whose pattern matches inside the sort key ("01" of s0001, s0010..s0019, never at its start), and
     validate_hash over records with an empty hash key, whose sort key is hashed instead"""
-    rng = np.random.default_rng(21)
-    runs, _ = make_db(pgs, rng, 3, [b"", b"h1", b"a01b", b"h22"], 60)
+    runs = merge_inputs.empty_hash_keys(21)
     x = check(pgs, oracle, sim, runs, bottommost=True, ops_json=OPS_ANYWHERE_JSON, seg_weight=16 * 1024)
     assert x["stats"][7] > 0
     x = check(pgs, oracle, sim, runs, bottommost=True, validate_hash=True, pidx=1, partition_version=3, seg_weight=16 * 1024)
     assert x["stats"][8] > 0
+
+
+@pytest.mark.parametrize("block_size,ri", [(1024, 1), (1024, 2), (512, 3)])
+def test_sim_carried_restart_arrays(pgs, oracle, sim, block_size, ri):
+    """a block that spans batches closes in a batch in which the next block records restart points: the closed block's
+    restart array keeps the offsets of its own entries (check_run_format)"""
+    check(pgs, oracle, sim, merge_inputs.carried_restart_arrays(31), bottommost=True, restart_interval=ri, block_size=block_size,
+          seg_weight=64 * 1024)
