@@ -210,13 +210,9 @@ static int32_t upload_stage_a(Engine *e, int32_t level, const uint8_t *data, uin
                               const uint32_t *blk_size, uint32_t nb, UploadJob &j)
 {
     uint64_t prev_end = 0;
-    for (uint32_t b = 0; b < nb; b++) {
-        if (blk_off[b] % kBlockAlign || blk_off[b] < prev_end || blk_off[b] + blk_size[b] > data_bytes) {
-            set_error("run upload: bad block handle %u", b);
-            return PGS_INVALID_ARGUMENT;
-        }
-        prev_end = blk_off[b] + blk_size[b];
-        j.max_blk = std::max(j.max_blk, blk_size[b]);
+    if (const uint32_t b = run_handles_check(blk_off, blk_size, nb, data_bytes, prev_end, j.max_blk); b < nb) {
+        set_error("run upload: bad block handle %u", b);
+        return PGS_INVALID_ARGUMENT;
     }
     auto r = std::make_shared<Run>(e);
     j.r = r;

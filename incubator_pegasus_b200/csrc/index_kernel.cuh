@@ -117,6 +117,24 @@ k_index_walk(const uint8_t *__restrict__ data, const uint64_t *__restrict__ blk_
     if (err && lane == 0) atomicMax(&stats->error, err);
 }
 
+// host, before anything is copied: the handle rule of pgs_run_upload.  Every block starts on a multiple of kBlockAlign, at or
+// behind the end of the block before it, and ends inside the caller's data_bytes; gaps between blocks and bytes behind the last
+// one are allowed.  Returns nb, or the index of the first handle that breaks the rule; end = the end of the last block and
+// max_blk = the largest block size (of the handles in front of a bad one).
+inline uint32_t run_handles_check(const uint64_t *blk_off, const uint32_t *blk_size, uint32_t nb, uint64_t data_bytes, uint64_t &end,
+                                  uint32_t &max_blk)
+{
+    end = 0;
+    max_blk = 0;
+    for (uint32_t b = 0; b < nb; b++) {
+        // (no sum of offset and size on the left: an offset near 2^64 must not wrap into range)
+        if (blk_off[b] % kBlockAlign || blk_off[b] < end || blk_off[b] > data_bytes || blk_size[b] > data_bytes - blk_off[b]) return b;
+        end = blk_off[b] + blk_size[b];
+        max_blk = blk_size[b] > max_blk ? blk_size[b] : max_blk;
+    }
+    return nb;
+}
+
 // host, between the two passes: rec_cum / key_cum[0..nb] = exclusive prefix sums of the records and of the last-user-key
 // lengths of the blocks (the first record and the index key of every block).  false: the run is too large for the 32-bit
 // offsets of the index.

@@ -33,7 +33,8 @@ def sim():
 
 def sim_compact(pgs, sim, runs, *, bottommost, now=synth.NOW, default_ttl=0, validate_hash=False, pidx=0, partition_version=-1,
                 ops=None, enabled=True, block_size=4096, restart_interval=16, lanes=0, seg_weight=0):
-    brs = [pgs.build_run(r, block_size, restart_interval) for r in runs]
+    # an input given as a BlockRun is merged as it stands (tests/foreign_blocks.py writes such runs)
+    brs = [r if isinstance(r, pgs.BlockRun) else pgs.build_run(r, block_size, restart_interval) for r in runs]
     k = len(brs)
     data = (C.c_void_p * k)(*[b.data.ctypes.data for b in brs])
     nbytes = (C.c_uint64 * k)(*[b.data.shape[0] for b in brs])

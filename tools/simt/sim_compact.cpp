@@ -62,8 +62,9 @@ struct HostRun {
 };
 
 // the run's index and Bloom filter as pgs_run_upload builds them (engine.cu): the two passes of k_index_walk with the host
-// layout between them
-bool build_index(HostRun &r, uint32_t nb)
+// layout between them.  Returns the upload's status: what the blocks' walks reported (the largest), or kNotSupported for a run
+// beyond the index's 32-bit offsets
+int32_t build_index(HostRun &r, uint32_t nb)
 {
     std::vector<uint32_t> nrec(nb + 1), lastlen(nb + 1);
     IndexStats st{};
@@ -73,10 +74,10 @@ bool build_index(HostRun &r, uint32_t nb)
         PGS_LAUNCH(k_index_walk<false>, grid, kIdxWarps * 32, smem, 0, (const uint8_t *)r.d_data, (const uint64_t *)r.d_blk_off,
                    (const uint32_t *)r.d_blk_size, nb, nrec.data(), lastlen.data(), (const uint32_t *)nullptr, (uint8_t *)nullptr,
                    (const uint32_t *)nullptr, (uint32_t *)nullptr, (uint32_t *)nullptr, 0u, &st, 0u);
-    if (st.error) return false;
+    if (st.error) return (int32_t)st.error;
     host_alloc(r.mem, r.d_blk_rec, nb + 1, 0);
     host_alloc(r.mem, r.d_ikey_off, nb + 1, 0);
-    if (!index_layout(nrec.data(), lastlen.data(), nb, r.d_blk_rec, r.d_ikey_off)) return false;
+    if (!index_layout(nrec.data(), lastlen.data(), nb, r.d_blk_rec, r.d_ikey_off)) return PGS_NOT_SUPPORTED;
     host_alloc(r.mem, r.d_ikeys, r.d_ikey_off[nb] + 16, 0); // the product's slack (engine.cu)
     host_alloc(r.mem, r.d_rec_off, r.d_blk_rec[nb] + 1, 0);
     r.n_bloom_entries = st.n_records + st.n_prefix;
@@ -86,22 +87,26 @@ bool build_index(HostRun &r, uint32_t nb)
         PGS_LAUNCH(k_index_walk<true>, grid, kIdxWarps * 32, smem, 0, (const uint8_t *)r.d_data, (const uint64_t *)r.d_blk_off,
                    (const uint32_t *)r.d_blk_size, nb, (uint32_t *)nullptr, (uint32_t *)nullptr, (const uint32_t *)r.d_ikey_off,
                    r.d_ikeys, (const uint32_t *)r.d_blk_rec, r.d_rec_off, r.d_bloom, r.bloom_lines, &st, 0u);
-    if (st.error) return false;
+    if (st.error) return (int32_t)st.error;
     uint32_t max_blk = 0;
     for (uint32_t b = 0; b < nb; b++) max_blk = std::max(max_blk, r.d_blk_size[b]);
     run_info_from_index(st, nb, r.d_blk_off[nb], max_blk, r.info);
-    return true;
+    return PGS_OK;
 }
 
-// one run as the upload installs it: its blocks with the product's slack (engine.cu, compact.cu), the 16-aligned end of the
-// blocks as blk_off[nb], the index and the filter
-bool load_run(HostRun &r, const uint8_t *data, uint64_t data_bytes, const uint64_t *blk_off, const uint32_t *blk_size, uint32_t nb)
+// one run as the upload installs it (upload_stage_a of engine.cu): the handle rule, then the bytes up to the 16-aligned end of the
+// last block (what the caller holds behind it stays on the host) with the product's slack, that end as blk_off[nb], the index
+// and the filter.  Returns the upload's status.
+int32_t load_run(HostRun &r, const uint8_t *data, uint64_t data_bytes, const uint64_t *blk_off, const uint32_t *blk_size, uint32_t nb)
 {
-    memcpy(host_alloc(r.mem, r.d_data, data_bytes + 256, 0), data, data_bytes);
+    uint64_t last_end = 0;
+    uint32_t max_blk = 0;
+    if (run_handles_check(blk_off, blk_size, nb, data_bytes, last_end, max_blk) < nb) return PGS_INVALID_ARGUMENT;
+    const uint64_t end = (last_end + kBlockAlign - 1) / kBlockAlign * kBlockAlign;
+    memcpy(host_alloc(r.mem, r.d_data, end + 256, 0), data, std::min(data_bytes, end));
     memcpy(host_alloc(r.mem, r.d_blk_off, nb + 1, 0), blk_off, 8 * (size_t)nb);
     memcpy(host_alloc(r.mem, r.d_blk_size, nb, 0), blk_size, 4 * (size_t)nb);
-    const uint64_t end = nb ? blk_off[nb - 1] + blk_size[nb - 1] : 0;
-    r.d_blk_off[nb] = (end + 15) & ~15ull;
+    r.d_blk_off[nb] = end;
     return build_index(r, nb);
 }
 
@@ -127,7 +132,7 @@ int32_t sim_compact(uint32_t k, const uint8_t **data, const uint64_t *data_bytes
     P.k = k;
     CompactTotals T{};
     for (uint32_t i = 0; i < k; i++) {
-        if (!load_run(runs[i], data[i], data_bytes[i], blk_off[i], blk_size[i], n_blocks[i])) return PGS_CORRUPTION;
+        if (const int32_t rc = load_run(runs[i], data[i], data_bytes[i], blk_off[i], blk_size[i], n_blocks[i])) return rc;
         P.runs[i] = runs[i].dev();
         T.add(runs[i].info, runs[i].n_bloom_entries);
     }
@@ -214,21 +219,43 @@ static uint32_t copy_bloom(const HostRun &r, uint32_t *out, uint64_t cap)
 // the Bloom filter of the last sim_compact output (the one k_emit built)
 uint32_t sim_result_bloom(uint32_t *out, uint64_t cap) { return copy_bloom(g_res.run, out, cap); }
 
-// the Bloom filter the upload builds for one run (k_index_walk); 0 lines: a corrupt run
+// the Bloom filter the upload builds for one run (k_index_walk); 0 lines: a run the upload refuses
 uint32_t sim_run_bloom(const uint8_t *data, uint64_t data_bytes, const uint64_t *blk_off, const uint32_t *blk_size, uint32_t n_blocks,
                        uint32_t *out, uint64_t cap)
 {
     HostRun r;
-    return load_run(r, data, data_bytes, blk_off, blk_size, n_blocks) ? copy_bloom(r, out, cap) : 0;
+    return load_run(r, data, data_bytes, blk_off, blk_size, n_blocks) == PGS_OK ? copy_bloom(r, out, cap) : 0;
 }
 
-static bool load_runs(uint32_t k, const uint8_t **data, const uint64_t *data_bytes, const uint64_t **blk_off, const uint32_t **blk_size,
+// One run loaded as the upload loads it; returns the upload's status.  On PGS_OK: *info = its pgs_run_info (level and run id
+// zero), *n_bloom_entries and *bloom_lines = the filter's sizing, and every non-null array gets what the upload left on the
+// device: blk_rec[nb + 1], ikey_off[nb + 1], ikeys[ikey_off[nb]], rec_off[n_records], bloom[16 * lines] (the caller sizes them
+// from its own model of the run; at most the cap of each, in elements, is written).
+int32_t sim_run_index(const uint8_t *data, uint64_t data_bytes, const uint64_t *blk_off, const uint32_t *blk_size, uint32_t n_blocks,
+                      pgs_run_info *info, uint64_t *n_bloom_entries, uint32_t *bloom_lines, uint32_t *blk_rec, uint32_t *ikey_off,
+                      uint64_t blk_cap, uint8_t *ikeys, uint64_t ikeys_cap, uint32_t *rec_off, uint64_t rec_cap, uint32_t *bloom,
+                      uint64_t bloom_cap)
+{
+    HostRun r;
+    if (const int32_t rc = load_run(r, data, data_bytes, blk_off, blk_size, n_blocks)) return rc;
+    *info = r.info;
+    *n_bloom_entries = r.n_bloom_entries;
+    *bloom_lines = r.bloom_lines;
+    if (blk_rec) memcpy(blk_rec, r.d_blk_rec, 4 * std::min<uint64_t>(blk_cap, n_blocks + 1ull));
+    if (ikey_off) memcpy(ikey_off, r.d_ikey_off, 4 * std::min<uint64_t>(blk_cap, n_blocks + 1ull));
+    if (ikeys) memcpy(ikeys, r.d_ikeys, std::min<uint64_t>(ikeys_cap, r.d_ikey_off[n_blocks]));
+    if (rec_off) memcpy(rec_off, r.d_rec_off, 4 * std::min<uint64_t>(rec_cap, r.d_blk_rec[n_blocks]));
+    if (bloom) copy_bloom(r, bloom, bloom_cap);
+    return PGS_OK;
+}
+
+static int32_t load_runs(uint32_t k, const uint8_t **data, const uint64_t *data_bytes, const uint64_t **blk_off, const uint32_t **blk_size,
                       const uint32_t *n_blocks, std::vector<HostRun> &runs)
 {
     runs.resize(k);
     for (uint32_t i = 0; i < k; i++)
-        if (!load_run(runs[i], data[i], data_bytes[i], blk_off[i], blk_size[i], n_blocks[i])) return false;
-    return true;
+        if (const int32_t rc = load_run(runs[i], data[i], data_bytes[i], blk_off[i], blk_size[i], n_blocks[i])) return rc;
+    return PGS_OK;
 }
 
 // The run set of a read launch over the loaded runs (newest first), as the library's snapshot builds it.  compacted: the run
@@ -283,7 +310,7 @@ int32_t sim_get(uint32_t k, const uint8_t **data, const uint64_t *data_bytes, co
                 uint64_t arena_cap, pgs_get_result *results, uint64_t *stats, uint32_t use_bloom)
 {
     std::vector<HostRun> runs;
-    if (!load_runs(k, data, data_bytes, blk_off, blk_size, n_blocks, runs)) return PGS_CORRUPTION;
+    if (const int32_t rc = load_runs(k, data, data_bytes, blk_off, blk_size, n_blocks, runs)) return rc;
     ReadRunSet R;
     if (const int32_t rc = read_slots(runs, use_bloom & 4, use_bloom & 2, use_bloom & 1, R)) return rc;
     GetParams P{};
@@ -313,7 +340,7 @@ int32_t sim_scan(uint32_t k, const uint8_t **data, const uint64_t *data_bytes, c
                  uint32_t pool_bytes)
 {
     std::vector<HostRun> runs;
-    if (!load_runs(k, data, data_bytes, blk_off, blk_size, n_blocks, runs)) return PGS_CORRUPTION;
+    if (const int32_t rc = load_runs(k, data, data_bytes, blk_off, blk_size, n_blocks, runs)) return rc;
     const ScanBatch B = flatten_scan_requests(reqs, n);
     if (B.any_reverse && lanes) return PGS_INVALID_ARGUMENT; // k_scan has no lane groups and no multi-partition shape
     ReadRunSet R;
