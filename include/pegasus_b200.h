@@ -213,6 +213,45 @@ PGS_API int32_t pgs_compact_ex(pgs_partition *p, const uint64_t *run_ids, uint32
                                int32_t out_level, int32_t bottommost, const pgs_filter_params *fp,
                                uint32_t now, uint32_t flags, pgs_compact_result *out);
 
+/* ---- partition split ------------------------------------------------------------------------
+ * Splits partition `src` (index pidx of `src_count`) into its dst_count / src_count children on the
+ * device.  Child i is partition pidx + i * src_count and receives, for every run of the parent, one
+ * run at the same level holding the records with (pegasus_key_hash(key) % dst_count) / src_count == i
+ * in the run's order: every version and tombstone with its trailer, values byte-identical, no filter.
+ * Records with an empty user key (the empty write) are dropped and counted.  The reference's
+ * local_partition_split (src/shell/commands/local_partition_split.cpp:238-283) routes records the
+ * same way but refuses runs that hold deletions; here they are split.
+ *   dst_count must be src_count * 2^n (n >= 1) and n_dst == dst_count / src_count; dst[i] may be
+ *   NULL (child i is not built: the online split, where the parent itself keeps index 0).  Every
+ *   other destination belongs to src's engine, has index pidx + i * src_count and no runs:
+ *   PGS_INVALID_ARGUMENT otherwise, as for bad counts.  A destination may belong to another app
+ *   (local_partition_split writes the children into a new table).  A destination with another
+ *   data_version, or more than PGS_SPLIT_MAX_CHILDREN children: PGS_NOT_SUPPORTED.
+ *   The parent is never modified.  The children's runs are installed only after every run of every
+ *   child was built; on any error no child changes. */
+#define PGS_SPLIT_MAX_CHILDREN 32
+typedef struct {
+    uint64_t records;     /* records of the child's runs                                          */
+    uint64_t tombstones;
+    uint64_t raw_bytes;   /* sum(user key + value)                                                */
+    uint64_t block_bytes; /* encoded blocks                                                       */
+    uint32_t runs;        /* runs installed                                                       */
+    uint32_t reserved;
+} pgs_split_child_result;
+typedef struct {
+    pgs_split_child_result child[PGS_SPLIT_MAX_CHILDREN];
+    uint64_t in_records, in_bytes; /* over the parent's runs (in_bytes = sum(user key + value))  */
+    uint64_t dropped_empty;        /* empty writes dropped                                         */
+    float device_ms;               /* CUDA-event time from the first launch to the last           */
+    float kernel_ms;               /* CUDA-event time of the split's kernels: the sum of the next three */
+    float count_ms;                /* planner + counting walk                                      */
+    float walk_ms;                 /* writing walk                                                 */
+    float emit_ms;                 /* k_seg_scan + k_emit of every child                           */
+    uint32_t n_launches;
+} pgs_split_result;
+PGS_API int32_t pgs_partition_split(pgs_partition *src, uint32_t src_count, uint32_t dst_count,
+                                    pgs_partition *const *dst, uint32_t n_dst, pgs_split_result *out);
+
 /* Parse the JSON of the `user_specified_compaction` env (compaction_operation.cpp:162-186) into
  * the binary ops table.  Invalid JSON / rules yield an empty table like the reference.  Returns
  * bytes written (<= cap) or a negative status. */
@@ -568,6 +607,18 @@ PGS_API int32_t pgs_rrdb_manual_compact(pgs_server *s, uint32_t now, pgs_compact
 /* last_flushed_decree: the newest decree whose data lives in an HBM run (advanced by a memtable flush, like the decree the
  * reference persists in the SST meta CF); last_committed_decree: the newest decree applied to the memtable.  Nothing here is
  * durable across a process crash (no WAL / checkpoint yet: SURVEY 8 f4), so neither may drive replication-log GC. */
+/* Partition split of a replica (the online split manager's copy_checkpoint_to_dir(flush = true) +
+ * storage_apply_checkpoint, replica_split_manager.cpp:278, and local_partition_split): under the
+ * parent's writer lock its memtable is flushed and its runs are snapshotted; the snapshot's
+ * last_flushed_decree is the split's decree (*decree_out).  The parent then takes reads and writes
+ * again while pgs_partition_split builds the children from the snapshot.  children[i] (n of them,
+ * n == dst_count / src_count, NULL: not built) is a started, empty replica (no runs, empty memtable,
+ * decree 0) of index parent.pidx + i * src_count on the parent's engine.  On success each child holds
+ * its share of the snapshot, last_seq = the parent's (new writes win over copied versions),
+ * committed and flushed decree = the split's decree, durable decree 0, and the parent's
+ * manual_compact_last_finish_ms.  Errors as pgs_partition_split's; on an error no child changes. */
+PGS_API int32_t pgs_rrdb_split(pgs_server *parent, uint32_t src_count, uint32_t dst_count,
+                               pgs_server *const *children, uint32_t n, int64_t *decree_out);
 PGS_API int64_t pgs_rrdb_last_flushed_decree(pgs_server *s);
 PGS_API int64_t pgs_rrdb_last_committed_decree(pgs_server *s);
 /* Checkpoints (first slice of SURVEY 8 f4; sync_checkpoint / storage_apply_checkpoint, pegasus_server_impl.cpp:1951-2336).

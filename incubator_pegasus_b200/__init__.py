@@ -74,6 +74,20 @@ class CompactResult(C.Structure):
                 ("reserved", C.c_uint32)]
 
 
+SPLIT_MAX_CHILDREN = 32
+
+
+class SplitChildResult(C.Structure):
+    _fields_ = [("records", C.c_uint64), ("tombstones", C.c_uint64), ("raw_bytes", C.c_uint64), ("block_bytes", C.c_uint64),
+                ("runs", C.c_uint32), ("reserved", C.c_uint32)]
+
+
+class SplitResult(C.Structure):
+    _fields_ = [("child", SplitChildResult * SPLIT_MAX_CHILDREN), ("in_records", C.c_uint64), ("in_bytes", C.c_uint64),
+                ("dropped_empty", C.c_uint64), ("device_ms", C.c_float), ("kernel_ms", C.c_float), ("count_ms", C.c_float),
+                ("walk_ms", C.c_float), ("emit_ms", C.c_float), ("n_launches", C.c_uint32)]
+
+
 class GetResult(C.Structure):
     _fields_ = [("status", C.c_int32), ("expire_ts", C.c_uint32), ("value_off", C.c_uint32),
                 ("value_len", C.c_uint32), ("expired", C.c_uint8), ("reserved", C.c_uint8 * 3)]
@@ -216,6 +230,8 @@ def lib() -> C.CDLL:
     L.pgs_blocks_decode.argtypes = [vp, vp, vp, C.c_uint32, C.POINTER(DecodeSizes), vp, vp, vp, vp, vp, vp]
     for name, args in {
         "pgs_get_batch": [vp, vp, vp, C.c_uint32, C.c_uint32, vp, C.c_uint64, vp, u64p],
+        "pgs_partition_split": [vp, C.c_uint32, C.c_uint32, C.POINTER(vp), C.c_uint32, C.POINTER(SplitResult)],
+        "pgs_rrdb_split": [vp, C.c_uint32, C.c_uint32, C.POINTER(vp), C.c_uint32, C.POINTER(C.c_int64)],
         "pgs_range_scan": [vp, C.POINTER(ScanRequest), C.c_uint32, vp, C.c_uint64, vp, C.c_uint32, vp, C.c_uint32,
                            C.POINTER(ScanResult)],
         "pgs_rrdb_start": [vp, C.c_int32, C.c_int32, C.POINTER(ServerOptions), C.c_char_p, C.c_uint32, C.POINTER(vp)],
@@ -546,6 +562,15 @@ def hotkey_state(server, hotkey_type: int) -> int:
     return int(lib().pgs_rrdb_hotkey_state(server, hotkey_type))
 
 
+def rrdb_split(parent, src_count: int, dst_count: int, children) -> int:
+    """pgs_rrdb_split: the pgs_server handle `parent` into its children (server handles, or None: not built); returns the
+    split's decree"""
+    handles = (C.c_void_p * max(1, len(children)))(*[c if c is not None else None for c in children])
+    decree = C.c_int64()
+    _check(lib().pgs_rrdb_split(parent, src_count, dst_count, handles, len(children), C.byref(decree)), "rrdb_split")
+    return decree.value
+
+
 def partition_index(hash_key: bytes, sort_key: bytes, partition_count: int) -> int:
     return int(lib().pgs_partition_index(hash_key, len(hash_key), sort_key, len(sort_key), partition_count))
 
@@ -626,6 +651,14 @@ class Partition:
         res = CompactResult()
         _check(lib().pgs_compact_ex(self.h, ids.ctypes.data_as(u64p), ids.shape[0], out_level, bottommost,
                                     C.byref(fp), now, flags, C.byref(res)), "compact")
+        return res
+
+    def split(self, src_count: int, dst_count: int, children) -> SplitResult:
+        """pgs_partition_split: this partition (index pidx of src_count) into dst_count / src_count children; children[i]
+        is the empty Partition pidx + i * src_count of the same engine, or None (child i is not built)"""
+        handles = (C.c_void_p * max(1, len(children)))(*[c.h.value if c is not None else None for c in children])
+        res = SplitResult()
+        _check(lib().pgs_partition_split(self.h, src_count, dst_count, handles, len(children), C.byref(res)), "partition_split")
         return res
 
     def prefix_scan_batch(self, hashkeys, max_records: int = 1000, arena_stride: int = 32768, alloc=None) -> "ScanBatch":

@@ -237,9 +237,10 @@ PGS_HD uint32_t emit_warp_layout(uint32_t bb, uint32_t RI, uint32_t ks, uint32_t
 }
 // fills the derived fields of P (P.k, P.block_size, P.restart_interval must be set); false = not supported
 constexpr uint32_t kWalkMinG = 4; // default lanes per merge group (see group.cuh)
-// walk_groups = merge groups the device runs at the same time (0: not known yet, the default segment budget is used)
+// walk_groups = merge groups the device runs at the same time (0: not known yet, the default segment budget is used);
+// force_Q = the segment count of a plan made elsewhere (a partition split's child is emitted over its parent's segments)
 inline bool compact_geometry(MergeParams &P, const CompactTotals &T, uint32_t max_smem, CompactGeometry &geo, uint32_t force_G = 0,
-                             uint64_t force_weight = 0, uint64_t walk_groups = 0)
+                             uint64_t force_weight = 0, uint64_t walk_groups = 0, uint32_t force_Q = 0)
 {
     const uint32_t k = P.k;
     P.total_blocks = (uint32_t)T.total_blocks;
@@ -305,6 +306,7 @@ inline bool compact_geometry(MergeParams &P, const CompactTotals &T, uint32_t ma
     if (force_weight) P.tile_weight = force_weight;
     uint64_t Q = (W_total + P.tile_weight - 1) / P.tile_weight;
     if (Q == 0) Q = 1;
+    if (force_Q) Q = force_Q;
     if (Q > 0x7FFFFFF0ull) return false;
     P.Q = (uint32_t)Q;
     // output capacity (every segment starts a new block; two neighbouring blocks of a segment hold more than block_size bytes)

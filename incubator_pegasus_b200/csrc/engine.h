@@ -131,6 +131,10 @@ int32_t scan_many(pgs_partition *const *parts, uint32_t n_parts, const uint32_t 
 // request gets PGS_NOT_SUPPORTED otherwise (the server folds L0 first, server.cpp)
 bool scan_stages_every_run(pgs_partition *ph);
 
+// pgs_partition_split over the runs `snap` of src (nullptr: its current runs)
+int32_t partition_split(pgs_partition *src, const std::vector<std::shared_ptr<Run>> *snap, uint32_t src_count, uint32_t dst_count,
+                        pgs_partition *const *dst, uint32_t n_dst, pgs_split_result *out);
+
 void set_error(const char *fmt, ...);
 int32_t cuda_fail(cudaError_t e, const char *what);
 #define PGS_CUDA(expr)                                                                             \

@@ -1102,6 +1102,60 @@ int32_t pgs_rrdb_apply_checkpoint(pgs_server *h, const char *cdir)
     s.last_committed_decree = s.last_flushed_decree = s.last_durable_decree = m.decree;
     return PGS_OK;
 }
+// ---- partition split (local_partition_split.cpp:179-298; replica_split_manager.cpp:278 copy_checkpoint_to_dir(flush = true) +
+// storage_apply_checkpoint) ---------------------------------------------------------------------------------------------------
+int32_t pgs_rrdb_split(pgs_server *parent, uint32_t src_count, uint32_t dst_count, pgs_server *const *children, uint32_t n,
+                       int64_t *decree_out)
+{
+    if (!parent || !children || src_count == 0 || n == 0 || n > 1024) return PGS_INVALID_ARGUMENT;
+    Server &s = parent->s;
+    // the children stay locked for the whole call: nothing reaches them until they hold the split state
+    std::vector<Server *> kids;
+    for (uint32_t i = 0; i < n; i++) {
+        if (!children[i]) continue;
+        if (children[i] == parent) return PGS_INVALID_ARGUMENT;
+        kids.push_back(&children[i]->s);
+    }
+    std::vector<Server *> order = kids;
+    std::sort(order.begin(), order.end());
+    if (std::adjacent_find(order.begin(), order.end()) != order.end()) return PGS_INVALID_ARGUMENT;
+    std::vector<std::unique_lock<std::shared_mutex>> held;
+    for (Server *k : order) held.emplace_back(k->mu);
+    for (uint32_t i = 0; i < n; i++) {
+        if (!children[i]) continue;
+        Server &c = children[i]->s;
+        if (!c.mem.empty() || !c.runs().empty() || c.last_committed_decree != 0 || c.last_flushed_decree != 0 ||
+            (int64_t)c.pidx != (int64_t)s.pidx + (int64_t)i * src_count) {
+            set_error("rrdb_split: child %u is not an empty, new replica of index %lld", i, (long long)s.pidx + (long long)i * src_count);
+            return PGS_INVALID_ARGUMENT;
+        }
+    }
+    // the parent's state as copy_checkpoint_to_dir(flush = true) fixes it: memtable flushed, runs snapshotted, under its
+    // writer lock; after that the parent takes reads and writes again while the snapshot is split
+    std::vector<std::shared_ptr<Run>> snap;
+    int64_t decree;
+    uint64_t last_seq, mc_finish;
+    {
+        std::unique_lock<std::shared_mutex> w(s.mu);
+        if (const int32_t st = s.flush_mem()) return st;
+        snap = s.runs();
+        decree = s.last_flushed_decree;
+        last_seq = s.last_seq;
+        mc_finish = s.manual_compact_last_finish_ms;
+    }
+    std::vector<pgs_partition *> dst(n, nullptr);
+    for (uint32_t i = 0; i < n; i++)
+        if (children[i]) dst[i] = children[i]->s.part;
+    if (const int32_t st = partition_split(s.part, &snap, src_count, dst_count, dst.data(), n, nullptr)) return st;
+    for (Server *k : kids) {
+        k->last_seq = last_seq; // new writes on the child win over every copied version
+        k->last_committed_decree = k->last_flushed_decree = decree;
+        k->last_durable_decree = 0;
+        k->manual_compact_last_finish_ms = mc_finish;
+    }
+    if (decree_out) *decree_out = decree;
+    return PGS_OK;
+}
 int64_t pgs_rrdb_last_flushed_decree(pgs_server *h) { RLOCKED(h); return h->s.last_flushed_decree; }
 int64_t pgs_rrdb_last_committed_decree(pgs_server *h) { RLOCKED(h); return h->s.last_committed_decree; }
 

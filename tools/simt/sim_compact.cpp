@@ -9,6 +9,7 @@
 #include "../../incubator_pegasus_b200/csrc/index_kernel.cuh"
 #include "../../incubator_pegasus_b200/csrc/read_kernels.cuh"
 #include "../../incubator_pegasus_b200/csrc/scan_kernel.cuh"
+#include "../../incubator_pegasus_b200/csrc/split_kernels.cuh"
 
 #include <cstdarg>
 #include <memory>
@@ -117,6 +118,13 @@ struct Merged { // the output of the last sim_compact call
     MergeStats st{};
     uint32_t Q = 0;
 } g_res;
+
+struct Split { // the children of the last sim_split call
+    std::vector<HostRun> child;
+    std::vector<MergeStats> st;
+    std::vector<uint8_t> built;
+    uint32_t Q = 0;
+} g_split;
 
 } // namespace
 
@@ -400,5 +408,99 @@ uint32_t sim_hotkey_capture(const uint8_t *keys, const uint32_t *key_off, const 
 
 // the bucket hash of format.h, for the tests' model
 uint64_t sim_hotkey_hash(const uint8_t *p, uint32_t len) { return hotkey_hash(p, len); }
+
+// One parent run split into dst_count / src_count children through split_plan / split_buffers / split_child / split_launch,
+// as pgs_partition_split runs it; want = the children that are built (bit c).  seg_weight: smaller segments (0: the product's
+// default budget).  Returns a status; the children stay in a static buffer until the next call (sim_split_child_* read them),
+// *dropped = the empty writes.
+int32_t sim_split(const uint8_t *data, uint64_t data_bytes, const uint64_t *blk_off, const uint32_t *blk_size, uint32_t n_blocks,
+                  uint32_t block_size, uint32_t restart_interval, uint32_t src_count, uint32_t dst_count, uint32_t want, uint64_t seg_weight,
+                  uint64_t *dropped)
+{
+    HostRun in;
+    if (const int32_t rc = load_run(in, data, data_bytes, blk_off, blk_size, n_blocks)) return rc;
+    if (src_count == 0 || dst_count % src_count) return PGS_INVALID_ARGUMENT;
+    const uint32_t NC = dst_count / src_count;
+    SplitParams SP{};
+    SP.M.runs[0] = in.dev();
+    SP.M.block_size = block_size;
+    SP.M.restart_interval = restart_interval;
+    SP.M.data_version = 1;
+    crc64_make_table(crc_tab);
+    SP.M.crc_table = (const unsigned long long *)crc_tab;
+    SP.S = NC; SP.src_count = src_count; SP.dst_count = dst_count; SP.want = want;
+    CompactTotals T{};
+    T.add(in.info, in.n_bloom_entries);
+    const uint32_t smem = compact_smem_budget(kSimSmemOptin);
+    SplitGeometry geo{};
+    if (const int32_t rc = split_plan(SP, T, smem, geo, 0, seg_weight)) return rc;
+    Split &R = g_split;
+    R = Split{};
+    R.child.resize(NC);
+    R.built.assign(NC, 0);
+    HostMem scratch;
+    split_buffers(SP, [&](auto *&p, uint64_t n, int fill, bool) { host_alloc(scratch, p, n, fill == kNoFill ? 0xEE : fill); });
+    for (uint32_t c = 0; c < NC; c++) SP.stats[c] = merge_stats_init();
+    split_launch(SP, geo, nullptr, nullptr, 0, 2, 2, nullptr, [](int) {});
+    R.st.assign(SP.stats, SP.stats + NC);
+    *dropped = *SP.dropped;
+    for (uint32_t c = 0; c < NC; c++)
+        if (R.st[c].error) { fprintf(stderr, "sim_split: counting pass status %u (child %u)\n", R.st[c].error, c); return (int32_t)R.st[c].error; }
+    std::vector<MergeParams> Pc;
+    std::vector<CompactGeometry> gc;
+    for (uint32_t c = 0; c < NC; c++) {
+        if (!((want >> c) & 1u) || R.st[c].cnt[EV_OUT] == 0) continue;
+        MergeParams P{};
+        CompactGeometry g{};
+        CompactTotals Tc{};
+        if (!split_child(SP, R.st[c], SP.prefixes[c], smem, P, g, Tc)) return PGS_NOT_SUPPORTED;
+        HostRun &run = R.child[c];
+        compact_buffers(P, g, Tc, run, [&](auto *&p, uint64_t n, int fill, bool out) {
+            if (out) host_alloc(run.mem, p, n, fill == kNoFill ? 0xEE : fill);
+        });
+        split_child_scratch(SP, c, P);
+        Pc.push_back(P);
+        gc.push_back(g);
+        R.built[c] = 1;
+    }
+    split_launch(SP, geo, Pc.data(), gc.data(), (uint32_t)Pc.size(), 2, 2, nullptr, [](int) {});
+    R.st.assign(SP.stats, SP.stats + NC);
+    R.Q = SP.M.Q;
+    for (uint32_t c = 0; c < NC; c++) {
+        if (R.st[c].error) { fprintf(stderr, "sim_split: status %u at segment %u (child %u)\n", R.st[c].error, R.st[c].error_seg, c); return (int32_t)R.st[c].error; }
+        if (!R.built[c]) continue;
+        pgs_compact_result cr{};
+        R.child[c].n_bloom_entries = compact_result_stats(R.st[c], 0, cr, R.child[c].info);
+    }
+    return PGS_OK;
+}
+
+// child c of the last sim_split: 0 = not built (or nothing for it); else *info = its pgs_run_info, *n_segments = the parent's
+// segments, *index_key_bytes = its index keys' bytes
+int32_t sim_split_child_info(uint32_t c, pgs_run_info *info, uint32_t *n_segments, uint64_t *index_key_bytes)
+{
+    if (c >= g_split.child.size() || !g_split.built[c]) return 0;
+    *info = g_split.child[c].info;
+    *n_segments = g_split.Q;
+    *index_key_bytes = g_split.st[c].tot_keyb;
+    return 1;
+}
+void sim_split_child_copy(uint32_t c, uint8_t *data, uint64_t *blk_off, uint32_t *blk_size, uint32_t *blk_rec, uint32_t *ikey_off, uint8_t *ikeys)
+{
+    const HostRun &r = g_split.child[c];
+    const uint32_t nb = r.info.n_blocks;
+    memcpy(data, r.d_data, r.info.data_bytes);
+    memcpy(blk_off, r.d_blk_off, 8 * (size_t)(nb + 1));
+    memcpy(blk_size, r.d_blk_size, 4 * (size_t)nb);
+    memcpy(blk_rec, r.d_blk_rec, 4 * (size_t)(nb + 1));
+    memcpy(ikey_off, r.d_ikey_off, 4 * (size_t)(nb + 1));
+    memcpy(ikeys, r.d_ikeys, g_split.st[c].tot_keyb);
+}
+// 1 when child c's Bloom filter admits the byte string
+int32_t sim_split_child_bloom_check(uint32_t c, const uint8_t *key, uint32_t len)
+{
+    const HostRun &r = g_split.child[c];
+    return bloom_may_contain(r.d_bloom, r.bloom_lines, bloom_hash_bytes(key, len)) ? 1 : 0;
+}
 
 } // extern "C"
