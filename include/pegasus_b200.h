@@ -150,6 +150,25 @@ typedef struct {
     int32_t level;
 } pgs_run_src;
 PGS_API int32_t pgs_run_upload_many(pgs_partition *p, const pgs_run_src *runs, uint32_t n, uint64_t *run_ids_out);
+/* Build one sorted run on the device from n flat records and install it, as the host builder plus pgs_run_upload would:
+ * the blocks, their handles and the run's info are byte for byte those of pgs_run_builder_add_many + pgs_run_builder_finish
+ * at the engine's block_size / restart_interval followed by pgs_run_upload (only the run id differs).  Records are in
+ * internal-key order (user key ascending, then seq<<8|type strictly descending); record i's user key is
+ * keys[key_off[i] .. key_off[i+1]), its value vals[val_off[i] .. val_off[i+1]).  Host arrays may be pageable or pinned.
+ *   n == 0: PGS_OK, *run_id_out = 0, nothing resident.
+ *   out of order (as pgs_run_builder_add returns), or offsets that are not ascending: PGS_INVALID_ARGUMENT.
+ *   a user key over 4096 bytes, or a run past the index's 32-bit record / index-key offsets: PGS_NOT_SUPPORTED.
+ * All or nothing: on an error the partition's run list is unchanged.
+ * The whole input is resident on the device for the duration of the call, with about 4 * ceil(log2 n) + 25 bytes of
+ * scratch per record besides. */
+PGS_API int32_t pgs_run_build(pgs_partition *p, int32_t level, uint64_t n,
+                              const uint8_t *keys, const uint64_t *key_off,
+                              const uint8_t *vals, const uint64_t *val_off,
+                              const uint64_t *seq, const uint8_t *type,
+                              uint64_t *run_id_out);
+/* device times (ms) of the calling thread's last successful pgs_run_build: [0] input copy, [1] block plan (record, next-block,
+ * chain and scan passes), [2] block writing, [3] index and Bloom filter (the upload's two passes) */
+PGS_API void pgs_run_build_last_ms(float *ms4);
 PGS_API int32_t pgs_run_drop(pgs_partition *p, uint64_t run_id);
 PGS_API int32_t pgs_run_info_get(pgs_partition *p, uint64_t run_id, pgs_run_info *out);
 /* run ids in read order (newest first: L0 by recency, then L1, L2, ...) */

@@ -204,6 +204,9 @@ def lib() -> C.CDLL:
     L.pgs_run_upload.argtypes = [vp, C.c_int32, vp, C.c_uint64, vp, vp, C.c_uint32, u64p]
     L.pgs_get_batch_multi.argtypes = [C.POINTER(vp), C.c_uint32, vp, vp, vp, C.c_uint32, C.c_uint32, vp, C.c_uint64, vp, u64p]
     L.pgs_run_upload_many.argtypes = [vp, C.POINTER(RunSrc), C.c_uint32, u64p]
+    L.pgs_run_build.argtypes = [vp, C.c_int32, C.c_uint64, vp, vp, vp, vp, vp, vp, u64p]
+    L.pgs_run_build_last_ms.argtypes = [C.POINTER(C.c_float)]
+    L.pgs_run_build_last_ms.restype = None
     L.pgs_run_drop.argtypes = [vp, C.c_uint64]
     L.pgs_run_info_get.argtypes = [vp, C.c_uint64, C.POINTER(RunInfo)]
     L.pgs_run_list.argtypes = [vp, u64p, C.c_uint32, u32p]
@@ -571,6 +574,13 @@ def rrdb_split(parent, src_count: int, dst_count: int, children) -> int:
     return decree.value
 
 
+def run_build_last_ms() -> list[float]:
+    """device times (ms) of this thread's last Partition.build_records: input copy, block plan, block writing, index"""
+    ms = (C.c_float * 4)()
+    lib().pgs_run_build_last_ms(ms)
+    return list(ms)
+
+
 def partition_index(hash_key: bytes, sort_key: bytes, partition_count: int) -> int:
     return int(lib().pgs_partition_index(hash_key, len(hash_key), sort_key, len(sort_key), partition_count))
 
@@ -609,6 +619,14 @@ class Partition:
 
     def upload_records(self, recs: Records, level: int = 0) -> int:
         return self.upload(build_run(recs), level)
+
+    def build_records(self, recs: Records, level: int = 0) -> int:
+        """the run of `recs` (in internal-key order) built on the device at the engine's block geometry (pgs_run_build): the
+        same blocks and run info as upload(build_run(recs)) at that geometry; 0 for no records"""
+        rid = C.c_uint64()
+        _check(lib().pgs_run_build(self.h, level, recs.n, _ptr(recs.keys), _ptr(recs.key_off), _ptr(recs.vals), _ptr(recs.val_off),
+                                   _ptr(recs.seq), _ptr(recs.type), C.byref(rid)), "run_build")
+        return rid.value
 
     def run_info(self, run_id: int) -> RunInfo:
         info = RunInfo()

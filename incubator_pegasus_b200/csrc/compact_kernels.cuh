@@ -75,13 +75,6 @@ PGS_HD uint32_t entry_head_len(uint32_t shared, uint32_t kd, uint32_t vlen) { re
 PGS_HD uint32_t block_bytes(uint32_t entry_bytes, uint32_t nrest) { return entry_bytes + 4 * (nrest + 1); }
 PGS_HD uint32_t block_span(uint32_t size) { return (size + kBlockAlign - 1) & ~(kBlockAlign - 1); }
 PGS_HD uint32_t restart_count(uint32_t n, uint32_t RI) { return (n + RI - 1) / RI; } // restart points of n entries
-PGS_DEV uint32_t put_varint32_s(uint8_t *p, uint32_t v) // shared-memory / generic byte stores
-{
-    uint32_t n = 0;
-    while (v >= 128u) { p[n++] = (uint8_t)(v | 128u); v >>= 7; }
-    p[n++] = (uint8_t)v;
-    return n;
-}
 // the three varints of an entry head at p; returns their bytes
 PGS_DEV uint32_t put_entry_varints(uint8_t *p, uint32_t shared, uint32_t kd, uint32_t vlen)
 {

@@ -151,6 +151,13 @@ PGS_DEV uint32_t get_varint32(const uint8_t *p, uint32_t avail, uint32_t &v)
     }
     return 0;
 }
+PGS_DEV uint32_t put_varint32_s(uint8_t *p, uint32_t v) // shared-memory / generic byte stores; returns bytes written
+{
+    uint32_t n = 0;
+    while (v >= 128u) { p[n++] = (uint8_t)(v | 128u); v >>= 7; }
+    p[n++] = (uint8_t)v;
+    return n;
+}
 
 // ---- byte-string compare -------------------------------------------------------------------------
 // generic pointers, any alignment; returns <0, 0, >0 like memcmp-then-length

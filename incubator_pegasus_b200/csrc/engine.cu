@@ -7,6 +7,7 @@
 #include <algorithm>
 #include <cstring>
 
+#include "build_kernels.cuh"
 #include "engine.h"
 #include "index_kernel.cuh"
 
@@ -207,14 +208,9 @@ struct UploadJob {
     }
 };
 
-static int32_t upload_stage_a(Engine *e, int32_t level, const uint8_t *data, uint64_t data_bytes, const uint64_t *blk_off,
-                              const uint32_t *blk_size, uint32_t nb, UploadJob &j)
+// the job's pinned staging, its Run and the device buffers of the first pass, for nb blocks that end at `end` (16-aligned)
+static int32_t upload_job_init(Engine *e, int32_t level, uint32_t nb, uint64_t end, UploadJob &j)
 {
-    uint64_t prev_end = 0;
-    if (const uint32_t b = run_handles_check(blk_off, blk_size, nb, data_bytes, prev_end, j.max_blk); b < nb) {
-        set_error("run upload: bad block handle %u", b);
-        return PGS_INVALID_ARGUMENT;
-    }
     auto r = std::make_shared<Run>(e);
     j.r = r;
     j.eng = e;
@@ -235,31 +231,64 @@ static int32_t upload_stage_a(Engine *e, int32_t level, const uint8_t *data, uin
     r->level = level;
     r->info.level = level;
     r->info.n_blocks = nb;
-    const uint64_t end = (prev_end + kBlockAlign - 1) / kBlockAlign * kBlockAlign;
-    const uint64_t nbytes = data_bytes < end ? data_bytes : end;
     r->info.data_bytes = end;
-    cudaStream_t st = e->stream, cp = e->up_copy;
+    cudaStream_t st = e->stream;
     PGS_CUDA(e->alloc_data(*r, end + 256));
     PGS_CUDA(cudaMallocAsync(&r->d_blk_off, sizeof(uint64_t) * (nb + 1), st));
     PGS_CUDA(cudaMallocAsync(&r->d_blk_size, sizeof(uint32_t) * nb, st));
     PGS_CUDA(cudaMallocAsync(&j.d_nrec, sizeof(uint32_t) * nb, st));
     PGS_CUDA(cudaMallocAsync(&j.d_lastlen, sizeof(uint32_t) * nb, st));
     PGS_CUDA(cudaMallocAsync(&j.d_stats, sizeof(IndexStats), st));
+    *j.hs_in = IndexStats{};
+    j.hs_in->min_seq = ~0ull;
+    PGS_CUDA(cudaMemcpyAsync(j.d_stats, j.hs_in, sizeof(IndexStats), cudaMemcpyHostToDevice, st));
+    return PGS_OK;
+}
+// the first index pass over the blocks [b0, b1) once their bytes are on the device
+static void upload_pass1(Engine *e, UploadJob &j, uint32_t b0, uint32_t b1)
+{
+    Run *r = j.r.get();
+    k_index_walk<false><<<(b1 - b0 + kIdxWarps - 1) / kIdxWarps, kIdxWarps * 32, kIdxWarps * kIdxScratch, e->stream>>>(
+        r->d_data, r->d_blk_off, r->d_blk_size, b1, j.d_nrec, j.d_lastlen, nullptr, nullptr, nullptr, nullptr, nullptr, 0, j.d_stats, b0);
+    e->launches++;
+}
+// after the last first-pass launch: its per-block results come back, j.pass1 marks their arrival
+static int32_t upload_pass1_done(Engine *e, UploadJob &j)
+{
+    const uint32_t nb = j.r->info.n_blocks;
+    cudaStream_t st = e->stream;
+    PGS_CUDA(cudaMemcpyAsync(j.nrec, j.d_nrec, sizeof(uint32_t) * nb, cudaMemcpyDeviceToHost, st));
+    PGS_CUDA(cudaMemcpyAsync(j.lastlen, j.d_lastlen, sizeof(uint32_t) * nb, cudaMemcpyDeviceToHost, st));
+    PGS_CUDA(cudaMemcpyAsync(j.hs_out, j.d_stats, sizeof(IndexStats), cudaMemcpyDeviceToHost, st));
+    PGS_CUDA(cudaEventCreateWithFlags(&j.pass1, cudaEventDisableTiming));
+    PGS_CUDA(cudaEventRecord(j.pass1, st));
+    return PGS_OK;
+}
+
+static int32_t upload_stage_a(Engine *e, int32_t level, const uint8_t *data, uint64_t data_bytes, const uint64_t *blk_off,
+                              const uint32_t *blk_size, uint32_t nb, UploadJob &j)
+{
+    uint64_t prev_end = 0;
+    if (const uint32_t b = run_handles_check(blk_off, blk_size, nb, data_bytes, prev_end, j.max_blk); b < nb) {
+        set_error("run upload: bad block handle %u", b);
+        return PGS_INVALID_ARGUMENT;
+    }
+    const uint64_t end = (prev_end + kBlockAlign - 1) / kBlockAlign * kBlockAlign;
+    const uint64_t nbytes = data_bytes < end ? data_bytes : end;
+    if (const int32_t rc = upload_job_init(e, level, nb, end, j)) return rc;
+    Run *r = j.r.get();
+    cudaStream_t st = e->stream, cp = e->up_copy;
     PGS_CUDA(cudaMemsetAsync(r->d_data + nbytes, 0, r->data_cap - nbytes, st));
     memcpy(j.off, blk_off, sizeof(uint64_t) * nb);
     j.off[nb] = end;
     memcpy(j.h_size, blk_size, sizeof(uint32_t) * nb);
-    *j.hs_in = IndexStats{};
-    j.hs_in->min_seq = ~0ull;
     PGS_CUDA(cudaMemcpyAsync(r->d_blk_off, j.off, sizeof(uint64_t) * (nb + 1), cudaMemcpyHostToDevice, st));
     PGS_CUDA(cudaMemcpyAsync(r->d_blk_size, j.h_size, sizeof(uint32_t) * nb, cudaMemcpyHostToDevice, st));
-    PGS_CUDA(cudaMemcpyAsync(j.d_stats, j.hs_in, sizeof(IndexStats), cudaMemcpyHostToDevice, st));
     cudaEvent_t ready;
     PGS_CUDA(cudaEventCreateWithFlags(&ready, cudaEventDisableTiming));
     j.events.push_back(ready);
     PGS_CUDA(cudaEventRecord(ready, st)); // the copy stream may touch the new buffers from here on
     PGS_CUDA(cudaStreamWaitEvent(cp, ready, 0));
-    const size_t smem = kIdxWarps * kIdxScratch;
     uint32_t b0 = 0;
     while (b0 < nb) { // chunks end on block boundaries
         uint32_t b1 = b0 + 1;
@@ -271,17 +300,10 @@ static int32_t upload_stage_a(Engine *e, int32_t level, const uint8_t *data, uin
         j.events.push_back(ev);
         PGS_CUDA(cudaEventRecord(ev, cp));
         PGS_CUDA(cudaStreamWaitEvent(st, ev, 0));
-        k_index_walk<false><<<(b1 - b0 + kIdxWarps - 1) / kIdxWarps, kIdxWarps * 32, smem, st>>>(
-            r->d_data, r->d_blk_off, r->d_blk_size, b1, j.d_nrec, j.d_lastlen, nullptr, nullptr, nullptr, nullptr, nullptr, 0, j.d_stats, b0);
-        e->launches++;
+        upload_pass1(e, j, b0, b1);
         b0 = b1;
     }
-    PGS_CUDA(cudaMemcpyAsync(j.nrec, j.d_nrec, sizeof(uint32_t) * nb, cudaMemcpyDeviceToHost, st));
-    PGS_CUDA(cudaMemcpyAsync(j.lastlen, j.d_lastlen, sizeof(uint32_t) * nb, cudaMemcpyDeviceToHost, st));
-    PGS_CUDA(cudaMemcpyAsync(j.hs_out, j.d_stats, sizeof(IndexStats), cudaMemcpyDeviceToHost, st));
-    PGS_CUDA(cudaEventCreateWithFlags(&j.pass1, cudaEventDisableTiming));
-    PGS_CUDA(cudaEventRecord(j.pass1, st));
-    return PGS_OK;
+    return upload_pass1_done(e, j);
 }
 
 static int32_t upload_stage_b(Engine *e, UploadJob &j)
@@ -494,6 +516,104 @@ int32_t pgs_run_upload_many(pgs_partition *ph, const pgs_run_src *runs, uint32_t
         return rc;
     }
     if (run_ids_out) for (uint32_t i = 0; i < n; i++) run_ids_out[i] = ids[i];
+    return PGS_OK;
+}
+
+// device times of the calling thread's last pgs_run_build: input copy, plan (record, next, chain and scan passes), blocks, index
+static thread_local float t_build_ms[4] = {0, 0, 0, 0};
+void pgs_run_build_last_ms(float *ms) { memcpy(ms, t_build_ms, sizeof t_build_ms); }
+
+int32_t pgs_run_build(pgs_partition *ph, int32_t level, uint64_t n, const uint8_t *keys, const uint64_t *key_off, const uint8_t *vals,
+                      const uint64_t *val_off, const uint64_t *seq, const uint8_t *type, uint64_t *run_id_out)
+{
+    if (!ph || level < 0 || (n && (!key_off || !val_off || !seq || !type))) return PGS_INVALID_ARGUMENT;
+    if (n && ((!keys && key_off[n]) || (!vals && val_off[n]))) return PGS_INVALID_ARGUMENT;
+    if (run_id_out) *run_id_out = 0;
+    memset(t_build_ms, 0, sizeof t_build_ms);
+    if (n == 0) return PGS_OK; // an empty run: id 0, nothing resident
+    if (n > kBuildMaxRecords) {
+        set_error("run build: %llu records exceed the index's 32-bit record offsets", (unsigned long long)n);
+        return PGS_NOT_SUPPORTED;
+    }
+    Partition &p = ph->p;
+    Engine *e = p.eng;
+    PGS_CUDA(cudaSetDevice(e->device));
+    cudaStream_t st = e->stream;
+    LaunchScratch S(st);
+    cudaEvent_t ev[5];
+    for (auto &x : ev) PGS_CUDA(S.event(x));
+    PGS_CUDA(cudaEventRecord(ev[0], st));
+    // the whole input goes to the device
+    BuildParams P{};
+    build_plan(P, (uint32_t)n, e->cfg.block_size, e->cfg.restart_interval);
+    const uint64_t kb = key_off[n], vb = val_off[n];
+    uint8_t *d_keys, *d_vals;
+    PGS_CUDA(S.alloc(d_keys, kb + 16));
+    PGS_CUDA(S.alloc(d_vals, vb + 16));
+    if (kb) PGS_CUDA(cudaMemcpyAsync(d_keys, keys, kb, cudaMemcpyHostToDevice, st));
+    if (vb) PGS_CUDA(cudaMemcpyAsync(d_vals, vals, vb, cudaMemcpyHostToDevice, st));
+    PGS_CUDA(S.upload(P.key_off, (const unsigned long long *)key_off, n + 1));
+    PGS_CUDA(S.upload(P.val_off, (const unsigned long long *)val_off, n + 1));
+    PGS_CUDA(S.upload(P.seq, (const unsigned long long *)seq, n));
+    PGS_CUDA(S.upload(P.type, type, n));
+    P.keys = d_keys;
+    P.vals = d_vals;
+    cudaError_t ce = cudaSuccess;
+    build_buffers(P, [&](auto *&q, uint64_t cnt, int fill) {
+        const size_t bytes = sizeof(*q) * cnt;
+        if (ce != cudaSuccess) return;
+        ce = S.alloc(q, bytes ? bytes : 16);
+        if (ce == cudaSuccess && fill != kNoFill) ce = cudaMemsetAsync(q, fill, bytes, st);
+    });
+    PGS_CUDA(ce);
+    PGS_CUDA(cudaEventRecord(ev[1], st));
+    e->launches += build_launch_plan(P, 0, st, [](int) {});
+    size_t pin_cap = 0;
+    auto *hsum = (BuildSummary *)e->take_pinned(sizeof(BuildSummary), &pin_cap);
+    if (!hsum) { set_error("run build: no pinned staging memory"); return PGS_IO_ERROR; }
+    ce = cudaMemcpyAsync(hsum, P.sum, sizeof(BuildSummary), cudaMemcpyDeviceToHost, st);
+    if (ce == cudaSuccess) ce = cudaEventRecord(ev[2], st);
+    if (ce == cudaSuccess) ce = cudaEventSynchronize(ev[2]);
+    const BuildSummary sum = *hsum;
+    e->give_pinned(hsum, pin_cap);
+    PGS_CUDA(ce);
+    if (const int32_t rc = build_status(sum.flags)) {
+        set_error(rc == PGS_INVALID_ARGUMENT ? "run build: records out of internal-key order, or offsets out of range"
+                                             : "run build: a user key over %u bytes, or a block over 4 GB", kMaxUkeyLen);
+        return rc;
+    }
+    // the blocks are written into the run's buffer, where the upload's passes take them
+    const uint32_t nb = (uint32_t)sum.n_blocks;
+    UploadJob j;
+    j.max_blk = sum.max_blk;
+    int32_t rc = upload_job_init(e, level, nb, sum.data_bytes, j);
+    if (rc == PGS_OK) {
+        Run *r = j.r.get();
+        P.data = r->d_data;
+        ce = cudaMemsetAsync(r->d_data + sum.data_bytes, 0, r->data_cap - sum.data_bytes, st);
+        if (ce == cudaSuccess) ce = cudaMemcpyAsync(r->d_blk_off, P.blk_off, sizeof(uint64_t) * (nb + 1), cudaMemcpyDeviceToDevice, st);
+        if (ce == cudaSuccess) ce = cudaMemcpyAsync(r->d_blk_size, P.blk_size, sizeof(uint32_t) * nb, cudaMemcpyDeviceToDevice, st);
+        if (ce == cudaSuccess) {
+            e->launches += build_launch_blocks(P, nb, 0, st);
+            ce = cudaEventRecord(ev[3], st);
+        }
+        rc = ce == cudaSuccess ? PGS_OK : cuda_fail(ce, "run build: blocks");
+    }
+    if (rc == PGS_OK) {
+        upload_pass1(e, j, 0, nb);
+        rc = upload_pass1_done(e, j);
+    }
+    if (rc == PGS_OK) rc = upload_stage_b(e, j);
+    if (rc == PGS_OK) {
+        ce = cudaEventRecord(ev[4], st);
+        rc = ce == cudaSuccess ? upload_stage_c(e, p, j, run_id_out) : cuda_fail(ce, "run build: index");
+    }
+    if (rc != PGS_OK) {
+        upload_abandon(e, j);
+        return rc;
+    }
+    if (cudaEventSynchronize(ev[4]) == cudaSuccess)
+        for (int i = 0; i < 4; i++) cudaEventElapsedTime(&t_build_ms[i], ev[i], ev[i + 1]);
     return PGS_OK;
 }
 

@@ -131,15 +131,33 @@ struct Server {
     int32_t flush_mem()
     {
         if (mem.empty()) return PGS_OK;
-        RunBuilder rb(eng->cfg.block_size, eng->cfg.restart_interval);
+        // the memtable (sorted, one version per key) flattened into pinned staging: key_off | val_off | seq | type | keys | values;
+        // the device encodes the blocks (pgs_run_build)
+        const uint64_t n = mem.size();
+        uint64_t kb = 0, vb = 0;
+        for (auto &kv : mem) { kb += kv.first.size(); vb += kv.second.value.size(); }
+        size_t cap = 0;
+        uint8_t *pin = (uint8_t *)eng->take_pinned(8 * (3 * n + 2) + n + kb + vb, &cap);
+        if (!pin) { set_error("flush: no pinned staging memory"); return PGS_IO_ERROR; }
+        uint64_t *key_off = (uint64_t *)pin, *val_off = key_off + n + 1, *seq = val_off + n + 1;
+        uint8_t *type = (uint8_t *)(seq + n), *keys = type + n, *vals = keys + kb;
+        uint64_t i = 0, ko = 0, vo = 0;
         for (auto &kv : mem) {
-            int32_t st = rb.add(kv.first, kv.second.seq, kv.second.type, kv.second.value);
-            if (st != PGS_OK) return st;
+            key_off[i] = ko;
+            val_off[i] = vo;
+            seq[i] = kv.second.seq;
+            type[i] = kv.second.type;
+            memcpy(keys + ko, kv.first.data(), kv.first.size());
+            memcpy(vals + vo, kv.second.value.data(), kv.second.value.size());
+            ko += kv.first.size();
+            vo += kv.second.value.size();
+            i++;
         }
-        rb.finish();
+        key_off[n] = ko;
+        val_off[n] = vo;
         uint64_t id = 0;
-        int32_t st = pgs_run_upload(part, 0, (const uint8_t *)rb.data().data(), rb.data().size(), rb.blk_off().data(),
-                                    rb.blk_size().data(), (uint32_t)rb.blk_off().size(), &id);
+        int32_t st = pgs_run_build(part, 0, n, keys, key_off, vals, val_off, seq, type, &id);
+        eng->give_pinned(pin, cap);
         if (st != PGS_OK) return st;
         mem.clear();
         mem_bytes = 0;

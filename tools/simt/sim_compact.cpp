@@ -4,6 +4,7 @@
 #include "simt.h"
 
 #define PGS_SIM 1
+#include "../../incubator_pegasus_b200/csrc/build_kernels.cuh"
 #include "../../incubator_pegasus_b200/csrc/compact_kernels.cuh"
 #include "../../incubator_pegasus_b200/csrc/hotkey_kernels.cuh"
 #include "../../incubator_pegasus_b200/csrc/index_kernel.cuh"
@@ -118,6 +119,11 @@ struct Merged { // the output of the last sim_compact call
     MergeStats st{};
     uint32_t Q = 0;
 } g_res;
+
+struct Built { // the run of the last sim_run_build call
+    HostRun run;
+    uint64_t data_bytes = 0;
+} g_built;
 
 struct Split { // the children of the last sim_split call
     std::vector<HostRun> child;
@@ -501,6 +507,60 @@ int32_t sim_split_child_bloom_check(uint32_t c, const uint8_t *key, uint32_t len
 {
     const HostRun &r = g_split.child[c];
     return bloom_may_contain(r.d_bloom, r.bloom_lines, bloom_hash_bytes(key, len)) ? 1 : 0;
+}
+
+// n flat records built into a run through build_plan / build_buffers / build_launch_plan / build_launch_blocks as pgs_run_build
+// runs them, then indexed by the upload's two passes.  grid_cap: at most this many CTAs per launch (0: the product's grids).
+// Returns pgs_run_build's status; on PGS_OK the run stays in a static buffer until the next call (sim_run_build_* read it).
+int32_t sim_run_build(uint64_t n, const uint8_t *keys, const uint64_t *key_off, const uint8_t *vals, const uint64_t *val_off,
+                      const uint64_t *seq, const uint8_t *type, uint32_t block_size, uint32_t restart_interval, uint32_t grid_cap)
+{
+    Built &R = g_built;
+    R = Built{};
+    if (n == 0) return PGS_OK;
+    if (n > kBuildMaxRecords) return PGS_NOT_SUPPORTED;
+    HostMem scratch;
+    BuildParams P{};
+    build_plan(P, (uint32_t)n, block_size, restart_interval);
+    uint8_t *k, *v, *t;
+    unsigned long long *ko, *vo, *sq;
+    memcpy(host_alloc(scratch, k, key_off[n] + 16, 0), keys, key_off[n]); // the library's slack
+    memcpy(host_alloc(scratch, v, val_off[n] + 16, 0), vals, val_off[n]);
+    memcpy(host_alloc(scratch, ko, n + 1, 0), key_off, 8 * (n + 1));
+    memcpy(host_alloc(scratch, vo, n + 1, 0), val_off, 8 * (n + 1));
+    memcpy(host_alloc(scratch, sq, n, 0), seq, 8 * n);
+    memcpy(host_alloc(scratch, t, n, 0), type, n);
+    P.keys = k; P.vals = v; P.type = t; P.key_off = ko; P.val_off = vo; P.seq = sq;
+    build_buffers(P, [&](auto *&p, uint64_t cnt, int fill) { host_alloc(scratch, p, cnt, fill == kNoFill ? 0xEE : fill); });
+    build_launch_plan(P, grid_cap, nullptr, [](int) {});
+    const BuildSummary sum = *P.sum;
+    if (const int32_t rc = build_status(sum.flags)) return rc;
+    const uint32_t nb = (uint32_t)sum.n_blocks;
+    HostRun &r = R.run;
+    host_alloc(r.mem, r.d_data, sum.data_bytes + 256, 0xEE); // the library's slack, zeroed below as the library does
+    memset(r.d_data + sum.data_bytes, 0, 256);
+    memcpy(host_alloc(r.mem, r.d_blk_off, nb + 1, 0), P.blk_off, 8 * (size_t)(nb + 1));
+    memcpy(host_alloc(r.mem, r.d_blk_size, nb, 0), P.blk_size, 4 * (size_t)nb);
+    P.data = r.d_data;
+    build_launch_blocks(P, nb, grid_cap, nullptr);
+    R.data_bytes = sum.data_bytes;
+    if (const int32_t rc = build_index(r, nb)) return rc;
+    if (r.info.max_block_size != sum.max_blk) { fprintf(stderr, "sim_run_build: largest block %u, the index saw %u\n", sum.max_blk, r.info.max_block_size); return PGS_CORRUPTION; }
+    return PGS_OK;
+}
+// the last sim_run_build's sizes and info (level and run id zero)
+void sim_run_build_info(uint64_t *data_bytes, uint32_t *n_blocks, pgs_run_info *info)
+{
+    *data_bytes = g_built.data_bytes;
+    *n_blocks = g_built.run.info.n_blocks;
+    *info = g_built.run.info;
+}
+void sim_run_build_copy(uint8_t *data, uint64_t *blk_off, uint32_t *blk_size)
+{
+    const HostRun &r = g_built.run;
+    memcpy(data, r.d_data, g_built.data_bytes);
+    memcpy(blk_off, r.d_blk_off, 8 * (size_t)r.info.n_blocks);
+    memcpy(blk_size, r.d_blk_size, 4 * (size_t)r.info.n_blocks);
 }
 
 } // extern "C"
