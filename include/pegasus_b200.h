@@ -190,7 +190,7 @@ typedef struct {
     uint32_t default_ttl;
     int32_t pidx;
     int32_t partition_version;
-    const uint8_t *ops; /* may be NULL */
+    const uint8_t *ops; /* may be NULL; a malformed table: pgs_compact returns PGS_INVALID_ARGUMENT */
     uint32_t ops_len;
 } pgs_filter_params;
 
@@ -272,8 +272,9 @@ PGS_API int32_t pgs_partition_split(pgs_partition *src, uint32_t src_count, uint
                                     pgs_partition *const *dst, uint32_t n_dst, pgs_split_result *out);
 
 /* Parse the JSON of the `user_specified_compaction` env (compaction_operation.cpp:162-186) into
- * the binary ops table.  Invalid JSON / rules yield an empty table like the reference.  Returns
- * bytes written (<= cap) or a negative status. */
+ * the binary ops table.  Invalid JSON / rules yield an empty table like the reference.  A pattern
+ * longer than 65 535 bytes (it matches no key) is stored as the empty pattern; an op of more than
+ * 65 535 rules: -PGS_INVALID_ARGUMENT.  Returns bytes written (<= cap) or a negative status. */
 PGS_API int64_t pgs_compaction_ops_parse(const char *json, uint32_t json_len, uint32_t data_version,
                                          uint8_t *out, uint32_t cap, uint32_t *n_ops_out);
 

@@ -81,7 +81,8 @@ extern "C" int32_t pgs_compact_ex(pgs_partition *ph, const uint64_t *run_ids, ui
     P.bottommost = bottommost ? 1 : 0;
     P.now = now;
     P.data_version = part.data_version;
-    const uint32_t ops_len = compact_filter(P, fp);
+    uint32_t ops_len = 0;
+    if (!compact_filter(P, fp, ops_len)) { set_error("compact: malformed ops table of %u bytes", fp->ops_len); return PGS_INVALID_ARGUMENT; }
     if (P.validate_hash) P.crc_table = (const unsigned long long *)e->d_crc;
     CompactGeometry geo{};
     uint32_t force_G = 0; // diagnostics: PGS_WALK_G = lanes per merge group (1, 2, 4, 8, 16)

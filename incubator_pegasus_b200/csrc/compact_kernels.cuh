@@ -328,19 +328,23 @@ inline bool compact_geometry(MergeParams &P, const CompactTotals &T, uint32_t ma
 // the shared memory a compaction launch is planned for: the device's opt-in maximum per CTA less 1 KB (226 KB on an H100)
 inline uint32_t compact_smem_budget(uint32_t max_smem_optin) { return max_smem_optin - 1024; }
 
-// the filter and policy fields of P from the caller's filter parameters (nullptr: no filter); returns how many bytes of
-// fp->ops the launch needs in device memory at P.ops (0: no user ops)
-inline uint32_t compact_filter(MergeParams &P, const pgs_filter_params *fp)
+// the filter and policy fields of P from the caller's filter parameters (nullptr: no filter); ops_len = how many bytes of
+// fp->ops the launch needs in device memory at P.ops (0: no user ops).  Returns false, and nothing may be launched, when
+// fp->ops is not a well-formed ops table (ops_table_valid).
+inline bool compact_filter(MergeParams &P, const pgs_filter_params *fp, uint32_t &ops_len)
 {
-    if (!fp) return 0;
+    ops_len = 0;
+    if (!fp) return true;
     P.enabled = fp->enabled;
     P.validate_hash = fp->validate_hash;
     P.default_ttl = fp->default_ttl;
     P.pidx = fp->pidx;
     P.partition_version = fp->partition_version;
-    if (!fp->ops || fp->ops_len < 4) return 0;
+    if (!fp->ops || fp->ops_len == 0) return true;
+    if (!ops_table_valid(fp->ops, fp->ops_len)) return false;
     memcpy(&P.n_ops, fp->ops, 4);
-    return fp->ops_len;
+    ops_len = fp->ops_len;
+    return true;
 }
 
 // Every buffer of one launch: buf(pointer, elements, fill, out) allocates the elements and, unless fill is kNoFill, sets each

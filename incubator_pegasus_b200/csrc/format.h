@@ -116,6 +116,30 @@ enum { RULE_HASHKEY = 0, RULE_SORTKEY = 1, RULE_TTL_RANGE = 2 };
 enum { MATCH_ANYWHERE = 0, MATCH_PREFIX = 1, MATCH_POSTFIX = 2, MATCH_INVALID = 3 };
 enum { TTL_FROM_NOW = 0, TTL_FROM_CURRENT = 1, TTL_TIMESTAMP = 2, TTL_INVALID = 3 };
 
+// true when t[0..len) is a table of the form above that the compaction kernel may walk: every op and rule type is known and
+// the walk ends exactly at len.  A caller of the C ABI may hand in any bytes; the kernel trusts the framing.
+inline bool ops_table_valid(const uint8_t *t, uint64_t len)
+{
+    if (len < 4) return false;
+    const uint32_t n_ops = t[0] | (uint32_t)t[1] << 8 | (uint32_t)t[2] << 16 | (uint32_t)t[3] << 24;
+    uint64_t p = 4;
+    for (uint32_t o = 0; o < n_ops; o++) {
+        if (len - p < 8) return false;
+        const uint32_t op_type = t[p], ttl_type = t[p + 1], n_rules = t[p + 2] | (uint32_t)t[p + 3] << 8;
+        if (op_type > OP_DELETE || ttl_type > TTL_INVALID) return false;
+        p += 8;
+        for (uint32_t r = 0; r < n_rules; r++) {
+            if (len - p < 12) return false;
+            const uint32_t rule_type = t[p], match_type = t[p + 1], pl = t[p + 2] | (uint32_t)t[p + 3] << 8;
+            if (rule_type > RULE_TTL_RANGE || match_type > MATCH_INVALID) return false;
+            const uint64_t step = 12 + ((pl + 3) & ~3u);
+            if (len - p < step) return false;
+            p += step;
+        }
+    }
+    return p == len;
+}
+
 // what kernels see of one HBM-resident sorted run
 struct RunDev {
     const uint8_t *data;      // blocks, each start 16-aligned; readable up to blk_off[nb] (+slack)

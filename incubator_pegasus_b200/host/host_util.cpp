@@ -226,16 +226,29 @@ struct Parser {
             case 'f': o.push_back('\f'); break;
             case '"': case '\\': case '/': o.push_back(c); break;
             case 'u': {
-                if (end - p < 4) return false;
-                unsigned cp = 0;
-                for (int i = 0; i < 4; i++) {
-                    char h = *p++;
-                    cp = cp * 16 + (h >= '0' && h <= '9' ? h - '0' : h >= 'a' && h <= 'f' ? h - 'a' + 10 : h >= 'A' && h <= 'F' ? h - 'A' + 10 : 0xFFFF);
-                    if (cp > 0xFFFFF) return false;
+                auto hex4 = [&](unsigned &cp) {
+                    if (end - p < 4) return false;
+                    cp = 0;
+                    for (int i = 0; i < 4; i++) {
+                        char h = *p++;
+                        cp = cp * 16 + (h >= '0' && h <= '9' ? h - '0' : h >= 'a' && h <= 'f' ? h - 'a' + 10 : h >= 'A' && h <= 'F' ? h - 'A' + 10 : 0xFFFF);
+                        if (cp > 0xFFFFF) return false;
+                    }
+                    return true;
+                };
+                unsigned cp;
+                if (!hex4(cp)) return false;
+                if (cp >= 0xD800 && cp <= 0xDFFF) { // RapidJSON: a high surrogate needs a low one after it; a lone low one is an error
+                    unsigned lo;
+                    if (cp > 0xDBFF || end - p < 2 || p[0] != '\\' || p[1] != 'u') return false;
+                    p += 2;
+                    if (!hex4(lo) || lo < 0xDC00 || lo > 0xDFFF) return false;
+                    cp = (((cp - 0xD800) << 10) | (lo - 0xDC00)) + 0x10000;
                 }
                 if (cp < 0x80) o.push_back((char)cp);
                 else if (cp < 0x800) { o.push_back((char)(0xC0 | cp >> 6)); o.push_back((char)(0x80 | (cp & 63))); }
-                else { o.push_back((char)(0xE0 | cp >> 12)); o.push_back((char)(0x80 | ((cp >> 6) & 63))); o.push_back((char)(0x80 | (cp & 63))); }
+                else if (cp < 0x10000) { o.push_back((char)(0xE0 | cp >> 12)); o.push_back((char)(0x80 | ((cp >> 6) & 63))); o.push_back((char)(0x80 | (cp & 63))); }
+                else { o.push_back((char)(0xF0 | cp >> 18)); o.push_back((char)(0x80 | ((cp >> 12) & 63))); o.push_back((char)(0x80 | ((cp >> 6) & 63))); o.push_back((char)(0x80 | (cp & 63))); }
                 break;
             }
             default: return false;
@@ -426,19 +439,24 @@ int64_t ops_parse(std::string_view json, uint32_t /*data_version*/, std::string 
         } else {
             continue;
         }
+        // the table's counts are 16-bit: more rules than that cannot be framed, so the whole env is refused
+        if (rules.size() > 0xFFFF) { out.clear(); if (n_ops_out) *n_ops_out = 0; return -PGS_INVALID_ARGUMENT; }
         uint16_t nr = (uint16_t)rules.size();
         out.push_back((char)op_type);
         out.push_back((char)ttl_type);
         out.append((const char *)&nr, 2);
         out.append((const char *)&ttl_value, 4);
         for (auto &r : rules) {
-            uint16_t pl = (uint16_t)r.pattern.size();
+            // a pattern longer than 65 535 bytes is longer than any hash key (16-bit length) or user key (kMaxUkeyLen), so
+            // it never matches; it is stored as the empty pattern, which never matches either (string_pattern_match)
+            const bool fits = r.pattern.size() <= 0xFFFF;
+            uint16_t pl = fits ? (uint16_t)r.pattern.size() : 0;
             out.push_back((char)r.type);
             out.push_back((char)r.match);
             out.append((const char *)&pl, 2);
             out.append((const char *)&r.start_ttl, 4);
             out.append((const char *)&r.stop_ttl, 4);
-            out += r.pattern;
+            if (fits) out += r.pattern;
             while (out.size() % 4) out.push_back(0);
         }
         n_ops++;
@@ -550,6 +568,7 @@ int64_t pgs_compaction_ops_parse(const char *json, uint32_t json_len, uint32_t d
 {
     std::string bin;
     int64_t n = ops_parse(std::string_view(json, json_len), data_version, bin, n_ops_out);
+    if (n < 0) return n;
     if ((uint64_t)n > cap) return -PGS_INCOMPLETE;
     memcpy(out, bin.data(), bin.size());
     return n;

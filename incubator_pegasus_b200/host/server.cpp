@@ -681,7 +681,7 @@ int32_t pgs_rrdb_update_app_envs(pgs_server *h, const char *envs, uint32_t n_env
         }
         auto fo = em.find("user_specified_compaction"); // :2985-3001: absent -> cleared
         if (fo == em.end()) s.ops_bin.clear();
-        else { s.ops_bin.clear(); if (!fo->second.empty()) ops_parse(fo->second, s.data_version, s.ops_bin, nullptr); }
+        else { s.ops_bin.clear(); if (!fo->second.empty() && ops_parse(fo->second, s.data_version, s.ops_bin, nullptr) < 0) s.ops_bin.clear(); }
     }
     // start_manual_compact_if_needed (pegasus_manual_compact_service.cpp:83-121): the disabled flag, the running-count limit, then
     // the `once` rule and, when it does not fire, the `periodic` one (times of the local day that holds `now`); the compaction

@@ -123,20 +123,34 @@ struct JP {
                 case 'r': out += '\r'; break;
                 case 't': out += '\t'; break;
                 case 'u': {
-                    if (e - p < 5) return false;
-                    unsigned cp = 0;
-                    for (int i = 1; i <= 4; i++) {
-                        char c = p[i];
-                        cp <<= 4;
-                        if (c >= '0' && c <= '9') cp |= c - '0';
-                        else if (c >= 'a' && c <= 'f') cp |= c - 'a' + 10;
-                        else if (c >= 'A' && c <= 'F') cp |= c - 'A' + 10;
-                        else return false;
+                    // p points at the 'u' of an escape; reads its four hex digits and leaves p on the last one
+                    auto hex4 = [&](unsigned &cp) {
+                        if (e - p < 5) return false;
+                        cp = 0;
+                        for (int i = 1; i <= 4; i++) {
+                            char c = p[i];
+                            cp <<= 4;
+                            if (c >= '0' && c <= '9') cp |= c - '0';
+                            else if (c >= 'a' && c <= 'f') cp |= c - 'a' + 10;
+                            else if (c >= 'A' && c <= 'F') cp |= c - 'A' + 10;
+                            else return false;
+                        }
+                        p += 4;
+                        return true;
+                    };
+                    unsigned cp;
+                    if (!hex4(cp)) return false;
+                    if (cp >= 0xD800 && cp <= 0xDFFF) { // RapidJSON's surrogate rule: a high surrogate and a low one make one code point
+                        unsigned lo;
+                        if (cp > 0xDBFF || e - p < 3 || p[1] != '\\' || p[2] != 'u') return false;
+                        p += 2;
+                        if (!hex4(lo) || lo < 0xDC00 || lo > 0xDFFF) return false;
+                        cp = (((cp - 0xD800) << 10) | (lo - 0xDC00)) + 0x10000;
                     }
-                    p += 4;
                     if (cp < 0x80) out += (char)cp;
                     else if (cp < 0x800) { out += (char)(0xC0 | (cp >> 6)); out += (char)(0x80 | (cp & 0x3F)); }
-                    else { out += (char)(0xE0 | (cp >> 12)); out += (char)(0x80 | ((cp >> 6) & 0x3F)); out += (char)(0x80 | (cp & 0x3F)); }
+                    else if (cp < 0x10000) { out += (char)(0xE0 | (cp >> 12)); out += (char)(0x80 | ((cp >> 6) & 0x3F)); out += (char)(0x80 | (cp & 0x3F)); }
+                    else { out += (char)(0xF0 | (cp >> 18)); out += (char)(0x80 | ((cp >> 12) & 0x3F)); out += (char)(0x80 | ((cp >> 6) & 0x3F)); out += (char)(0x80 | (cp & 0x3F)); }
                     break;
                 }
                 default: return false;
@@ -467,6 +481,9 @@ DropReason compaction_filter(const FilterParams &fp, sv key, sv value, uint32_t 
 {
     if (!fp.enabled) return kKeep;     // :61-63
     if (key.size() < 2) return kKeep;  // :67-69 (empty write)
+    // a value too short for its expire_ts header: pegasus_extract_expire_ts reads past it (an assert of data_input that
+    // release builds compile out); such a value is kept as it stands (DESIGN §8)
+    if (value.size() < 4) return kKeep;
     uint32_t expire_ts = extract_expire_ts(fp.data_version, value);
     sv entry = value;
     if (fp.default_ttl != 0 && expire_ts == 0) { // :73-79

@@ -32,7 +32,8 @@ def sim():
 
 
 def sim_compact(pgs, sim, runs, *, bottommost, now=synth.NOW, default_ttl=0, validate_hash=False, pidx=0, partition_version=-1,
-                ops=None, enabled=True, block_size=4096, restart_interval=16, lanes=0, seg_weight=0):
+                ops=None, enabled=True, block_size=4096, restart_interval=16, lanes=0, seg_weight=0, data_version=1, status=0):
+    # status: the status sim_compact must return; a failed launch returns (None, None)
     # an input given as a BlockRun is merged as it stands (tests/foreign_blocks.py writes such runs)
     brs = [r if isinstance(r, pgs.BlockRun) else pgs.build_run(r, block_size, restart_interval) for r in runs]
     k = len(brs)
@@ -44,7 +45,7 @@ def sim_compact(pgs, sim, runs, *, bottommost, now=synth.NOW, default_ttl=0, val
     fp = pgs.FilterParams()
     fp.enabled = 1 if enabled else 0
     fp.validate_hash = 1 if validate_hash else 0
-    fp.data_version = 1
+    fp.data_version = data_version
     fp.default_ttl = default_ttl
     fp.pidx = pidx
     fp.partition_version = partition_version
@@ -54,7 +55,9 @@ def sim_compact(pgs, sim, runs, *, bottommost, now=synth.NOW, default_ttl=0, val
     crc = (C.c_uint64 * 256)(*crc_table()) if validate_hash else None
     st = sim.sim_compact(k, data, nbytes, off, size, nb, block_size, restart_interval, 1 if bottommost else 0, C.byref(fp), now,
                          lanes, C.c_uint64(seg_weight), crc)
-    assert st == 0, st
+    assert st == status, st
+    if st:
+        return None, None
     db, nblk, nseg = C.c_uint64(), C.c_uint32(), C.c_uint32()
     sim.sim_result_sizes(C.byref(db), C.byref(nblk), C.byref(nseg))
     n = nblk.value
@@ -113,19 +116,21 @@ def check(pgs, oracle, sim, runs, *, bottommost, ops_json=None, **kw):
     if "lanes" not in kw:  # the one-thread-per-segment shape and a lane-group shape of the same source
         check(pgs, oracle, sim, runs, bottommost=bottommost, ops_json=ops_json, lanes=8, **kw)
         kw["lanes"] = 1
-    ops_bin = pgs.parse_ops(ops_json) if ops_json else None
+    ops_bin = pgs.parse_ops(ops_json, kw.get("data_version", 1)) if ops_json else None
     got_run, x = sim_compact(pgs, sim, runs, bottommost=bottommost, ops=ops_bin, **kw)
-    okw = {k: v for k, v in kw.items() if k in ("enabled", "default_ttl", "validate_hash", "pidx", "partition_version")}
-    oops = oracle.Ops(ops_json) if ops_json else None  # keeps the parsed table alive across orc_compact
+    okw = {k: v for k, v in kw.items() if k in ("enabled", "default_ttl", "validate_hash", "pidx", "partition_version", "data_version")}
+    oops = oracle.Ops(ops_json, okw.get("data_version", 1)) if ops_json else None  # keeps the parsed table alive across orc_compact
     fp = oracle.filter_params(ops=oops, **okw)
     want_run, st = oracle.compact([oracle.Run.from_records(r) for r in runs], bottommost, fp, kw.get("now", synth.NOW))
     want = want_run.records()
     for i, f in enumerate(STAT_FIELDS):
         assert x["stats"][i] == getattr(st, f), (f, x["stats"][i], getattr(st, f))
+    x["got"] = []
     if want.n == 0:
         assert got_run.n_blocks == 0
         return x
     got = pgs.decode_blocks(got_run)
+    x["got"] = got.to_list()
     assert got.n == want.n, (got.n, want.n)
     assert got.same_as(want)
     assert got.same_as(oracle.Run.from_blocks(got_run).records())  # independent decoder of the raw blocks

@@ -154,9 +154,11 @@ int32_t sim_compact(uint32_t k, const uint8_t **data, const uint64_t *data_bytes
     P.restart_interval = restart_interval;
     P.bottommost = bottommost ? 1 : 0;
     P.now = now;
-    P.data_version = 1;
+    P.data_version = fp ? fp->data_version : 1;
     HostMem scratch;
-    if (const uint32_t n = compact_filter(P, fp)) {
+    uint32_t n = 0;
+    if (!compact_filter(P, fp, n)) return PGS_INVALID_ARGUMENT;
+    if (n) {
         uint8_t *ops;
         memcpy(host_alloc(scratch, ops, n, 0), fp->ops, n);
         P.ops = ops;
