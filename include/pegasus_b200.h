@@ -166,9 +166,32 @@ PGS_API int32_t pgs_run_build(pgs_partition *p, int32_t level, uint64_t n,
                               const uint8_t *vals, const uint64_t *val_off,
                               const uint64_t *seq, const uint8_t *type,
                               uint64_t *run_id_out);
-/* device times (ms) of the calling thread's last successful pgs_run_build: [0] input copy, [1] block plan (record, next-block,
- * chain and scan passes), [2] block writing, [3] index and Bloom filter (the upload's two passes) */
+/* pgs_run_build for n flat records in any order: they are sorted on the device into internal-key order (user keys bytewise as
+ * unsigned bytes, a proper prefix first; equal user keys by seq<<8|type descending), then built as pgs_run_build builds.  The
+ * installed run (blocks, handles, pgs_run_info) is byte for byte the one pgs_run_build makes from the same records stably sorted
+ * into internal-key order; only the run id differs.  Shadowed versions are kept (compaction drops them).
+ * Statuses, in this order of precedence:
+ *   offsets (key_off / val_off) not ascending: PGS_INVALID_ARGUMENT;
+ *   else a user key over 4096 bytes, or n > 0xFFFFFFF0: PGS_NOT_SUPPORTED;
+ *   else two records with the same user key, seq and type (a duplicate internal key): PGS_INVALID_ARGUMENT;
+ *   else pgs_run_build's statuses.
+ *   n == 0: PGS_OK, *run_id_out = 0, nothing resident.
+ * All or nothing: on an error the partition's run list is unchanged and every device buffer of the call is freed.
+ * Device memory: while sorting, the input (key_off[n] + val_off[n] + 32 bytes, and 25 bytes per record), the sorted copy (the
+ * same again) and the sort's scratch (60 bytes per record, plus about 1 KB per 4096 records); while building, the sorted copy,
+ * pgs_run_build's scratch (about 4 * ceil(log2 n) + 25 bytes per record) and the run.  The input and the sort's scratch are
+ * freed before the build's scratch is taken.
+ * Rounds: one per 8 bytes of the longest prefix two user keys share, plus two; each round costs the records still tied. */
+PGS_API int32_t pgs_run_build_unsorted(pgs_partition *p, int32_t level, uint64_t n,
+                                       const uint8_t *keys, const uint64_t *key_off,
+                                       const uint8_t *vals, const uint64_t *val_off,
+                                       const uint64_t *seq, const uint8_t *type, uint64_t *run_id_out);
+/* device times (ms) of the calling thread's last successful pgs_run_build or pgs_run_build_unsorted: [0] input copy, [1] block
+ * plan (record, next-block, chain and scan passes), [2] block writing, [3] index and Bloom filter (the upload's two passes) */
 PGS_API void pgs_run_build_last_ms(float *ms4);
+/* device time (ms) of the sort and the gather of the sorted copy in the calling thread's last successful pgs_run_build_unsorted
+ */
+PGS_API float pgs_run_build_last_sort_ms(void);
 PGS_API int32_t pgs_run_drop(pgs_partition *p, uint64_t run_id);
 PGS_API int32_t pgs_run_info_get(pgs_partition *p, uint64_t run_id, pgs_run_info *out);
 /* run ids in read order (newest first: L0 by recency, then L1, L2, ...) */

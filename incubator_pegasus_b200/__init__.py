@@ -207,6 +207,9 @@ def lib() -> C.CDLL:
     L.pgs_run_build.argtypes = [vp, C.c_int32, C.c_uint64, vp, vp, vp, vp, vp, vp, u64p]
     L.pgs_run_build_last_ms.argtypes = [C.POINTER(C.c_float)]
     L.pgs_run_build_last_ms.restype = None
+    L.pgs_run_build_unsorted.argtypes = [vp, C.c_int32, C.c_uint64, vp, vp, vp, vp, vp, vp, u64p]
+    L.pgs_run_build_last_sort_ms.argtypes = []
+    L.pgs_run_build_last_sort_ms.restype = C.c_float
     L.pgs_run_drop.argtypes = [vp, C.c_uint64]
     L.pgs_run_info_get.argtypes = [vp, C.c_uint64, C.POINTER(RunInfo)]
     L.pgs_run_list.argtypes = [vp, u64p, C.c_uint32, u32p]
@@ -581,6 +584,11 @@ def run_build_last_ms() -> list[float]:
     return list(ms)
 
 
+def run_build_last_sort_ms() -> float:
+    """device time (ms) of the sort and the gather of this thread's last Partition.build_records_unsorted"""
+    return float(lib().pgs_run_build_last_sort_ms())
+
+
 def partition_index(hash_key: bytes, sort_key: bytes, partition_count: int) -> int:
     return int(lib().pgs_partition_index(hash_key, len(hash_key), sort_key, len(sort_key), partition_count))
 
@@ -626,6 +634,14 @@ class Partition:
         rid = C.c_uint64()
         _check(lib().pgs_run_build(self.h, level, recs.n, _ptr(recs.keys), _ptr(recs.key_off), _ptr(recs.vals), _ptr(recs.val_off),
                                    _ptr(recs.seq), _ptr(recs.type), C.byref(rid)), "run_build")
+        return rid.value
+
+    def build_records_unsorted(self, recs: Records, level: int = 0) -> int:
+        """the run of `recs` in any order, sorted into internal-key order and built on the device (pgs_run_build_unsorted): the
+        same blocks and run info as build_records of the records sorted first; 0 for no records"""
+        rid = C.c_uint64()
+        _check(lib().pgs_run_build_unsorted(self.h, level, recs.n, _ptr(recs.keys), _ptr(recs.key_off), _ptr(recs.vals),
+                                            _ptr(recs.val_off), _ptr(recs.seq), _ptr(recs.type), C.byref(rid)), "run_build_unsorted")
         return rid.value
 
     def run_info(self, run_id: int) -> RunInfo:

@@ -10,6 +10,7 @@
 #include "build_kernels.cuh"
 #include "engine.h"
 #include "index_kernel.cuh"
+#include "sort_kernels.cuh"
 
 namespace pgs {
 
@@ -519,45 +520,19 @@ int32_t pgs_run_upload_many(pgs_partition *ph, const pgs_run_src *runs, uint32_t
     return PGS_OK;
 }
 
-// device times of the calling thread's last pgs_run_build: input copy, plan (record, next, chain and scan passes), blocks, index
+// device times of the calling thread's last pgs_run_build or pgs_run_build_unsorted: input copy, plan (record, next, chain and
+// scan passes), blocks, index; and the sort and gather of the last pgs_run_build_unsorted
 static thread_local float t_build_ms[4] = {0, 0, 0, 0};
+static thread_local float t_sort_ms = 0;
 void pgs_run_build_last_ms(float *ms) { memcpy(ms, t_build_ms, sizeof t_build_ms); }
+float pgs_run_build_last_sort_ms(void) { return t_sort_ms; }
 
-int32_t pgs_run_build(pgs_partition *ph, int32_t level, uint64_t n, const uint8_t *keys, const uint64_t *key_off, const uint8_t *vals,
-                      const uint64_t *val_off, const uint64_t *seq, const uint8_t *type, uint64_t *run_id_out)
+// The build from device copies of the records in internal-key order (P's inputs set): its scratch, ev[1], the plan, ev[2], the
+// blocks, ev[3], the index, ev[4], and the run installed.  On an error nothing is installed.
+static int32_t run_build_sorted(Engine *e, Partition &p, int32_t level, BuildParams &P, LaunchScratch &S, cudaEvent_t *ev,
+                                uint64_t *run_id_out)
 {
-    if (!ph || level < 0 || (n && (!key_off || !val_off || !seq || !type))) return PGS_INVALID_ARGUMENT;
-    if (n && ((!keys && key_off[n]) || (!vals && val_off[n]))) return PGS_INVALID_ARGUMENT;
-    if (run_id_out) *run_id_out = 0;
-    memset(t_build_ms, 0, sizeof t_build_ms);
-    if (n == 0) return PGS_OK; // an empty run: id 0, nothing resident
-    if (n > kBuildMaxRecords) {
-        set_error("run build: %llu records exceed the index's 32-bit record offsets", (unsigned long long)n);
-        return PGS_NOT_SUPPORTED;
-    }
-    Partition &p = ph->p;
-    Engine *e = p.eng;
-    PGS_CUDA(cudaSetDevice(e->device));
     cudaStream_t st = e->stream;
-    LaunchScratch S(st);
-    cudaEvent_t ev[5];
-    for (auto &x : ev) PGS_CUDA(S.event(x));
-    PGS_CUDA(cudaEventRecord(ev[0], st));
-    // the whole input goes to the device
-    BuildParams P{};
-    build_plan(P, (uint32_t)n, e->cfg.block_size, e->cfg.restart_interval);
-    const uint64_t kb = key_off[n], vb = val_off[n];
-    uint8_t *d_keys, *d_vals;
-    PGS_CUDA(S.alloc(d_keys, kb + 16));
-    PGS_CUDA(S.alloc(d_vals, vb + 16));
-    if (kb) PGS_CUDA(cudaMemcpyAsync(d_keys, keys, kb, cudaMemcpyHostToDevice, st));
-    if (vb) PGS_CUDA(cudaMemcpyAsync(d_vals, vals, vb, cudaMemcpyHostToDevice, st));
-    PGS_CUDA(S.upload(P.key_off, (const unsigned long long *)key_off, n + 1));
-    PGS_CUDA(S.upload(P.val_off, (const unsigned long long *)val_off, n + 1));
-    PGS_CUDA(S.upload(P.seq, (const unsigned long long *)seq, n));
-    PGS_CUDA(S.upload(P.type, type, n));
-    P.keys = d_keys;
-    P.vals = d_vals;
     cudaError_t ce = cudaSuccess;
     build_buffers(P, [&](auto *&q, uint64_t cnt, int fill) {
         const size_t bytes = sizeof(*q) * cnt;
@@ -608,12 +583,141 @@ int32_t pgs_run_build(pgs_partition *ph, int32_t level, uint64_t n, const uint8_
         ce = cudaEventRecord(ev[4], st);
         rc = ce == cudaSuccess ? upload_stage_c(e, p, j, run_id_out) : cuda_fail(ce, "run build: index");
     }
-    if (rc != PGS_OK) {
-        upload_abandon(e, j);
-        return rc;
+    if (rc != PGS_OK) upload_abandon(e, j);
+    return rc;
+}
+
+int32_t pgs_run_build(pgs_partition *ph, int32_t level, uint64_t n, const uint8_t *keys, const uint64_t *key_off, const uint8_t *vals,
+                      const uint64_t *val_off, const uint64_t *seq, const uint8_t *type, uint64_t *run_id_out)
+{
+    if (!ph || level < 0 || (n && (!key_off || !val_off || !seq || !type))) return PGS_INVALID_ARGUMENT;
+    if (n && ((!keys && key_off[n]) || (!vals && val_off[n]))) return PGS_INVALID_ARGUMENT;
+    if (run_id_out) *run_id_out = 0;
+    memset(t_build_ms, 0, sizeof t_build_ms);
+    if (n == 0) return PGS_OK; // an empty run: id 0, nothing resident
+    if (n > kBuildMaxRecords) {
+        set_error("run build: %llu records exceed the index's 32-bit record offsets", (unsigned long long)n);
+        return PGS_NOT_SUPPORTED;
     }
+    Partition &p = ph->p;
+    Engine *e = p.eng;
+    PGS_CUDA(cudaSetDevice(e->device));
+    cudaStream_t st = e->stream;
+    LaunchScratch S(st);
+    cudaEvent_t ev[5];
+    for (auto &x : ev) PGS_CUDA(S.event(x));
+    PGS_CUDA(cudaEventRecord(ev[0], st));
+    // the whole input goes to the device
+    BuildParams P{};
+    build_plan(P, (uint32_t)n, e->cfg.block_size, e->cfg.restart_interval);
+    const uint64_t kb = key_off[n], vb = val_off[n];
+    uint8_t *d_keys, *d_vals;
+    PGS_CUDA(S.alloc(d_keys, kb + 16));
+    PGS_CUDA(S.alloc(d_vals, vb + 16));
+    if (kb) PGS_CUDA(cudaMemcpyAsync(d_keys, keys, kb, cudaMemcpyHostToDevice, st));
+    if (vb) PGS_CUDA(cudaMemcpyAsync(d_vals, vals, vb, cudaMemcpyHostToDevice, st));
+    PGS_CUDA(S.upload(P.key_off, (const unsigned long long *)key_off, n + 1));
+    PGS_CUDA(S.upload(P.val_off, (const unsigned long long *)val_off, n + 1));
+    PGS_CUDA(S.upload(P.seq, (const unsigned long long *)seq, n));
+    PGS_CUDA(S.upload(P.type, type, n));
+    P.keys = d_keys;
+    P.vals = d_vals;
+    if (const int32_t rc = run_build_sorted(e, p, level, P, S, ev, run_id_out)) return rc;
     if (cudaEventSynchronize(ev[4]) == cudaSuccess)
         for (int i = 0; i < 4; i++) cudaEventElapsedTime(&t_build_ms[i], ev[i], ev[i + 1]);
+    return PGS_OK;
+}
+
+int32_t pgs_run_build_unsorted(pgs_partition *ph, int32_t level, uint64_t n, const uint8_t *keys, const uint64_t *key_off,
+                               const uint8_t *vals, const uint64_t *val_off, const uint64_t *seq, const uint8_t *type,
+                               uint64_t *run_id_out)
+{
+    if (!ph || level < 0 || (n && (!key_off || !val_off || !seq || !type))) return PGS_INVALID_ARGUMENT;
+    if (n && ((!keys && key_off[n]) || (!vals && val_off[n]))) return PGS_INVALID_ARGUMENT;
+    if (run_id_out) *run_id_out = 0;
+    memset(t_build_ms, 0, sizeof t_build_ms);
+    t_sort_ms = 0;
+    if (n == 0) return PGS_OK; // an empty run: id 0, nothing resident
+    if (n > kBuildMaxRecords) {
+        const int32_t rc = sort_status_too_many(n, key_off, val_off);
+        set_error(rc == PGS_INVALID_ARGUMENT ? "run build: offsets not ascending"
+                                             : "run build: %llu records exceed the index's 32-bit record offsets", (unsigned long long)n);
+        return rc;
+    }
+    Partition &p = ph->p;
+    Engine *e = p.eng;
+    PGS_CUDA(cudaSetDevice(e->device));
+    cudaStream_t st = e->stream;
+    LaunchScratch S(st);
+    cudaEvent_t ev[5], ev_copied, ev_read;
+    for (auto &x : ev) PGS_CUDA(S.event(x));
+    PGS_CUDA(S.event(ev_copied));
+    PGS_CUDA(S.event(ev_read));
+    PGS_CUDA(cudaEventRecord(ev[0], st));
+    BuildParams P{};
+    build_plan(P, (uint32_t)n, e->cfg.block_size, e->cfg.restart_interval);
+    {
+        // the input and the sort's scratch are freed (stream-ordered) once the sorted copy is written
+        LaunchScratch SS(st);
+        SortParams Q{};
+        sort_plan(Q, (uint32_t)n);
+        const uint64_t kb = key_off[n], vb = val_off[n];
+        uint8_t *d_keys, *d_vals;
+        PGS_CUDA(SS.alloc(d_keys, kb + 16));
+        PGS_CUDA(SS.alloc(d_vals, vb + 16));
+        if (kb) PGS_CUDA(cudaMemcpyAsync(d_keys, keys, kb, cudaMemcpyHostToDevice, st));
+        if (vb) PGS_CUDA(cudaMemcpyAsync(d_vals, vals, vb, cudaMemcpyHostToDevice, st));
+        PGS_CUDA(SS.upload(Q.key_off, (const unsigned long long *)key_off, n + 1));
+        PGS_CUDA(SS.upload(Q.val_off, (const unsigned long long *)val_off, n + 1));
+        PGS_CUDA(SS.upload(Q.seq, (const unsigned long long *)seq, n));
+        PGS_CUDA(SS.upload(Q.type, type, n));
+        Q.keys = d_keys;
+        Q.vals = d_vals;
+        PGS_CUDA(cudaEventRecord(ev_copied, st));
+        cudaError_t ce = cudaSuccess;
+        auto alloc_in = [&](LaunchScratch &to) {
+            return [&](auto *&q, uint64_t cnt, int fill) {
+                const size_t bytes = sizeof(*q) * cnt;
+                if (ce != cudaSuccess) return;
+                ce = to.alloc(q, bytes ? bytes : 16);
+                if (ce == cudaSuccess && fill != kNoFill) ce = cudaMemsetAsync(q, fill, bytes, st);
+            };
+        };
+        sort_buffers(Q, kb, vb, alloc_in(SS), alloc_in(S)); // the sorted copy lives as long as the build's scratch
+        PGS_CUDA(ce);
+        size_t pin_cap = 0;
+        auto *hsum = (SortSummary *)e->take_pinned(sizeof(SortSummary), &pin_cap);
+        if (!hsum) { set_error("run build: no pinned staging memory"); return PGS_IO_ERROR; }
+        uint32_t launches = 0;
+        const int32_t rc = sort_launch(Q, 0, st, [&](SortSummary &s) -> int32_t {
+            cudaError_t c = cudaMemcpyAsync(hsum, Q.sum, sizeof(SortSummary), cudaMemcpyDeviceToHost, st);
+            if (c == cudaSuccess) c = cudaEventRecord(ev_read, st);
+            if (c == cudaSuccess) c = cudaEventSynchronize(ev_read);
+            if (c != cudaSuccess) return cuda_fail(c, "run build: sort");
+            s = *hsum;
+            return PGS_OK;
+        }, launches);
+        e->give_pinned(hsum, pin_cap);
+        e->launches += launches;
+        if (rc) {
+            if (rc != PGS_IO_ERROR)
+                set_error(rc == PGS_INVALID_ARGUMENT ? "run build: offsets out of range, or two records with the same user key, seq and type"
+                                                     : "run build: a user key over %u bytes", kMaxUkeyLen);
+            return rc;
+        }
+        P.keys = Q.s_keys;
+        P.vals = Q.s_vals;
+        P.type = Q.s_type;
+        P.key_off = Q.s_key_off;
+        P.val_off = Q.s_val_off;
+        P.seq = Q.s_seq;
+    }
+    if (const int32_t rc = run_build_sorted(e, p, level, P, S, ev, run_id_out)) return rc;
+    if (cudaEventSynchronize(ev[4]) == cudaSuccess) {
+        cudaEventElapsedTime(&t_build_ms[0], ev[0], ev_copied);
+        cudaEventElapsedTime(&t_sort_ms, ev_copied, ev[1]);
+        for (int i = 1; i < 4; i++) cudaEventElapsedTime(&t_build_ms[i], ev[i], ev[i + 1]);
+    }
     return PGS_OK;
 }
 

@@ -116,3 +116,18 @@ def compaction_runs(k: int = 4, n_per_run: int = 25_000, hk_len: int = 16, sk_le
 
 def total_bytes(runs) -> int:
     return int(sum(r.keys.shape[0] + r.vals.shape[0] for r in runs))
+
+
+def shuffled(recs: Records, seed: int = 1) -> Records:
+    """the records of `recs` (fixed-width keys) in a seeded random order"""
+    n = recs.n
+    perm = np.random.default_rng(seed).permutation(n)
+    klen, vlen = np.diff(recs.key_off.astype(np.int64)), np.diff(recs.val_off.astype(np.int64))
+    kw = int(klen[0]) if n else 0
+    assert (klen == kw).all(), "fixed-width keys only"
+    keys = recs.keys[int(recs.key_off[0]):int(recs.key_off[0]) + n * kw].reshape(n, kw)[perm].reshape(-1)
+    voff = np.zeros(n + 1, np.uint64)
+    voff[1:] = np.cumsum(vlen[perm])
+    src = np.repeat(recs.val_off[:-1].astype(np.int64)[perm] - voff[:-1].astype(np.int64), vlen[perm]) + np.arange(int(voff[-1]))
+    return Records(np.ascontiguousarray(keys), np.arange(n + 1, dtype=np.uint64) * np.uint64(kw), recs.vals[src], voff,
+                   recs.seq[perm].copy(), recs.type[perm].copy())

@@ -10,6 +10,7 @@
 #include "../../incubator_pegasus_b200/csrc/index_kernel.cuh"
 #include "../../incubator_pegasus_b200/csrc/read_kernels.cuh"
 #include "../../incubator_pegasus_b200/csrc/scan_kernel.cuh"
+#include "../../incubator_pegasus_b200/csrc/sort_kernels.cuh"
 #include "../../incubator_pegasus_b200/csrc/split_kernels.cuh"
 
 #include <cstdarg>
@@ -511,28 +512,14 @@ int32_t sim_split_child_bloom_check(uint32_t c, const uint8_t *key, uint32_t len
     return bloom_may_contain(r.d_bloom, r.bloom_lines, bloom_hash_bytes(key, len)) ? 1 : 0;
 }
 
-// n flat records built into a run through build_plan / build_buffers / build_launch_plan / build_launch_blocks as pgs_run_build
-// runs them, then indexed by the upload's two passes.  grid_cap: at most this many CTAs per launch (0: the product's grids).
-// Returns pgs_run_build's status; on PGS_OK the run stays in a static buffer until the next call (sim_run_build_* read it).
-int32_t sim_run_build(uint64_t n, const uint8_t *keys, const uint64_t *key_off, const uint8_t *vals, const uint64_t *val_off,
-                      const uint64_t *seq, const uint8_t *type, uint32_t block_size, uint32_t restart_interval, uint32_t grid_cap)
+} // extern "C"
+
+namespace {
+// the build of records in internal-key order (P's inputs set) as pgs_run_build runs it: scratch, plan, blocks, then the upload's
+// two index passes.  Returns pgs_run_build's status; on PGS_OK the run is g_built's.
+int32_t build_sorted(BuildParams &P, HostMem &scratch, uint32_t grid_cap)
 {
     Built &R = g_built;
-    R = Built{};
-    if (n == 0) return PGS_OK;
-    if (n > kBuildMaxRecords) return PGS_NOT_SUPPORTED;
-    HostMem scratch;
-    BuildParams P{};
-    build_plan(P, (uint32_t)n, block_size, restart_interval);
-    uint8_t *k, *v, *t;
-    unsigned long long *ko, *vo, *sq;
-    memcpy(host_alloc(scratch, k, key_off[n] + 16, 0), keys, key_off[n]); // the library's slack
-    memcpy(host_alloc(scratch, v, val_off[n] + 16, 0), vals, val_off[n]);
-    memcpy(host_alloc(scratch, ko, n + 1, 0), key_off, 8 * (n + 1));
-    memcpy(host_alloc(scratch, vo, n + 1, 0), val_off, 8 * (n + 1));
-    memcpy(host_alloc(scratch, sq, n, 0), seq, 8 * n);
-    memcpy(host_alloc(scratch, t, n, 0), type, n);
-    P.keys = k; P.vals = v; P.type = t; P.key_off = ko; P.val_off = vo; P.seq = sq;
     build_buffers(P, [&](auto *&p, uint64_t cnt, int fill) { host_alloc(scratch, p, cnt, fill == kNoFill ? 0xEE : fill); });
     build_launch_plan(P, grid_cap, nullptr, [](int) {});
     const BuildSummary sum = *P.sum;
@@ -549,6 +536,68 @@ int32_t sim_run_build(uint64_t n, const uint8_t *keys, const uint64_t *key_off, 
     if (const int32_t rc = build_index(r, nb)) return rc;
     if (r.info.max_block_size != sum.max_blk) { fprintf(stderr, "sim_run_build: largest block %u, the index saw %u\n", sum.max_blk, r.info.max_block_size); return PGS_CORRUPTION; }
     return PGS_OK;
+}
+} // namespace
+
+extern "C" {
+
+// n flat records built into a run through build_plan / build_buffers / build_launch_plan / build_launch_blocks as pgs_run_build
+// runs them, then indexed by the upload's two passes.  grid_cap: at most this many CTAs per launch (0: the product's grids).
+// Returns pgs_run_build's status; on PGS_OK the run stays in a static buffer until the next call (sim_run_build_* read it).
+int32_t sim_run_build(uint64_t n, const uint8_t *keys, const uint64_t *key_off, const uint8_t *vals, const uint64_t *val_off,
+                      const uint64_t *seq, const uint8_t *type, uint32_t block_size, uint32_t restart_interval, uint32_t grid_cap)
+{
+    g_built = Built{};
+    if (n == 0) return PGS_OK;
+    if (n > kBuildMaxRecords) return PGS_NOT_SUPPORTED;
+    HostMem scratch;
+    BuildParams P{};
+    build_plan(P, (uint32_t)n, block_size, restart_interval);
+    uint8_t *k, *v, *t;
+    unsigned long long *ko, *vo, *sq;
+    memcpy(host_alloc(scratch, k, key_off[n] + 16, 0), keys, key_off[n]); // the library's slack
+    memcpy(host_alloc(scratch, v, val_off[n] + 16, 0), vals, val_off[n]);
+    memcpy(host_alloc(scratch, ko, n + 1, 0), key_off, 8 * (n + 1));
+    memcpy(host_alloc(scratch, vo, n + 1, 0), val_off, 8 * (n + 1));
+    memcpy(host_alloc(scratch, sq, n, 0), seq, 8 * n);
+    memcpy(host_alloc(scratch, t, n, 0), type, n);
+    P.keys = k; P.vals = v; P.type = t; P.key_off = ko; P.val_off = vo; P.seq = sq;
+    return build_sorted(P, scratch, grid_cap);
+}
+
+// n flat records in any order sorted through sort_plan / sort_buffers / sort_launch as pgs_run_build_unsorted runs them, then
+// built from the sorted copy as sim_run_build builds.  Returns pgs_run_build_unsorted's status; on PGS_OK the run is read with
+// sim_run_build_info / sim_run_build_copy.  *launches_out (if not null): the sort's launches.
+int32_t sim_run_build_unsorted(uint64_t n, const uint8_t *keys, const uint64_t *key_off, const uint8_t *vals, const uint64_t *val_off,
+                               const uint64_t *seq, const uint8_t *type, uint32_t block_size, uint32_t restart_interval,
+                               uint32_t grid_cap, uint32_t *launches_out)
+{
+    g_built = Built{};
+    if (launches_out) *launches_out = 0;
+    if (n == 0) return PGS_OK;
+    if (n > kBuildMaxRecords) return sort_status_too_many(n, key_off, val_off);
+    HostMem scratch;
+    SortParams Q{};
+    sort_plan(Q, (uint32_t)n);
+    uint8_t *k, *v, *t;
+    unsigned long long *ko, *vo, *sq;
+    memcpy(host_alloc(scratch, k, key_off[n] + 16, 0), keys, key_off[n]); // the library's slack
+    memcpy(host_alloc(scratch, v, val_off[n] + 16, 0), vals, val_off[n]);
+    memcpy(host_alloc(scratch, ko, n + 1, 0), key_off, 8 * (n + 1));
+    memcpy(host_alloc(scratch, vo, n + 1, 0), val_off, 8 * (n + 1));
+    memcpy(host_alloc(scratch, sq, n, 0), seq, 8 * n);
+    memcpy(host_alloc(scratch, t, n, 0), type, n);
+    Q.keys = k; Q.vals = v; Q.type = t; Q.key_off = ko; Q.val_off = vo; Q.seq = sq;
+    auto alloc = [&](auto *&p, uint64_t cnt, int fill) { host_alloc(scratch, p, cnt, fill == kNoFill ? 0xEE : fill); };
+    sort_buffers(Q, key_off[n], val_off[n], alloc, alloc);
+    uint32_t launches = 0;
+    const int32_t rc = sort_launch(Q, grid_cap, nullptr, [&](SortSummary &s) { s = *Q.sum; return (int32_t)PGS_OK; }, launches);
+    if (launches_out) *launches_out = launches;
+    if (rc) return rc;
+    BuildParams P{};
+    build_plan(P, (uint32_t)n, block_size, restart_interval);
+    P.keys = Q.s_keys; P.vals = Q.s_vals; P.type = Q.s_type; P.key_off = Q.s_key_off; P.val_off = Q.s_val_off; P.seq = Q.s_seq;
+    return build_sorted(P, scratch, grid_cap);
 }
 // the last sim_run_build's sizes and info (level and run id zero)
 void sim_run_build_info(uint64_t *data_bytes, uint32_t *n_blocks, pgs_run_info *info)
