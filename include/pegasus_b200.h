@@ -365,6 +365,9 @@ typedef struct {
     uint64_t arena_used;
 } pgs_scan_result;
 
+/* One scan; arena_cap is also its slice on the device, rounded up to 16 bytes.  pgs_kv's offsets are 32-bit, so a slice
+ * holds at most 4 GiB - 16 bytes, whatever arena_cap says: an output that passes its slice or kv_cap records gets
+ * PGS_ABORTED (retry with more room); an output that fits the slice but not arena_cap gets PGS_INCOMPLETE. */
 PGS_API int32_t pgs_range_scan(pgs_partition *p, const pgs_scan_request *req, uint32_t now,
                                uint8_t *arena, uint64_t arena_cap, pgs_kv *kvs, uint32_t kv_cap,
                                uint8_t *resume_key, uint32_t resume_cap, pgs_scan_result *out);
@@ -373,14 +376,21 @@ PGS_API int32_t pgs_range_scan(pgs_partition *p, const pgs_scan_request *req, ui
  * thread pools submits).  Request i may use up to arena_stride bytes / kv_stride records on the
  * device; the outputs come back packed: request i's records are kvs[kv_base[i] .. kv_base[i+1]),
  * their offsets are relative to arena + arena_base[i] (arena_base / kv_base have n+1 entries),
- * its resume key (if iter_valid) is resume_keys + i*resume_stride. */
+ * its resume key (if iter_valid) is resume_keys + i*resume_stride.  For n > 1, arena_base[i+1] -
+ * arena_base[i] is request i's arena_used rounded up to 16 (the padding bytes are unspecified);
+ * for n == 1 it is arena_used.  kv_base is the exclusive prefix of n_kvs.  The device slice is
+ * arena_stride rounded up to 16 and at most 4 GiB - 16 bytes (pgs_kv's offsets are 32-bit): an
+ * output that passes it or kv_stride records gets PGS_ABORTED.  arena_cap must cover
+ * arena_base[n] and kv_cap kv_base[n], or the call returns PGS_INCOMPLETE and leaves arena, kvs,
+ * arena_base and kv_base unwritten. */
 PGS_API int32_t pgs_range_scan_many(pgs_partition *p, const pgs_scan_request *reqs, uint32_t n,
                                     uint32_t now, uint64_t arena_stride, uint32_t kv_stride,
                                     uint8_t *arena, uint64_t arena_cap, pgs_kv *kvs, uint64_t kv_cap,
                                     uint8_t *resume_keys, uint32_t resume_stride,
                                     pgs_scan_result *results, uint64_t *arena_base, uint32_t *kv_base);
 /* The same for FORWARD scans over several partitions of one engine in ONE launch (SURVEY 8 f3): request i merges the runs of
- * parts[req_part[i]] only.  A reverse request gets PGS_NOT_SUPPORTED (those go through pgs_range_scan_many). */
+ * parts[req_part[i]] only.  A reverse request gets PGS_NOT_SUPPORTED (those go through pgs_range_scan_many).  Slices,
+ * packing and statuses as for pgs_range_scan_many. */
 PGS_API int32_t pgs_range_scan_many_multi(pgs_partition *const *parts, uint32_t n_parts, const pgs_scan_request *reqs,
                                           const uint32_t *req_part, uint32_t n, uint32_t now, uint64_t arena_stride,
                                           uint32_t kv_stride, uint8_t *arena, uint64_t arena_cap, pgs_kv *kvs,

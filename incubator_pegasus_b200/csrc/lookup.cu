@@ -6,8 +6,9 @@
 //
 // A read is planned and launched by the functions next to its kernels, which the simulator (tools/simt) calls too, as a
 // compaction is: read_run_set (the partition slots' runs), get_plan / scan_plan (kernel and shared memory), get_buffers /
-// scan_buffers (every device buffer with its size and initial content) and read_launch.  This file adds what is the library's
-// own: the run snapshot, the occupancy cap, device scratch, events, the read-back and the hot-key capture.
+// scan_buffers (every device buffer with its size and initial content) and read_launch, and a scan batch's packed read-back by
+// pack_offsets_launch / pack_copy_launch.  This file adds what is the library's own: the run snapshot, the occupancy cap, device
+// scratch, events, the copies back to the host and the hot-key capture.
 #include <algorithm>
 #include <cstring>
 
@@ -17,43 +18,6 @@
 #include "scan_kernel.cuh"
 
 namespace pgs {
-
-// pack the per-request output slices densely so that one D2H copy brings a whole batch back
-__global__ void k_pack_offsets(const pgs_scan_result *__restrict__ res, uint32_t n, unsigned long long *__restrict__ abase,
-                               uint32_t *__restrict__ kbase)
-{
-    __shared__ uint32_t scratch[33];
-    __shared__ unsigned long long carry_a;
-    __shared__ uint32_t carry_k;
-    if (threadIdx.x == 0) { carry_a = 0; carry_k = 0; }
-    __syncthreads();
-    for (uint32_t base = 0; base < n; base += blockDim.x) {
-        uint32_t i = base + threadIdx.x;
-        uint32_t a = i < n ? (uint32_t)((res[i].arena_used + 15) & ~15ull) : 0;
-        uint32_t k = i < n ? res[i].n_kvs : 0;
-        uint32_t ta, tk;
-        uint32_t pa = block_excl_scan(a, scratch, &ta);
-        uint32_t pk = block_excl_scan(k, scratch, &tk);
-        if (i < n) { abase[i] = carry_a + pa; kbase[i] = carry_k + pk; }
-        __syncthreads();
-        if (threadIdx.x == 0) { carry_a += ta; carry_k += tk; }
-        __syncthreads();
-    }
-    if (threadIdx.x == 0) { abase[n] = carry_a; kbase[n] = carry_k; }
-}
-__global__ void k_pack_copy(const pgs_scan_result *__restrict__ res, uint32_t n, const uint8_t *__restrict__ arena,
-                            unsigned long long arena_stride, const pgs_kv *__restrict__ kvs, uint32_t kv_stride,
-                            const unsigned long long *__restrict__ abase, const uint32_t *__restrict__ kbase,
-                            uint8_t *__restrict__ parena, pgs_kv *__restrict__ pkvs)
-{
-    for (uint32_t i = blockIdx.x; i < n; i += gridDim.x) {
-        uint32_t chunks = (uint32_t)((res[i].arena_used + 15) >> 4);
-        const uint4 *src = (const uint4 *)(arena + (size_t)i * arena_stride);
-        uint4 *dst = (uint4 *)(parena + abase[i]);
-        for (uint32_t c = threadIdx.x; c < chunks; c += blockDim.x) dst[c] = src[c];
-        for (uint32_t k = threadIdx.x; k < res[i].n_kvs; k += blockDim.x) pkvs[kbase[i] + k] = kvs[(size_t)i * kv_stride + k];
-    }
-}
 
 void set_last_read_stats(float ms, uint64_t probed, uint64_t skipped);
 
@@ -193,30 +157,24 @@ int32_t scan_many(pgs_partition *const *parts, uint32_t n_parts, const uint32_t 
         if (out.arena_base) { out.arena_base[0] = 0; out.arena_base[1] = results[0].arena_used; }
         if (out.kv_base) { out.kv_base[0] = 0; out.kv_base[1] = results[0].n_kvs; }
     } else {
-        unsigned long long *d_abase = nullptr;
-        uint32_t *d_kbase = nullptr;
-        PGS_CUDA(S.alloc(d_abase, sizeof(unsigned long long) * (n + 1)));
-        PGS_CUDA(S.alloc(d_kbase, sizeof(uint32_t) * (n + 1)));
-        k_pack_offsets<<<1, 1024, 0, st>>>(P.results, n, d_abase, d_kbase);
+        ScanPack K;
+        pack_offsets_launch(P, K, st, device_buffers(S, ce));
+        PGS_CUDA(ce);
         std::vector<unsigned long long> ab(n + 1);
         std::vector<uint32_t> kb(n + 1);
-        PGS_CUDA(cudaMemcpyAsync(ab.data(), d_abase, sizeof(unsigned long long) * (n + 1), cudaMemcpyDeviceToHost, st));
-        PGS_CUDA(cudaMemcpyAsync(kb.data(), d_kbase, sizeof(uint32_t) * (n + 1), cudaMemcpyDeviceToHost, st));
+        PGS_CUDA(cudaMemcpyAsync(ab.data(), K.arena_base, sizeof(unsigned long long) * (n + 1), cudaMemcpyDeviceToHost, st));
+        PGS_CUDA(cudaMemcpyAsync(kb.data(), K.kv_base, sizeof(uint32_t) * (n + 1), cudaMemcpyDeviceToHost, st));
         PGS_CUDA(cudaMemcpyAsync(results, P.results, sizeof(pgs_scan_result) * n, cudaMemcpyDeviceToHost, st));
         PGS_CUDA(cudaMemcpyAsync(&herr, P.error, 4, cudaMemcpyDeviceToHost, st));
         PGS_CUDA(cudaStreamSynchronize(st));
         e->launches++;
         if (!herr) {
             if (ab[n] > out.arena_cap || kb[n] > out.kv_cap) { set_error("scan_many: output arena too small"); return PGS_INCOMPLETE; }
-            uint8_t *d_parena = nullptr;
-            pgs_kv *d_pkvs = nullptr;
-            PGS_CUDA(S.alloc(d_parena, ab[n] + 16));
-            PGS_CUDA(S.alloc(d_pkvs, sizeof(pgs_kv) * ((size_t)kb[n] + 1)));
-            k_pack_copy<<<std::min<uint32_t>(n, 8 * e->sm_count), 128, 0, st>>>(P.results, n, P.arena, P.arena_stride, P.kvs, P.kv_stride, d_abase,
-                                                                              d_kbase, d_parena, d_pkvs);
+            pack_copy_launch(P, K, ab[n], kb[n], 8 * e->sm_count, st, device_buffers(S, ce));
+            PGS_CUDA(ce);
             e->launches++;
-            if (ab[n]) PGS_CUDA(cudaMemcpyAsync(out.arena, d_parena, ab[n], cudaMemcpyDeviceToHost, st));
-            if (kb[n]) PGS_CUDA(cudaMemcpyAsync(out.kvs, d_pkvs, sizeof(pgs_kv) * kb[n], cudaMemcpyDeviceToHost, st));
+            if (ab[n]) PGS_CUDA(cudaMemcpyAsync(out.arena, K.arena, ab[n], cudaMemcpyDeviceToHost, st));
+            if (kb[n]) PGS_CUDA(cudaMemcpyAsync(out.kvs, K.kvs, sizeof(pgs_kv) * kb[n], cudaMemcpyDeviceToHost, st));
             if (out.resume && resume_stride) PGS_CUDA(cudaMemcpyAsync(out.resume, P.resume, (size_t)P.resume_stride * n, cudaMemcpyDeviceToHost, st));
             PGS_CUDA(cudaStreamSynchronize(st));
         }

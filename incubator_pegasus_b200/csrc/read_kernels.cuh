@@ -14,6 +14,8 @@
 //               sort-key filters) record by record, exactly in the reference's order.  The 32/G groups of a warp run in lock
 //               step on different requests; entries are read straight from HBM, records are copied to the output arena.
 //   (reverse scans keep the block-staging kernel k_scan of lookup.cu.)
+//   k_pack_offsets / k_pack_copy  the packed read-back of a scan batch of either kernel: one CTA places every request's
+//               output, then one CTA per request copies it to its place.
 #pragma once
 #include <algorithm>
 #include <cstring>
@@ -576,13 +578,16 @@ inline ScanBatch flatten_scan_requests(const pgs_scan_request *reqs, uint32_t n)
 }
 
 // the per-request output slices of a scan launch (P.KS set): kv_stride records, an arena slice of arena_stride bytes rounded
-// up to 16, and a resume-key slot of resume_stride bytes.  A slot shorter than the launch's key slot cannot hold every resume
-// key: then the kernels write them to slots of KS bytes and none is reported (returns false).
+// up to 16, and a resume-key slot of resume_stride bytes.  pgs_kv's offsets are 32-bit, so a slice holds at most 4 GiB - 16
+// bytes: an output that passes that ends as any output that passes its slice, with PGS_ABORTED.  A slot shorter than the
+// launch's key slot cannot hold every resume key: then the kernels write them to slots of KS bytes and none is reported
+// (returns false).
+constexpr unsigned long long kMaxScanSlice = (1ull << 32) - 16;
 inline bool scan_output_strides(ScanParams &P, unsigned long long arena_stride, uint32_t kv_stride, uint32_t resume_stride)
 {
     const bool report_resume = resume_stride >= P.KS;
     P.kv_stride = kv_stride;
-    P.arena_stride = (arena_stride + 15) & ~15ull;
+    P.arena_stride = std::min((arena_stride + 15) & ~15ull, kMaxScanSlice);
     P.resume_stride = report_resume ? resume_stride : P.KS;
     return report_resume;
 }
@@ -768,6 +773,67 @@ inline bool scan_buffers(ScanParams &P, const ReadRunSet &R, const ScanBatch &B,
     P.ticket = P.error + 1;
     multi_buffers(R, P.multi_runs, P.multi_begin, P.req_part, req_part, n, buf);
     return report_resume;
+}
+
+// ---- the packed read-back of a scan batch of n > 1 requests (the library and the simulator) -------------------------------------
+// k_pack_offsets places request i's output at arena_base[i] of one packed arena, with arena_base[i + 1] - arena_base[i] = its
+// arena_used rounded up to 16, and its kvs at kv_base[i], the exclusive prefix of n_kvs.  The caller reads the totals
+// arena_base[n] and kv_base[n]; when they fit its arena and kv array, k_pack_copy copies every slice to its place, so that one copy
+// each brings the whole batch back.  The bytes between a request's output and the next 16-byte boundary are left unspecified.
+__global__ void __launch_bounds__(1024) k_pack_offsets(const pgs_scan_result *__restrict__ res, uint32_t n, unsigned long long *__restrict__ abase,
+                                                      uint32_t *__restrict__ kbase)
+{
+    auto add = [&](uint32_t i, unsigned long long (&v)[2]) { v[0] += (res[i].arena_used + 15) & ~15ull; v[1] += res[i].n_kvs; };
+    uint32_t q0, q1;
+    unsigned long long pre[2], tot[2];
+    cta_excl_scan<2>(n, add, q0, q1, pre, tot);
+    for (uint32_t i = q0; i < q1; i++) {
+        abase[i] = pre[0];
+        kbase[i] = (uint32_t)pre[1];
+        add(i, pre);
+    }
+    if (threadIdx.x == 0) { abase[n] = tot[0]; kbase[n] = (uint32_t)tot[1]; }
+}
+__global__ void k_pack_copy(const pgs_scan_result *__restrict__ res, uint32_t n, const uint8_t *__restrict__ arena,
+                            unsigned long long arena_stride, const pgs_kv *__restrict__ kvs, uint32_t kv_stride,
+                            const unsigned long long *__restrict__ abase, const uint32_t *__restrict__ kbase,
+                            uint8_t *__restrict__ parena, pgs_kv *__restrict__ pkvs)
+{
+    for (uint32_t i = blockIdx.x; i < n; i += gridDim.x) {
+        uint32_t chunks = (uint32_t)((res[i].arena_used + 15) >> 4);
+        const uint4 *src = (const uint4 *)(arena + (size_t)i * arena_stride);
+        uint4 *dst = (uint4 *)(parena + abase[i]);
+        for (uint32_t c = threadIdx.x; c < chunks; c += blockDim.x) dst[c] = src[c];
+        for (uint32_t k = threadIdx.x; k < res[i].n_kvs; k += blockDim.x) pkvs[kbase[i] + k] = kvs[(size_t)i * kv_stride + k];
+    }
+}
+
+// the buffers of a packed read-back, each allocated by the launch that writes it
+struct ScanPack {
+    unsigned long long *arena_base = nullptr; // n + 1 entries
+    uint32_t *kv_base = nullptr;              // n + 1 entries
+    uint8_t *arena = nullptr;                 // arena_base[n] bytes + 16 of slack
+    pgs_kv *kvs = nullptr;                    // kv_base[n] + 1 records
+};
+// the offsets of the launched batch P, on one CTA; buf as for scan_buffers
+template <class F>
+inline void pack_offsets_launch(const ScanParams &P, ScanPack &K, cudaStream_t st, F &&buf)
+{
+    buf(K.arena_base, sizeof(unsigned long long) * (P.n + 1ull), ReadInit{});
+    buf(K.kv_base, sizeof(uint32_t) * (P.n + 1ull), ReadInit{});
+    if (!K.arena_base || !K.kv_base) return; // an allocation failed: the caller reports its allocator's status
+    PGS_LAUNCH(k_pack_offsets, 1, 1024, 0, st, (const pgs_scan_result *)P.results, P.n, K.arena_base, K.kv_base);
+}
+// the packed arena and kvs of P (arena_bytes = arena_base[n], n_kvs = kv_base[n]), one request per CTA on at most max_ctas CTAs
+template <class F>
+inline void pack_copy_launch(const ScanParams &P, ScanPack &K, uint64_t arena_bytes, uint64_t n_kvs, uint32_t max_ctas, cudaStream_t st, F &&buf)
+{
+    buf(K.arena, arena_bytes + 16, ReadInit{});
+    buf(K.kvs, sizeof(pgs_kv) * (n_kvs + 1), ReadInit{});
+    if (!K.arena || !K.kvs) return;
+    PGS_LAUNCH(k_pack_copy, std::min(P.n, max_ctas), 128, 0, st, (const pgs_scan_result *)P.results, P.n,
+               (const uint8_t *)P.arena, P.arena_stride, (const pgs_kv *)P.kvs, P.kv_stride, (const unsigned long long *)K.arena_base,
+               (const uint32_t *)K.kv_base, K.arena, K.kvs);
 }
 
 } // namespace pgs

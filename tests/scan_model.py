@@ -263,3 +263,58 @@ def answer(r, arena, kvs, resume):
 
 def diff(got, want):
     return {k: (got[k], want[k]) for k in want if got[k] != want[k]}
+
+
+# ---- the packed read-back of a batch (pgs_range_scan / pgs_range_scan_many[_multi]) ---------------------------------------------
+SLICE_MAX = 2**32 - 16  # pgs_kv's offsets are 32-bit: the most one request's slice holds
+
+
+def round16(x):
+    return (x + 15) & ~15
+
+
+def slice_bytes(arena_stride):
+    """the arena slice each request of a batch writes into"""
+    return min(round16(arena_stride), SLICE_MAX)
+
+
+def pack_offsets(used, n_kvs):
+    """k_pack_offsets: request i's output at arena_base[i], each one rounded up to 16 bytes, and its kvs at kv_base[i]"""
+    ab, kb = [0], [0]
+    for u, k in zip(used, n_kvs):
+        ab.append(ab[-1] + round16(u))
+        kb.append(kb[-1] + k)
+    return ab, kb
+
+
+def model_batch(answers, arena_stride, kv_stride, arena_cap, kv_cap):
+    """the status and (arena_base, kv_base) of a batch whose requests answer `answers` (model_scan dicts).  PGS_ABORTED when an
+    output passes its slice or kv_stride records; else PGS_INCOMPLETE when the packed batch passes arena_cap or kv_cap; else
+    PGS_OK.  A batch of one request is read back unpadded."""
+    used = [sum(len(k) + len(v) for k, v, _ in a["kvs"]) for a in answers]
+    n_kvs = [len(a["kvs"]) for a in answers]
+    if any(u > slice_bytes(arena_stride) or k > kv_stride for u, k in zip(used, n_kvs)):
+        return "ABORTED", None, None
+    ab, kb = ([0, used[0]], [0, n_kvs[0]]) if len(answers) == 1 else pack_offsets(used, n_kvs)
+    if ab[-1] > arena_cap or kb[-1] > kv_cap:
+        return "INCOMPLETE", None, None
+    return "OK", ab, kb
+
+
+def check_packed(results, arena, kvs, ab, kb, answers, want_ab, want_kb):
+    """a packed read-back against the model: the bases, every result's sizes, every kv's offsets, and the output bytes
+    [ab[i], ab[i] + arena_used[i]) of every request (never the padding after them)"""
+    assert [int(x) for x in ab] == want_ab and [int(x) for x in kb] == want_kb
+    outs = {}  # a batch repeats its requests: each answer's bytes joined once
+    for i, a in enumerate(answers):
+        r, base = results[i], int(ab[i])
+        out = outs.get(id(a))
+        if out is None:
+            out = outs[id(a)] = b"".join(k + v for k, v, _ in a["kvs"])
+        assert (r.arena_used, r.n_kvs) == (len(out), len(a["kvs"])), i
+        assert arena[base:base + len(out)].tobytes() == out, i
+        off = 0
+        for j, (k, v, ets) in enumerate(a["kvs"]):
+            kv = kvs[int(kb[i]) + j]
+            assert (kv.key_off, kv.key_len, kv.value_off, kv.value_len, kv.expire_ts) == (off, len(k), off + len(k), len(v), ets), (i, j)
+            off += len(k) + len(v)

@@ -350,11 +350,11 @@ int32_t sim_get(uint32_t k, const uint8_t **data, const uint64_t *data_bytes, co
 // lanes per group; lanes & 0x100: the multi-partition shape of pgs_range_scan_many_multi (read_slots; request i belongs to
 // slot i % 3).  pool_bytes (k_scan only): 0 = the pool the product gives a batch of n requests; otherwise at most pool_bytes,
 // but never below the smallest pool (scan_min_pool: one block of every run), so that a small value forces chunks of about
-// one block.
-int32_t sim_scan(uint32_t k, const uint8_t **data, const uint64_t *data_bytes, const uint64_t **blk_off, const uint32_t **blk_size,
+// one block.  arena_base not null: the packed read-back of sim_scan_packed.
+static int32_t scan_read_back(uint32_t k, const uint8_t **data, const uint64_t *data_bytes, const uint64_t **blk_off, const uint32_t **blk_size,
                  const uint32_t *n_blocks, const pgs_scan_request *reqs, uint32_t n, uint32_t now, uint64_t arena_stride, uint32_t kv_stride,
                  uint8_t *arena, pgs_kv *kvs, uint8_t *resume, uint32_t resume_stride, pgs_scan_result *results, uint32_t lanes,
-                 uint32_t pool_bytes)
+                 uint32_t pool_bytes, uint64_t *arena_base, uint32_t *kv_base, uint64_t arena_cap, uint64_t kv_cap)
 {
     std::vector<HostRun> runs;
     if (const int32_t rc = load_runs(k, data, data_bytes, blk_off, blk_size, n_blocks, runs)) return rc;
@@ -371,14 +371,71 @@ int32_t sim_scan(uint32_t k, const uint8_t **data, const uint64_t *data_bytes, c
     const bool report_resume = scan_buffers(P, R, B, slot_of_each(n).data(), arena_stride, kv_stride, resume_stride, host_buffers(mem));
     read_launch(L, P, L.kernel == k_scan ? 3 : 2, nullptr);
     memcpy(results, P.results, sizeof(pgs_scan_result) * n);
+    ScanPack K;
+    std::vector<unsigned long long> ab{0, n ? results[0].arena_used : 0};
+    std::vector<uint32_t> kb{0, n ? results[0].n_kvs : 0};
+    if (arena_base && n > 1) {
+        pack_offsets_launch(P, K, nullptr, host_buffers(mem));
+        ab.assign(K.arena_base, K.arena_base + n + 1);
+        kb.assign(K.kv_base, K.kv_base + n + 1);
+    }
     if (P.error[0]) return (int32_t)P.error[0];
+    if (arena_base && n) {
+        if (ab[n] > arena_cap || kb[n] > kv_cap) return PGS_INCOMPLETE;
+        if (n > 1) {
+            pack_copy_launch(P, K, ab[n], kb[n], 2, nullptr, host_buffers(mem));
+            memcpy(arena, K.arena, ab[n]);
+            memcpy(kvs, K.kvs, sizeof(pgs_kv) * kb[n]);
+        } else {
+            memcpy(arena, P.arena, ab[1]);
+            memcpy(kvs, P.kvs, sizeof(pgs_kv) * kb[1]);
+        }
+        memcpy(arena_base, ab.data(), 8 * (n + 1ull));
+        memcpy(kv_base, kb.data(), 4 * (n + 1ull));
+    }
     for (uint64_t i = 0; i < n; i++) {
         const pgs_scan_result &r = results[i];
-        memcpy(arena + i * P.arena_stride, P.arena + i * P.arena_stride, r.arena_used);
-        memcpy(kvs + i * kv_stride, P.kvs + i * kv_stride, sizeof(pgs_kv) * r.n_kvs);
+        if (!arena_base) {
+            memcpy(arena + i * P.arena_stride, P.arena + i * P.arena_stride, r.arena_used);
+            memcpy(kvs + i * kv_stride, P.kvs + i * kv_stride, sizeof(pgs_kv) * r.n_kvs);
+        }
         if (report_resume && r.iter_valid) memcpy(resume + i * resume_stride, P.resume + i * P.resume_stride, r.resume_len);
     }
     return PGS_OK;
+}
+
+int32_t sim_scan(uint32_t k, const uint8_t **data, const uint64_t *data_bytes, const uint64_t **blk_off, const uint32_t **blk_size,
+                 const uint32_t *n_blocks, const pgs_scan_request *reqs, uint32_t n, uint32_t now, uint64_t arena_stride, uint32_t kv_stride,
+                 uint8_t *arena, pgs_kv *kvs, uint8_t *resume, uint32_t resume_stride, pgs_scan_result *results, uint32_t lanes,
+                 uint32_t pool_bytes)
+{
+    return scan_read_back(k, data, data_bytes, blk_off, blk_size, n_blocks, reqs, n, now, arena_stride, kv_stride, arena, kvs, resume,
+                          resume_stride, results, lanes, pool_bytes, nullptr, nullptr, 0, 0);
+}
+
+// sim_scan with the batch read back as scan_many reads it: request i's kvs at kvs[kv_base[i] ..) with offsets relative to
+// arena + arena_base[i] (pack_offsets_launch / pack_copy_launch for n > 1, the slice itself for n == 1), and PGS_INCOMPLETE,
+// with arena_base / kv_base unset, when arena_base[n] > arena_cap or kv_base[n] > kv_cap.  Resume keys as sim_scan.
+int32_t sim_scan_packed(uint32_t k, const uint8_t **data, const uint64_t *data_bytes, const uint64_t **blk_off, const uint32_t **blk_size,
+                        const uint32_t *n_blocks, const pgs_scan_request *reqs, uint32_t n, uint32_t now, uint64_t arena_stride,
+                        uint32_t kv_stride, uint8_t *arena, uint64_t arena_cap, pgs_kv *kvs, uint64_t kv_cap, uint8_t *resume,
+                        uint32_t resume_stride, pgs_scan_result *results, uint64_t *arena_base, uint32_t *kv_base, uint32_t lanes)
+{
+    return scan_read_back(k, data, data_bytes, blk_off, blk_size, n_blocks, reqs, n, now, arena_stride, kv_stride, arena, kvs, resume,
+                          resume_stride, results, lanes, 0, arena_base, kv_base, arena_cap, kv_cap);
+}
+
+// k_pack_offsets alone (pack_offsets_launch) over n results the caller makes up: arena_base / kv_base get its n + 1 offsets
+void sim_pack_offsets(const pgs_scan_result *results, uint32_t n, uint64_t *arena_base, uint32_t *kv_base)
+{
+    HostMem mem;
+    ScanParams P{};
+    P.n = n;
+    memcpy(host_alloc(mem, P.results, n, 0), results, sizeof(pgs_scan_result) * n);
+    ScanPack K;
+    pack_offsets_launch(P, K, nullptr, host_buffers(mem));
+    memcpy(arena_base, K.arena_base, 8 * (n + 1ull));
+    memcpy(kv_base, K.kv_base, 4 * (n + 1ull));
 }
 
 // k_hotkey_capture over n keys of n_slots partition slots (key_part null: every key is slot 0).  Per slot: state (0 off,
