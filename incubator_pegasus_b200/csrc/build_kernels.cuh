@@ -30,7 +30,7 @@ constexpr uint32_t kBuildThreads = 256;
 constexpr uint32_t kBuildTile = kBuildThreads * 16;    // records per CTA of the scan
 constexpr uint32_t kBuildScanThreads = 1024;          // the one CTA that scans the tiles
 constexpr uint32_t kBuildWarps = 8;                   // warps (= blocks in flight) per CTA of k_build_blocks
-constexpr uint64_t kBuildMaxRecords = 0xFFFFFFF0ull;  // index_layout's limit on the records of a run
+constexpr uint64_t kBuildMaxRecords = 0xFFFFFFF0ull;  // index_buffers' limit on the records of a run
 constexpr uint32_t kBuildBlockTooLarge = 0xFFFFFFFFu; // k_build_next: a block past 32 bits
 
 // BuildSummary::flags
@@ -64,8 +64,6 @@ struct BuildParams {
     // output (after the summary): the run's block bytes
     uint8_t *data;
 };
-
-PGS_HD uint64_t build_pad(uint64_t v) { return (v + kBlockAlign - 1) & ~(uint64_t)(kBlockAlign - 1); }
 
 // byte p of record i's internal key: user key || fixed64_le(seq << 8 | type)
 PGS_DEV uint32_t ikey_byte(const uint8_t *uk, uint64_t ulen, unsigned long long tr, uint64_t p)
@@ -154,7 +152,7 @@ __global__ void __launch_bounds__(kBuildThreads) k_build_mark(const uint32_t *__
 // the (start, padded bytes) of record i, added into v
 PGS_DEV void build_start_add(const BuildParams &P, uint32_t i, unsigned long long (&v)[2])
 {
-    if (P.mark[i]) { v[0] += 1; v[1] += build_pad(P.bsize[i]); }
+    if (P.mark[i]) { v[0] += 1; v[1] += block_pad(P.bsize[i]); }
 }
 
 __global__ void __launch_bounds__(kBuildThreads) k_build_tile_sums(const BuildParams P)
@@ -209,7 +207,7 @@ __global__ void __launch_bounds__(kBuildThreads) k_build_place(const BuildParams
         if (size == kBuildBlockTooLarge) flags = kBuildHugeBlock;
         max_blk = max(max_blk, size);
         pre[0] += 1;
-        pre[1] += build_pad(size);
+        pre[1] += block_pad(size);
     }
     if (max_blk) atomicMax(&P.sum->max_blk, max_blk);
     if (flags) atomicOr(&P.sum->flags, flags);
@@ -260,7 +258,7 @@ __global__ void __launch_bounds__(kBuildWarps * 32) k_build_blocks(const BuildPa
             carry += __shfl_sync(kFull, incl, 31);
         }
         if (lane == 0) { uint8_t *r = base + size - 4; r[0] = (uint8_t)nrst; r[1] = (uint8_t)(nrst >> 8); r[2] = (uint8_t)(nrst >> 16); r[3] = (uint8_t)(nrst >> 24); }
-        for (uint32_t p = size + lane; p < build_pad(size); p += 32) base[p] = 0;
+        for (uint32_t p = size + lane; p < block_pad(size); p += 32) base[p] = 0;
     }
 }
 
@@ -274,6 +272,19 @@ inline void build_plan(BuildParams &P, uint32_t n, uint32_t block_size, uint32_t
     P.levels = 1;
     while ((1ull << P.levels) < n) P.levels++;
     P.tiles = (n + kBuildTile - 1) / kBuildTile;
+}
+// The caller's n flat records as the inputs of P (BuildParams or SortParams), through buf(pointer, bytes, init) as get_buffers
+// uses it.  The keys and the values keep 16 bytes of slack behind them.
+template <class Params, class F>
+void stage_records(Params &P, uint64_t n, const uint8_t *keys, const uint64_t *key_off, const uint8_t *vals, const uint64_t *val_off,
+                   const uint64_t *seq, const uint8_t *type, F &&buf)
+{
+    buf(P.keys, key_off[n] + 16, ReadInit{keys, key_off[n]});
+    buf(P.vals, val_off[n] + 16, ReadInit{vals, val_off[n]});
+    buf(P.key_off, 8 * (n + 1), ReadInit{key_off, 8 * (n + 1)});
+    buf(P.val_off, 8 * (n + 1), ReadInit{val_off, 8 * (n + 1)});
+    buf(P.seq, 8 * n, ReadInit{seq, 8 * n});
+    buf(P.type, n, ReadInit{type, n});
 }
 // The scratch of the first phase: alloc(p, count, fill) with fill = a byte value or kNoFill.  4·R + 25 bytes per record
 // (R = ceil(log2 n) levels of next), plus the tiles.

@@ -204,12 +204,7 @@ int32_t split_run(Engine *e, const Run &in, const SplitParams &proto, std::vecto
 
     LaunchScratch S(st);
     cudaError_t ce = cudaSuccess;
-    split_buffers(SP, [&](auto *&p, uint64_t n, int fill, bool) {
-        const size_t bytes = sizeof(*p) * n;
-        if (ce != cudaSuccess) return;
-        ce = S.alloc(p, bytes ? bytes : 16);
-        if (ce == cudaSuccess && fill != kNoFill) ce = cudaMemsetAsync(p, fill, bytes, st);
-    });
+    split_buffers(SP, scratch_buffers(S, ce));
     PGS_CUDA(ce);
     std::vector<MergeStats> hs(NC, merge_stats_init());
     PGS_CUDA(cudaMemcpyAsync(SP.stats, hs.data(), sizeof(MergeStats) * NC, cudaMemcpyHostToDevice, st));

@@ -24,6 +24,14 @@ namespace pgs {
 constexpr uint32_t kWarp = 32;
 constexpr uint32_t kFull = 0xffffffffu;
 constexpr int kNoFill = -1; // a launch buffer the host leaves unset (compact_buffers, get_buffers, scan_buffers)
+// the initial content of a launch buffer: src_bytes copied from the host, or every byte set to fill, or none
+struct ReadInit {
+    const void *src = nullptr;
+    uint64_t src_bytes = 0;
+    int fill = kNoFill;
+};
+constexpr ReadInit kZero{nullptr, 0, 0};
+void set_error(const char *fmt, ...); // the message of a refused call (engine.cu; the simulator prints it)
 
 // ---- shared-memory addressing / mbarrier / TMA bulk (cp.async.bulk) ----------------------------
 #ifdef PGS_SIM

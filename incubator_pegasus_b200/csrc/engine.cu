@@ -188,24 +188,24 @@ constexpr uint64_t kUploadChunk = 32ull << 20;
 
 struct UploadJob {
     std::shared_ptr<Run> r;
-    Engine *eng = nullptr;
+    Engine *eng;
     // pinned staging (one allocation): off[nb+1] u64 | blk_size[nb] u32 | nrec[nb] | lastlen[nb] | rec_cum[nb+1] | key_cum[nb+1] | 2 x IndexStats
     void *pin = nullptr;
     size_t pin_cap = 0;
     uint64_t *off = nullptr;
     uint32_t *h_size = nullptr, *nrec = nullptr, *lastlen = nullptr, *rec_cum = nullptr, *key_cum = nullptr;
     IndexStats *hs_in = nullptr, *hs_out = nullptr;
-    uint32_t *d_nrec = nullptr, *d_lastlen = nullptr;
-    IndexStats *d_stats = nullptr;
-    IndexStats hs{};
+    IndexParams X{};
+    LaunchScratch S; // pass 1's device scratch
     std::vector<cudaEvent_t> events;
     cudaEvent_t pass1 = nullptr;
     uint32_t max_blk = 0;
+    explicit UploadJob(Engine *e) : eng(e), S(e->stream) {}
     ~UploadJob()
     {
         for (cudaEvent_t ev : events) cudaEventDestroy(ev);
         if (pass1) cudaEventDestroy(pass1);
-        if (pin && eng) eng->give_pinned(pin, pin_cap);
+        if (pin) eng->give_pinned(pin, pin_cap);
     }
 };
 
@@ -214,7 +214,6 @@ static int32_t upload_job_init(Engine *e, int32_t level, uint32_t nb, uint64_t e
 {
     auto r = std::make_shared<Run>(e);
     j.r = r;
-    j.eng = e;
     {
         const size_t need = 8ull * (nb + 2) + 4ull * (nb + 1) * 5 + 2 * sizeof(IndexStats) + 64;
         j.pin = e->take_pinned(need, &j.pin_cap);
@@ -237,30 +236,22 @@ static int32_t upload_job_init(Engine *e, int32_t level, uint32_t nb, uint64_t e
     PGS_CUDA(e->alloc_data(*r, end + 256));
     PGS_CUDA(cudaMallocAsync(&r->d_blk_off, sizeof(uint64_t) * (nb + 1), st));
     PGS_CUDA(cudaMallocAsync(&r->d_blk_size, sizeof(uint32_t) * nb, st));
-    PGS_CUDA(cudaMallocAsync(&j.d_nrec, sizeof(uint32_t) * nb, st));
-    PGS_CUDA(cudaMallocAsync(&j.d_lastlen, sizeof(uint32_t) * nb, st));
-    PGS_CUDA(cudaMallocAsync(&j.d_stats, sizeof(IndexStats), st));
-    *j.hs_in = IndexStats{};
-    j.hs_in->min_seq = ~0ull;
-    PGS_CUDA(cudaMemcpyAsync(j.d_stats, j.hs_in, sizeof(IndexStats), cudaMemcpyHostToDevice, st));
+    j.X = IndexParams{r->d_data, r->d_blk_off, r->d_blk_size, nb};
+    cudaError_t ce = cudaSuccess;
+    index_scratch(j.X, scratch_buffers(j.S, ce));
+    PGS_CUDA(ce);
+    *j.hs_in = index_stats_init();
+    PGS_CUDA(cudaMemcpyAsync(j.X.stats, j.hs_in, sizeof(IndexStats), cudaMemcpyHostToDevice, st));
     return PGS_OK;
-}
-// the first index pass over the blocks [b0, b1) once their bytes are on the device
-static void upload_pass1(Engine *e, UploadJob &j, uint32_t b0, uint32_t b1)
-{
-    Run *r = j.r.get();
-    k_index_walk<false><<<(b1 - b0 + kIdxWarps - 1) / kIdxWarps, kIdxWarps * 32, kIdxWarps * kIdxScratch, e->stream>>>(
-        r->d_data, r->d_blk_off, r->d_blk_size, b1, j.d_nrec, j.d_lastlen, nullptr, nullptr, nullptr, nullptr, nullptr, 0, j.d_stats, b0);
-    e->launches++;
 }
 // after the last first-pass launch: its per-block results come back, j.pass1 marks their arrival
 static int32_t upload_pass1_done(Engine *e, UploadJob &j)
 {
-    const uint32_t nb = j.r->info.n_blocks;
+    const uint32_t nb = j.X.nb;
     cudaStream_t st = e->stream;
-    PGS_CUDA(cudaMemcpyAsync(j.nrec, j.d_nrec, sizeof(uint32_t) * nb, cudaMemcpyDeviceToHost, st));
-    PGS_CUDA(cudaMemcpyAsync(j.lastlen, j.d_lastlen, sizeof(uint32_t) * nb, cudaMemcpyDeviceToHost, st));
-    PGS_CUDA(cudaMemcpyAsync(j.hs_out, j.d_stats, sizeof(IndexStats), cudaMemcpyDeviceToHost, st));
+    PGS_CUDA(cudaMemcpyAsync(j.nrec, j.X.nrec, sizeof(uint32_t) * nb, cudaMemcpyDeviceToHost, st));
+    PGS_CUDA(cudaMemcpyAsync(j.lastlen, j.X.lastlen, sizeof(uint32_t) * nb, cudaMemcpyDeviceToHost, st));
+    PGS_CUDA(cudaMemcpyAsync(j.hs_out, j.X.stats, sizeof(IndexStats), cudaMemcpyDeviceToHost, st));
     PGS_CUDA(cudaEventCreateWithFlags(&j.pass1, cudaEventDisableTiming));
     PGS_CUDA(cudaEventRecord(j.pass1, st));
     return PGS_OK;
@@ -274,7 +265,7 @@ static int32_t upload_stage_a(Engine *e, int32_t level, const uint8_t *data, uin
         set_error("run upload: bad block handle %u", b);
         return PGS_INVALID_ARGUMENT;
     }
-    const uint64_t end = (prev_end + kBlockAlign - 1) / kBlockAlign * kBlockAlign;
+    const uint64_t end = block_pad(prev_end);
     const uint64_t nbytes = data_bytes < end ? data_bytes : end;
     if (const int32_t rc = upload_job_init(e, level, nb, end, j)) return rc;
     Run *r = j.r.get();
@@ -301,7 +292,7 @@ static int32_t upload_stage_a(Engine *e, int32_t level, const uint8_t *data, uin
         j.events.push_back(ev);
         PGS_CUDA(cudaEventRecord(ev, cp));
         PGS_CUDA(cudaStreamWaitEvent(st, ev, 0));
-        upload_pass1(e, j, b0, b1);
+        e->launches += index_launch_pass1(j.X, b0, b1, st);
         b0 = b1;
     }
     return upload_pass1_done(e, j);
@@ -309,37 +300,20 @@ static int32_t upload_stage_a(Engine *e, int32_t level, const uint8_t *data, uin
 
 static int32_t upload_stage_b(Engine *e, UploadJob &j)
 {
-    Run *r = j.r.get();
-    const uint32_t nb = r->info.n_blocks;
+    const uint32_t nb = j.X.nb;
     cudaStream_t st = e->stream;
     PGS_CUDA(cudaEventSynchronize(j.pass1));
-    j.hs = *j.hs_out;
-    cudaFreeAsync(j.d_nrec, st);
-    cudaFreeAsync(j.d_lastlen, st);
-    j.d_nrec = j.d_lastlen = nullptr;
-    if (j.hs.error) {
-        set_error("run upload: block scan failed with status %u", j.hs.error);
-        return (int32_t)j.hs.error;
-    }
-    if (!index_layout(j.nrec, j.lastlen, nb, j.rec_cum, j.key_cum)) {
-        set_error("run too large for 32-bit record / index-key offsets");
-        return PGS_NOT_SUPPORTED;
-    }
-    const uint32_t rc = j.rec_cum[nb], kc = j.key_cum[nb];
-    PGS_CUDA(cudaMallocAsync(&r->d_blk_rec, sizeof(uint32_t) * (nb + 1), st));
-    PGS_CUDA(cudaMallocAsync(&r->d_ikey_off, sizeof(uint32_t) * (nb + 1), st));
-    PGS_CUDA(cudaMallocAsync(&r->d_ikeys, kc + 16, st));
-    PGS_CUDA(cudaMallocAsync(&r->d_rec_off, sizeof(uint32_t) * (rc + 1), st));
-    PGS_CUDA(cudaMemcpyAsync(r->d_blk_rec, j.rec_cum, sizeof(uint32_t) * (nb + 1), cudaMemcpyHostToDevice, st));
-    PGS_CUDA(cudaMemcpyAsync(r->d_ikey_off, j.key_cum, sizeof(uint32_t) * (nb + 1), cudaMemcpyHostToDevice, st));
-    r->n_bloom_entries = j.hs.n_records + j.hs.n_prefix;
-    r->bloom_lines = bloom_lines_for(r->n_bloom_entries);
-    PGS_CUDA(cudaMallocAsync(&r->d_bloom, (size_t)r->bloom_lines * 64, st));
-    PGS_CUDA(cudaMemsetAsync(r->d_bloom, 0, (size_t)r->bloom_lines * 64, st));
-    k_index_walk<true><<<(nb + kIdxWarps - 1) / kIdxWarps, kIdxWarps * 32, kIdxWarps * kIdxScratch, st>>>(
-        r->d_data, r->d_blk_off, r->d_blk_size, nb, nullptr, nullptr, r->d_ikey_off, r->d_ikeys, r->d_blk_rec, r->d_rec_off, r->d_bloom,
-        r->bloom_lines, j.d_stats, 0);
-    e->launches++;
+    cudaError_t ce = cudaSuccess;
+    const int32_t rc = index_buffers(j.X, *j.r, j.nrec, j.lastlen, *j.hs_out, j.rec_cum, j.key_cum, [&](auto *&p, uint64_t n, int fill) {
+        const size_t bytes = sizeof(*p) * n;
+        if (ce == cudaSuccess) ce = cudaMallocAsync((void **)&p, bytes, st); // ~Run frees the run's buffers
+        if (ce == cudaSuccess && fill != kNoFill) ce = cudaMemsetAsync(p, fill, bytes, st);
+    });
+    if (rc) return rc;
+    PGS_CUDA(ce);
+    PGS_CUDA(cudaMemcpyAsync(j.X.blk_rec, j.rec_cum, sizeof(uint32_t) * (nb + 1), cudaMemcpyHostToDevice, st));
+    PGS_CUDA(cudaMemcpyAsync(j.X.ikey_off, j.key_cum, sizeof(uint32_t) * (nb + 1), cudaMemcpyHostToDevice, st));
+    e->launches += index_launch_pass2(j.X, st);
     PGS_CUDA(cudaEventRecord(j.pass1, st)); // reused: now marks the end of the second pass
     return PGS_OK;
 }
@@ -348,9 +322,7 @@ static int32_t upload_stage_c(Engine *e, Partition &p, UploadJob &j, uint64_t *r
 {
     Run *r = j.r.get();
     PGS_CUDA(cudaEventSynchronize(j.pass1));
-    cudaFreeAsync(j.d_stats, e->stream);
-    j.d_stats = nullptr;
-    run_info_from_index(j.hs, r->info.n_blocks, r->info.data_bytes, j.max_blk, r->info);
+    run_info_from_index(*j.hs_out, r->info.n_blocks, r->info.data_bytes, j.max_blk, r->info);
     r->id = e->next_run_id++;
     r->info.run_id = r->id;
     {
@@ -360,16 +332,11 @@ static int32_t upload_stage_c(Engine *e, Partition &p, UploadJob &j, uint64_t *r
     if (run_id_out) *run_id_out = r->id;
     return PGS_OK;
 }
-// a failed job: nothing of it may still be in flight when its host vectors and device buffers go away
-static void upload_abandon(Engine *e, UploadJob &j)
+// a failed job: nothing of it may still be in flight when its host staging and device buffers go away
+static void upload_abandon(Engine *e)
 {
     cudaStreamSynchronize(e->up_copy);
     cudaStreamSynchronize(e->stream);
-    if (j.d_nrec) cudaFreeAsync(j.d_nrec, e->stream);
-    if (j.d_lastlen) cudaFreeAsync(j.d_lastlen, e->stream);
-    if (j.d_stats) cudaFreeAsync(j.d_stats, e->stream);
-    j.d_nrec = j.d_lastlen = nullptr;
-    j.d_stats = nullptr;
 }
 
 } // namespace pgs
@@ -499,7 +466,7 @@ int32_t pgs_run_upload_many(pgs_partition *ph, const pgs_run_src *runs, uint32_t
     int32_t rc = PGS_OK;
     auto stage_a = [&](uint32_t i) {
         if (runs[i].n_blocks == 0) return (int32_t)PGS_OK; // an empty run: id 0, nothing resident
-        jobs[i] = std::make_unique<UploadJob>();
+        jobs[i] = std::make_unique<UploadJob>(e);
         return upload_stage_a(e, runs[i].level, runs[i].data, runs[i].data_bytes, runs[i].blk_off, runs[i].blk_size, runs[i].n_blocks, *jobs[i]);
     };
     // the next run's bytes are queued on the link before this run's index is finished
@@ -512,7 +479,7 @@ int32_t pgs_run_upload_many(pgs_partition *ph, const pgs_run_src *runs, uint32_t
     }
     if (rc == PGS_OK && n && jobs[n - 1]) { rc = upload_stage_c(e, p, *jobs[n - 1], &ids[n - 1]); if (rc == PGS_OK) done = n; }
     if (rc != PGS_OK) { // all or nothing
-        for (auto &j : jobs) if (j) upload_abandon(e, *j);
+        upload_abandon(e);
         for (uint32_t i = 0; i < done; i++) if (ids[i]) pgs_run_drop(ph, ids[i]);
         return rc;
     }
@@ -534,12 +501,7 @@ static int32_t run_build_sorted(Engine *e, Partition &p, int32_t level, BuildPar
 {
     cudaStream_t st = e->stream;
     cudaError_t ce = cudaSuccess;
-    build_buffers(P, [&](auto *&q, uint64_t cnt, int fill) {
-        const size_t bytes = sizeof(*q) * cnt;
-        if (ce != cudaSuccess) return;
-        ce = S.alloc(q, bytes ? bytes : 16);
-        if (ce == cudaSuccess && fill != kNoFill) ce = cudaMemsetAsync(q, fill, bytes, st);
-    });
+    build_buffers(P, scratch_buffers(S, ce));
     PGS_CUDA(ce);
     PGS_CUDA(cudaEventRecord(ev[1], st));
     e->launches += build_launch_plan(P, 0, st, [](int) {});
@@ -559,7 +521,7 @@ static int32_t run_build_sorted(Engine *e, Partition &p, int32_t level, BuildPar
     }
     // the blocks are written into the run's buffer, where the upload's passes take them
     const uint32_t nb = (uint32_t)sum.n_blocks;
-    UploadJob j;
+    UploadJob j(e);
     j.max_blk = sum.max_blk;
     int32_t rc = upload_job_init(e, level, nb, sum.data_bytes, j);
     if (rc == PGS_OK) {
@@ -575,7 +537,7 @@ static int32_t run_build_sorted(Engine *e, Partition &p, int32_t level, BuildPar
         rc = ce == cudaSuccess ? PGS_OK : cuda_fail(ce, "run build: blocks");
     }
     if (rc == PGS_OK) {
-        upload_pass1(e, j, 0, nb);
+        e->launches += index_launch_pass1(j.X, 0, nb, st);
         rc = upload_pass1_done(e, j);
     }
     if (rc == PGS_OK) rc = upload_stage_b(e, j);
@@ -583,7 +545,7 @@ static int32_t run_build_sorted(Engine *e, Partition &p, int32_t level, BuildPar
         ce = cudaEventRecord(ev[4], st);
         rc = ce == cudaSuccess ? upload_stage_c(e, p, j, run_id_out) : cuda_fail(ce, "run build: index");
     }
-    if (rc != PGS_OK) upload_abandon(e, j);
+    if (rc != PGS_OK) upload_abandon(e);
     return rc;
 }
 
@@ -610,18 +572,9 @@ int32_t pgs_run_build(pgs_partition *ph, int32_t level, uint64_t n, const uint8_
     // the whole input goes to the device
     BuildParams P{};
     build_plan(P, (uint32_t)n, e->cfg.block_size, e->cfg.restart_interval);
-    const uint64_t kb = key_off[n], vb = val_off[n];
-    uint8_t *d_keys, *d_vals;
-    PGS_CUDA(S.alloc(d_keys, kb + 16));
-    PGS_CUDA(S.alloc(d_vals, vb + 16));
-    if (kb) PGS_CUDA(cudaMemcpyAsync(d_keys, keys, kb, cudaMemcpyHostToDevice, st));
-    if (vb) PGS_CUDA(cudaMemcpyAsync(d_vals, vals, vb, cudaMemcpyHostToDevice, st));
-    PGS_CUDA(S.upload(P.key_off, (const unsigned long long *)key_off, n + 1));
-    PGS_CUDA(S.upload(P.val_off, (const unsigned long long *)val_off, n + 1));
-    PGS_CUDA(S.upload(P.seq, (const unsigned long long *)seq, n));
-    PGS_CUDA(S.upload(P.type, type, n));
-    P.keys = d_keys;
-    P.vals = d_vals;
+    cudaError_t ce = cudaSuccess;
+    stage_records(P, n, keys, key_off, vals, val_off, seq, type, device_buffers(S, ce));
+    PGS_CUDA(ce);
     if (const int32_t rc = run_build_sorted(e, p, level, P, S, ev, run_id_out)) return rc;
     if (cudaEventSynchronize(ev[4]) == cudaSuccess)
         for (int i = 0; i < 4; i++) cudaEventElapsedTime(&t_build_ms[i], ev[i], ev[i + 1]);
@@ -661,29 +614,11 @@ int32_t pgs_run_build_unsorted(pgs_partition *ph, int32_t level, uint64_t n, con
         LaunchScratch SS(st);
         SortParams Q{};
         sort_plan(Q, (uint32_t)n);
-        const uint64_t kb = key_off[n], vb = val_off[n];
-        uint8_t *d_keys, *d_vals;
-        PGS_CUDA(SS.alloc(d_keys, kb + 16));
-        PGS_CUDA(SS.alloc(d_vals, vb + 16));
-        if (kb) PGS_CUDA(cudaMemcpyAsync(d_keys, keys, kb, cudaMemcpyHostToDevice, st));
-        if (vb) PGS_CUDA(cudaMemcpyAsync(d_vals, vals, vb, cudaMemcpyHostToDevice, st));
-        PGS_CUDA(SS.upload(Q.key_off, (const unsigned long long *)key_off, n + 1));
-        PGS_CUDA(SS.upload(Q.val_off, (const unsigned long long *)val_off, n + 1));
-        PGS_CUDA(SS.upload(Q.seq, (const unsigned long long *)seq, n));
-        PGS_CUDA(SS.upload(Q.type, type, n));
-        Q.keys = d_keys;
-        Q.vals = d_vals;
-        PGS_CUDA(cudaEventRecord(ev_copied, st));
         cudaError_t ce = cudaSuccess;
-        auto alloc_in = [&](LaunchScratch &to) {
-            return [&](auto *&q, uint64_t cnt, int fill) {
-                const size_t bytes = sizeof(*q) * cnt;
-                if (ce != cudaSuccess) return;
-                ce = to.alloc(q, bytes ? bytes : 16);
-                if (ce == cudaSuccess && fill != kNoFill) ce = cudaMemsetAsync(q, fill, bytes, st);
-            };
-        };
-        sort_buffers(Q, kb, vb, alloc_in(SS), alloc_in(S)); // the sorted copy lives as long as the build's scratch
+        stage_records(Q, n, keys, key_off, vals, val_off, seq, type, device_buffers(SS, ce));
+        PGS_CUDA(ce);
+        PGS_CUDA(cudaEventRecord(ev_copied, st));
+        sort_buffers(Q, key_off[n], val_off[n], scratch_buffers(SS, ce), scratch_buffers(S, ce)); // the sorted copy lives as long as the build's scratch
         PGS_CUDA(ce);
         size_t pin_cap = 0;
         auto *hsum = (SortSummary *)e->take_pinned(sizeof(SortSummary), &pin_cap);
@@ -705,12 +640,7 @@ int32_t pgs_run_build_unsorted(pgs_partition *ph, int32_t level, uint64_t n, con
                                                      : "run build: a user key over %u bytes", kMaxUkeyLen);
             return rc;
         }
-        P.keys = Q.s_keys;
-        P.vals = Q.s_vals;
-        P.type = Q.s_type;
-        P.key_off = Q.s_key_off;
-        P.val_off = Q.s_val_off;
-        P.seq = Q.s_seq;
+        build_inputs_sorted(P, Q);
     }
     if (const int32_t rc = run_build_sorted(e, p, level, P, S, ev, run_id_out)) return rc;
     if (cudaEventSynchronize(ev[4]) == cudaSuccess) {

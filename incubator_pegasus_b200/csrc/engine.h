@@ -13,7 +13,7 @@
 
 #include "../../include/pegasus_b200.h"
 #include "../host/hotkey.h"
-#include "format.h"
+#include "device_util.cuh"
 
 namespace pgs {
 
@@ -176,7 +176,27 @@ struct LaunchScratch {
     }
 };
 
-// scans an uploaded / freshly merged run's blocks on the device and fills the index + info
+// The (pointer, count, fill[, out]) buffers of a launch plan (build_buffers, sort_buffers, split_buffers, ...) in S: count
+// elements each, every byte set to fill unless it is kNoFill.  ce keeps the first failure; after it nothing is allocated.
+inline auto scratch_buffers(LaunchScratch &S, cudaError_t &ce)
+{
+    return [&S, &ce](auto *&p, uint64_t count, int fill, bool = false) {
+        const size_t bytes = sizeof(*p) * count;
+        if (ce != cudaSuccess) return;
+        ce = S.alloc(p, bytes ? bytes : 16);
+        if (ce == cudaSuccess && fill != kNoFill) ce = cudaMemsetAsync((void *)p, fill, bytes, S.st);
+    };
+}
+// The (pointer, bytes, ReadInit) buffers of a launch plan (get_buffers, scan_buffers, stage_records) in S, on its stream; ce
+// keeps the first failure
+inline auto device_buffers(LaunchScratch &S, cudaError_t &ce)
+{
+    return [&S, &ce](auto *&p, uint64_t bytes, ReadInit in) {
+        if (ce == cudaSuccess) ce = S.alloc(p, bytes);
+        if (ce == cudaSuccess && in.src) ce = cudaMemcpyAsync((void *)p, in.src, in.src_bytes, cudaMemcpyHostToDevice, S.st);
+        if (ce == cudaSuccess && in.fill != kNoFill) ce = cudaMemsetAsync((void *)p, in.fill, bytes, S.st);
+    };
+}
 
 } // namespace pgs
 

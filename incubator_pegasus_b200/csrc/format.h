@@ -28,6 +28,9 @@ constexpr uint32_t kMaxRuns = 16;        // k of one merge launch
 constexpr uint32_t kMaxUkeyLen = 4096;   // compaction / lookup fast path limit
 constexpr uint32_t kEpochBegin = 1451606400u; // src/base/pegasus_utils.h:39
 
+// v rounded up to kBlockAlign: a block's size with its zero padding, and the end of a run's last block as the run keeps it
+PGS_HD uint64_t block_pad(uint64_t v) { return (v + kBlockAlign - 1) & ~(uint64_t)(kBlockAlign - 1); }
+
 PGS_HD uint32_t be32(const uint8_t *p)
 {
     return ((uint32_t)p[0] << 24) | ((uint32_t)p[1] << 16) | ((uint32_t)p[2] << 8) | p[3];

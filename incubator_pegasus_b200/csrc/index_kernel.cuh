@@ -1,11 +1,11 @@
-// index_kernel.cuh — the block index and Bloom filter of a run, built on the device when the run is uploaded (engine.cu).
-// Also compiled by the host SIMT interpreter (tools/simt/sim_compact.cpp), so that the CPU suite reads runs through the
-// index and filter this kernel builds.
+// index_kernel.cuh — the block index and Bloom filter of a run, built on the device when the run is uploaded or built
+// (engine.cu).  Also compiled by the host SIMT interpreter (tools/simt/sim_compact.cpp), so that the CPU suite reads runs through
+// the index and filter this kernel builds, planned and launched as the library does.
 //
 // index build: one warp walks one block (entries are sequential inside a restart interval and the last key needs every
 // delta before it), the running internal key lives in a per-warp shared-memory scratch.  Two passes:
 //   k_index_walk<false>  records and last-user-key length per block, run statistics, number of Bloom prefix entries
-//   (host)               index_layout: prefix sums over the blocks -> blk_rec, ikey_off
+//   (host)               index_buffers: prefix sums over the blocks -> blk_rec, ikey_off
 //   k_index_walk<true>   index keys, entry offsets, Bloom filter (sized bloom_lines_for(n_records + n_prefix))
 #pragma once
 #include "group.cuh"
@@ -135,11 +135,57 @@ inline uint32_t run_handles_check(const uint64_t *blk_off, const uint32_t *blk_s
     return nb;
 }
 
-// host, between the two passes: rec_cum / key_cum[0..nb] = exclusive prefix sums of the records and of the last-user-key
-// lengths of the blocks (the first record and the index key of every block).  false: the run is too large for the 32-bit
-// offsets of the index.
-inline bool index_layout(const uint32_t *nrec, const uint32_t *lastlen, uint32_t nb, uint32_t *rec_cum, uint32_t *key_cum)
+// ---- plan, buffers, launches: shared by the upload and the run build (engine.cu) and the simulator (tools/simt/sim_compact.cpp)
+// index_scratch, pass 1 (once, or once per chunk of blocks), its results on the host, index_buffers, pass 2.
+struct IndexParams {
+    // the run's blocks: blk_off[nb + 1] (the last one the 16-aligned end of the blocks), blk_size[nb]
+    const uint8_t *data;
+    const uint64_t *blk_off;
+    const uint32_t *blk_size;
+    uint32_t nb;
+    // pass-1 scratch (index_scratch): records and last-user-key length per block, the run's statistics (index_stats_init)
+    uint32_t *nrec, *lastlen;
+    IndexStats *stats;
+    // the index (index_buffers): blk_rec / ikey_off [nb + 1], the index keys, the entry offsets, the Bloom filter
+    uint32_t *blk_rec, *ikey_off;
+    uint8_t *ikeys;
+    uint32_t *rec_off, *bloom;
+    uint32_t bloom_lines;
+};
+
+inline IndexStats index_stats_init() { return IndexStats{0, 0, 0, 0, ~0ull, 0, 0, 0, 0, 0, 0}; } // min_seq = ~0
+
+// pass 1's scratch through alloc(p, count, fill) (fill = a byte value or kNoFill); the caller sets *X.stats = index_stats_init()
+template <class Alloc>
+void index_scratch(IndexParams &X, Alloc &&alloc)
 {
+    alloc(X.nrec, X.nb, kNoFill);
+    alloc(X.lastlen, X.nb, kNoFill);
+    alloc(X.stats, 1, kNoFill);
+}
+
+// pass 1 over the blocks [b0, b1); returns the launches
+inline uint32_t index_launch_pass1(const IndexParams &X, uint32_t b0, uint32_t b1, cudaStream_t st)
+{
+    if (b1 <= b0) return 0;
+    PGS_LAUNCH(k_index_walk<false>, (b1 - b0 + kIdxWarps - 1) / kIdxWarps, kIdxWarps * 32, kIdxWarps * kIdxScratch, st, X.data, X.blk_off,
+               X.blk_size, b1, X.nrec, X.lastlen, nullptr, nullptr, nullptr, nullptr, nullptr, 0u, X.stats, b0);
+    return 1;
+}
+
+// Between the passes, with pass 1's nrec / lastlen [nb] and stats st on the host: the index layout into the host arrays rec_cum /
+// key_cum [nb + 1], the exclusive prefix sums of the records and of the last-user-key lengths (the first record and the index
+// key of every block; the caller copies them to X.blk_rec / X.ikey_off), and the run r's index buffers through alloc(p, count,
+// fill), X pointed at them.  Returns the walks' verdict, or kNotSupported beyond the index's 32-bit offsets.
+template <class RunT, class Alloc>
+int32_t index_buffers(IndexParams &X, RunT &r, const uint32_t *nrec, const uint32_t *lastlen, const IndexStats &st, uint32_t *rec_cum,
+                      uint32_t *key_cum, Alloc &&alloc)
+{
+    const uint32_t nb = X.nb;
+    if (st.error) {
+        set_error("run upload: block scan failed with status %u", st.error);
+        return (int32_t)st.error;
+    }
     uint64_t rc = 0, kc = 0;
     for (uint32_t b = 0; b < nb; b++) {
         rec_cum[b] = (uint32_t)rc;
@@ -147,10 +193,31 @@ inline bool index_layout(const uint32_t *nrec, const uint32_t *lastlen, uint32_t
         rc += nrec[b];
         kc += lastlen[b];
     }
-    if (rc > 0xFFFFFFF0ull || kc > 0xFFFFFFF0ull) return false;
+    if (rc > 0xFFFFFFF0ull || kc > 0xFFFFFFF0ull) {
+        set_error("run too large for 32-bit record / index-key offsets");
+        return PGS_NOT_SUPPORTED;
+    }
     rec_cum[nb] = (uint32_t)rc;
     key_cum[nb] = (uint32_t)kc;
-    return true;
+    alloc(r.d_blk_rec, nb + 1ull, kNoFill);
+    alloc(r.d_ikey_off, nb + 1ull, kNoFill);
+    alloc(r.d_ikeys, key_cum[nb] + 16ull, kNoFill);
+    alloc(r.d_rec_off, rec_cum[nb] + 1ull, kNoFill);
+    r.n_bloom_entries = st.n_records + st.n_prefix;
+    r.bloom_lines = bloom_lines_for(r.n_bloom_entries);
+    alloc(r.d_bloom, r.bloom_lines * 16ull, 0);
+    X.blk_rec = r.d_blk_rec, X.ikey_off = r.d_ikey_off, X.ikeys = r.d_ikeys;
+    X.rec_off = r.d_rec_off, X.bloom = r.d_bloom, X.bloom_lines = r.bloom_lines;
+    return PGS_OK;
+}
+
+// pass 2 over every block; returns the launches
+inline uint32_t index_launch_pass2(const IndexParams &X, cudaStream_t st)
+{
+    if (!X.nb) return 0;
+    PGS_LAUNCH(k_index_walk<true>, (X.nb + kIdxWarps - 1) / kIdxWarps, kIdxWarps * 32, kIdxWarps * kIdxScratch, st, X.data, X.blk_off,
+               X.blk_size, X.nb, nullptr, nullptr, X.ikey_off, X.ikeys, X.blk_rec, X.rec_off, X.bloom, X.bloom_lines, X.stats, 0u);
+    return 1;
 }
 
 // host, after the second pass: the run's pgs_run_info from the index statistics, the block count, the 16-aligned end of its

@@ -77,16 +77,6 @@ int32_t lookup_init_kernels(Engine &e)
     return PGS_OK;
 }
 
-// the buffers of a read launch (get_buffers, scan_buffers) in its device scratch, on its stream; ce = the first failure
-static auto device_buffers(LaunchScratch &S, cudaError_t &ce)
-{
-    return [&S, &ce](auto *&p, uint64_t bytes, ReadInit in) {
-        if (ce == cudaSuccess) ce = S.alloc(p, bytes);
-        if (ce == cudaSuccess && in.src) ce = cudaMemcpyAsync((void *)p, in.src, in.src_bytes, cudaMemcpyHostToDevice, S.st);
-        if (ce == cudaSuccess && in.fill != kNoFill) ce = cudaMemsetAsync((void *)p, in.fill, bytes, S.st);
-    };
-}
-
 // the CTAs of L the device holds at once (resident CTAs per SM for its dynamic shared memory; registers count too)
 template <class Params>
 static cudaError_t resident_ctas(const Engine &e, const ReadLaunch<Params> &L, uint64_t &ctas)

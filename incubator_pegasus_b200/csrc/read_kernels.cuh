@@ -642,7 +642,6 @@ inline scan_fwd_kernel_t scan_fwd_kernel(uint32_t G, bool multi)
 }
 
 // ---- the read launch plan: what the library (lookup.cu) and the simulator (tools/simt) both launch ------------------------------
-void set_error(const char *fmt, ...); // the message of a refused call (engine.cu; the simulator prints it)
 
 // the largest block of a launch's runs, in bytes and in records (k_scan's staging pool, scan_kernel.cuh)
 struct ScanBlockBound {
@@ -714,14 +713,6 @@ inline int32_t get_plan(GetParams &P, const ReadRunSet &R, uint32_t max_smem_opt
     L = {R.multi ? k_get<8, true> : k_get<8, false>, kReadThreads, geo.dyn, kReadThreads / geo.G};
     return PGS_OK;
 }
-
-// the initial content of a launch buffer: src_bytes copied from the host, or every byte set to fill, or none
-struct ReadInit {
-    const void *src = nullptr;
-    uint64_t src_bytes = 0;
-    int fill = kNoFill;
-};
-constexpr ReadInit kZero{nullptr, 0, 0};
 
 // the buffers of a multi-partition launch: its packed runs, their slot bounds, and the slot of each of its n requests
 template <class F>

@@ -368,6 +368,12 @@ void sort_buffers(SortParams &P, uint64_t kb, uint64_t vb, Alloc &&alloc, AllocO
     alloc_out(P.s_seq, n, kNoFill);
     alloc_out(P.s_type, n, kNoFill);
 }
+// the sorted copy handed to the build as its inputs
+inline void build_inputs_sorted(BuildParams &B, const SortParams &P)
+{
+    B.keys = P.s_keys, B.vals = P.s_vals, B.type = P.s_type;
+    B.key_off = P.s_key_off, B.val_off = P.s_val_off, B.seq = P.s_seq;
+}
 // the status of a summary's flags, in the documented precedence
 inline int32_t sort_status(uint32_t flags)
 {

@@ -64,36 +64,29 @@ struct HostRun {
     }
 };
 
-// the run's index and Bloom filter as pgs_run_upload builds them (engine.cu): the two passes of k_index_walk with the host
-// layout between them.  Returns the upload's status: what the blocks' walks reported (the largest), or kNotSupported for a run
-// beyond the index's 32-bit offsets
-int32_t build_index(HostRun &r, uint32_t nb)
+// the (pointer, count, fill[, out]) buffers of a launch plan in mem at the library's sizes; what the library leaves unset
+// (kNoFill) is poisoned until the kernels write it
+auto host_count_buffers(HostMem &mem)
 {
-    std::vector<uint32_t> nrec(nb + 1), lastlen(nb + 1);
-    IndexStats st{};
-    st.min_seq = ~0ull;
-    const uint32_t grid = (nb + kIdxWarps - 1) / kIdxWarps, smem = kIdxWarps * kIdxScratch;
-    if (nb)
-        PGS_LAUNCH(k_index_walk<false>, grid, kIdxWarps * 32, smem, 0, (const uint8_t *)r.d_data, (const uint64_t *)r.d_blk_off,
-                   (const uint32_t *)r.d_blk_size, nb, nrec.data(), lastlen.data(), (const uint32_t *)nullptr, (uint8_t *)nullptr,
-                   (const uint32_t *)nullptr, (uint32_t *)nullptr, (uint32_t *)nullptr, 0u, &st, 0u);
-    if (st.error) return (int32_t)st.error;
-    host_alloc(r.mem, r.d_blk_rec, nb + 1, 0);
-    host_alloc(r.mem, r.d_ikey_off, nb + 1, 0);
-    if (!index_layout(nrec.data(), lastlen.data(), nb, r.d_blk_rec, r.d_ikey_off)) return PGS_NOT_SUPPORTED;
-    host_alloc(r.mem, r.d_ikeys, r.d_ikey_off[nb] + 16, 0); // the product's slack (engine.cu)
-    host_alloc(r.mem, r.d_rec_off, r.d_blk_rec[nb] + 1, 0);
-    r.n_bloom_entries = st.n_records + st.n_prefix;
-    r.bloom_lines = bloom_lines_for(r.n_bloom_entries);
-    host_alloc(r.mem, r.d_bloom, (uint64_t)r.bloom_lines * 16, 0);
-    if (nb)
-        PGS_LAUNCH(k_index_walk<true>, grid, kIdxWarps * 32, smem, 0, (const uint8_t *)r.d_data, (const uint64_t *)r.d_blk_off,
-                   (const uint32_t *)r.d_blk_size, nb, (uint32_t *)nullptr, (uint32_t *)nullptr, (const uint32_t *)r.d_ikey_off,
-                   r.d_ikeys, (const uint32_t *)r.d_blk_rec, r.d_rec_off, r.d_bloom, r.bloom_lines, &st, 0u);
-    if (st.error) return (int32_t)st.error;
-    uint32_t max_blk = 0;
-    for (uint32_t b = 0; b < nb; b++) max_blk = std::max(max_blk, r.d_blk_size[b]);
-    run_info_from_index(st, nb, r.d_blk_off[nb], max_blk, r.info);
+    return [&mem](auto *&p, uint64_t count, int fill, bool = false) { host_alloc(mem, p, count, fill == kNoFill ? 0xEE : fill); };
+}
+
+// the run's index and Bloom filter as pgs_run_upload builds them (engine.cu): index_scratch, pass 1, index_buffers, pass 2.
+// max_blk: the run's largest block, as the library has it.  Returns the upload's status.
+int32_t build_index(HostRun &r, uint32_t nb, uint32_t max_blk)
+{
+    HostMem scratch;
+    IndexParams X{r.d_data, r.d_blk_off, r.d_blk_size, nb};
+    index_scratch(X, host_count_buffers(scratch));
+    *X.stats = index_stats_init();
+    index_launch_pass1(X, 0, nb, nullptr);
+    std::vector<uint32_t> rec_cum(nb + 1), key_cum(nb + 1);
+    if (const int32_t rc = index_buffers(X, r, X.nrec, X.lastlen, *X.stats, rec_cum.data(), key_cum.data(), host_count_buffers(r.mem))) return rc;
+    memcpy(r.d_blk_rec, rec_cum.data(), 4 * (nb + 1ull));
+    memcpy(r.d_ikey_off, key_cum.data(), 4 * (nb + 1ull));
+    index_launch_pass2(X, nullptr);
+    if (X.stats->error) return (int32_t)X.stats->error;
+    run_info_from_index(*X.stats, nb, r.d_blk_off[nb], max_blk, r.info);
     return PGS_OK;
 }
 
@@ -105,12 +98,12 @@ int32_t load_run(HostRun &r, const uint8_t *data, uint64_t data_bytes, const uin
     uint64_t last_end = 0;
     uint32_t max_blk = 0;
     if (run_handles_check(blk_off, blk_size, nb, data_bytes, last_end, max_blk) < nb) return PGS_INVALID_ARGUMENT;
-    const uint64_t end = (last_end + kBlockAlign - 1) / kBlockAlign * kBlockAlign;
+    const uint64_t end = block_pad(last_end);
     memcpy(host_alloc(r.mem, r.d_data, end + 256, 0), data, std::min(data_bytes, end));
     memcpy(host_alloc(r.mem, r.d_blk_off, nb + 1, 0), blk_off, 8 * (size_t)nb);
     memcpy(host_alloc(r.mem, r.d_blk_size, nb, 0), blk_size, 4 * (size_t)nb);
     r.d_blk_off[nb] = end;
-    return build_index(r, nb);
+    return build_index(r, nb, max_blk);
 }
 
 uint64_t crc_tab[256];
@@ -174,9 +167,7 @@ int32_t sim_compact(uint32_t k, const uint8_t **data, const uint64_t *data_bytes
     if (!compact_geometry(P, T, compact_smem_budget(kSimSmemOptin), geo, group_lanes, seg_weight)) return PGS_NOT_SUPPORTED;
     Merged &R = g_res;
     R = Merged{};
-    compact_buffers(P, geo, T, R.run, [&](auto *&p, uint64_t n, int fill, bool out) {
-        host_alloc(out ? R.run.mem : scratch, p, n, fill == kNoFill ? 0xEE : fill); // poisoned until the kernels write it
-    });
+    compact_buffers(P, geo, T, R.run, [&](auto *&p, uint64_t n, int fill, bool out) { host_count_buffers(out ? R.run.mem : scratch)(p, n, fill); });
     MergeStats st = merge_stats_init();
     P.stats = &st;
     compact_launch(P, geo, 2, 2, nullptr, [](int) {});
@@ -236,7 +227,7 @@ static uint32_t copy_bloom(const HostRun &r, uint32_t *out, uint64_t cap)
 // the Bloom filter of the last sim_compact output (the one k_emit built)
 uint32_t sim_result_bloom(uint32_t *out, uint64_t cap) { return copy_bloom(g_res.run, out, cap); }
 
-// the Bloom filter the upload builds for one run (k_index_walk); 0 lines: a run the upload refuses
+// the Bloom filter the upload builds for one run (the index build of build_index); 0 lines: a run the upload refuses
 uint32_t sim_run_bloom(const uint8_t *data, uint64_t data_bytes, const uint64_t *blk_off, const uint32_t *blk_size, uint32_t n_blocks,
                        uint32_t *out, uint64_t cap)
 {
@@ -305,7 +296,7 @@ static auto host_buffers(HostMem &mem)
 {
     return [&mem](auto *&p, uint64_t bytes, ReadInit in) {
         uint8_t *b;
-        host_alloc(mem, b, bytes, in.fill == kNoFill ? 0xEE : in.fill);
+        host_count_buffers(mem)(b, bytes, in.fill);
         if (in.src) memcpy(b, in.src, in.src_bytes);
         p = (std::remove_reference_t<decltype(p)>)b;
     };
@@ -505,7 +496,7 @@ int32_t sim_split(const uint8_t *data, uint64_t data_bytes, const uint64_t *blk_
     R.child.resize(NC);
     R.built.assign(NC, 0);
     HostMem scratch;
-    split_buffers(SP, [&](auto *&p, uint64_t n, int fill, bool) { host_alloc(scratch, p, n, fill == kNoFill ? 0xEE : fill); });
+    split_buffers(SP, host_count_buffers(scratch));
     for (uint32_t c = 0; c < NC; c++) SP.stats[c] = merge_stats_init();
     split_launch(SP, geo, nullptr, nullptr, 0, 2, 2, nullptr, [](int) {});
     R.st.assign(SP.stats, SP.stats + NC);
@@ -521,9 +512,7 @@ int32_t sim_split(const uint8_t *data, uint64_t data_bytes, const uint64_t *blk_
         CompactTotals Tc{};
         if (!split_child(SP, R.st[c], SP.prefixes[c], smem, P, g, Tc)) return PGS_NOT_SUPPORTED;
         HostRun &run = R.child[c];
-        compact_buffers(P, g, Tc, run, [&](auto *&p, uint64_t n, int fill, bool out) {
-            if (out) host_alloc(run.mem, p, n, fill == kNoFill ? 0xEE : fill);
-        });
+        compact_buffers(P, g, Tc, run, [&](auto *&p, uint64_t n, int fill, bool out) { if (out) host_count_buffers(run.mem)(p, n, fill); });
         split_child_scratch(SP, c, P);
         Pc.push_back(P);
         gc.push_back(g);
@@ -577,7 +566,7 @@ namespace {
 int32_t build_sorted(BuildParams &P, HostMem &scratch, uint32_t grid_cap)
 {
     Built &R = g_built;
-    build_buffers(P, [&](auto *&p, uint64_t cnt, int fill) { host_alloc(scratch, p, cnt, fill == kNoFill ? 0xEE : fill); });
+    build_buffers(P, host_count_buffers(scratch));
     build_launch_plan(P, grid_cap, nullptr, [](int) {});
     const BuildSummary sum = *P.sum;
     if (const int32_t rc = build_status(sum.flags)) return rc;
@@ -590,7 +579,10 @@ int32_t build_sorted(BuildParams &P, HostMem &scratch, uint32_t grid_cap)
     P.data = r.d_data;
     build_launch_blocks(P, nb, grid_cap, nullptr);
     R.data_bytes = sum.data_bytes;
-    if (const int32_t rc = build_index(r, nb)) return rc;
+    uint64_t end = 0;
+    uint32_t max_blk = 0; // from the built handles (the library takes the summary's)
+    run_handles_check(r.d_blk_off, r.d_blk_size, nb, sum.data_bytes, end, max_blk);
+    if (const int32_t rc = build_index(r, nb, max_blk)) return rc;
     if (r.info.max_block_size != sum.max_blk) { fprintf(stderr, "sim_run_build: largest block %u, the index saw %u\n", sum.max_blk, r.info.max_block_size); return PGS_CORRUPTION; }
     return PGS_OK;
 }
@@ -610,15 +602,7 @@ int32_t sim_run_build(uint64_t n, const uint8_t *keys, const uint64_t *key_off, 
     HostMem scratch;
     BuildParams P{};
     build_plan(P, (uint32_t)n, block_size, restart_interval);
-    uint8_t *k, *v, *t;
-    unsigned long long *ko, *vo, *sq;
-    memcpy(host_alloc(scratch, k, key_off[n] + 16, 0), keys, key_off[n]); // the library's slack
-    memcpy(host_alloc(scratch, v, val_off[n] + 16, 0), vals, val_off[n]);
-    memcpy(host_alloc(scratch, ko, n + 1, 0), key_off, 8 * (n + 1));
-    memcpy(host_alloc(scratch, vo, n + 1, 0), val_off, 8 * (n + 1));
-    memcpy(host_alloc(scratch, sq, n, 0), seq, 8 * n);
-    memcpy(host_alloc(scratch, t, n, 0), type, n);
-    P.keys = k; P.vals = v; P.type = t; P.key_off = ko; P.val_off = vo; P.seq = sq;
+    stage_records(P, n, keys, key_off, vals, val_off, seq, type, host_buffers(scratch));
     return build_sorted(P, scratch, grid_cap);
 }
 
@@ -636,24 +620,15 @@ int32_t sim_run_build_unsorted(uint64_t n, const uint8_t *keys, const uint64_t *
     HostMem scratch;
     SortParams Q{};
     sort_plan(Q, (uint32_t)n);
-    uint8_t *k, *v, *t;
-    unsigned long long *ko, *vo, *sq;
-    memcpy(host_alloc(scratch, k, key_off[n] + 16, 0), keys, key_off[n]); // the library's slack
-    memcpy(host_alloc(scratch, v, val_off[n] + 16, 0), vals, val_off[n]);
-    memcpy(host_alloc(scratch, ko, n + 1, 0), key_off, 8 * (n + 1));
-    memcpy(host_alloc(scratch, vo, n + 1, 0), val_off, 8 * (n + 1));
-    memcpy(host_alloc(scratch, sq, n, 0), seq, 8 * n);
-    memcpy(host_alloc(scratch, t, n, 0), type, n);
-    Q.keys = k; Q.vals = v; Q.type = t; Q.key_off = ko; Q.val_off = vo; Q.seq = sq;
-    auto alloc = [&](auto *&p, uint64_t cnt, int fill) { host_alloc(scratch, p, cnt, fill == kNoFill ? 0xEE : fill); };
-    sort_buffers(Q, key_off[n], val_off[n], alloc, alloc);
+    stage_records(Q, n, keys, key_off, vals, val_off, seq, type, host_buffers(scratch));
+    sort_buffers(Q, key_off[n], val_off[n], host_count_buffers(scratch), host_count_buffers(scratch));
     uint32_t launches = 0;
     const int32_t rc = sort_launch(Q, grid_cap, nullptr, [&](SortSummary &s) { s = *Q.sum; return (int32_t)PGS_OK; }, launches);
     if (launches_out) *launches_out = launches;
     if (rc) return rc;
     BuildParams P{};
     build_plan(P, (uint32_t)n, block_size, restart_interval);
-    P.keys = Q.s_keys; P.vals = Q.s_vals; P.type = Q.s_type; P.key_off = Q.s_key_off; P.val_off = Q.s_val_off; P.seq = Q.s_seq;
+    build_inputs_sorted(P, Q);
     return build_sorted(P, scratch, grid_cap);
 }
 // the last sim_run_build's sizes and info (level and run id zero)
