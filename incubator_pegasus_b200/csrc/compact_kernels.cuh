@@ -406,9 +406,10 @@ __global__ void __launch_bounds__(256) k_plan(const __grid_constant__ MergeParam
     const uint8_t *U = ri.ikeys + ri.ikey_off[b];
     uint32_t ulen = ri.ikey_off[b + 1] - ri.ikey_off[b];
     uint32_t pos[kMaxRuns];
-    unsigned long long Wb = 0, W = 0;
+    unsigned long long Wb = 0, W = 0, W0 = 0;
     for (uint32_t j = 0; j < P.k; j++) {
         const RunDev &rj = P.runs[j];
+        W0 += run_weight(rj, 0, P.rec_cost);
         uint32_t lo = 0, hi = rj.nb; // upper bound: #blocks with last key <= U
         if (j == i) { // the key's own run: its block, and the blocks after it that end with the same user key (older versions)
             lo = b + 1;
@@ -432,7 +433,9 @@ __global__ void __launch_bounds__(256) k_plan(const __grid_constant__ MergeParam
         W += run_weight(rj, ub, P.rec_cost);
         Wb += run_weight(rj, lb, P.rec_cost);
     }
-    unsigned long long q_lo = Wb / P.tile_weight + 1, q_hi = W / P.tile_weight;
+    // the weight starts at the runs' first blocks, not at zero: a run's first block may lie anywhere in its data (an upload
+    // takes any offsets), so the block of the smallest last key (every lb at 0) also bounds the segments in front of it
+    unsigned long long q_lo = Wb == W0 ? 1 : Wb / P.tile_weight + 1, q_hi = W / P.tile_weight;
     if (q_hi > P.Q - 1) q_hi = P.Q - 1;
     for (unsigned long long q = q_lo; q <= q_hi; q++) {
         for (uint32_t j = 0; j < P.k; j++) P.split_pos[q * P.k + j] = pos[j];

@@ -285,7 +285,8 @@ static int32_t upload_stage_a(Engine *e, int32_t level, const uint8_t *data, uin
     while (b0 < nb) { // chunks end on block boundaries
         uint32_t b1 = b0 + 1;
         while (b1 < nb && j.off[b1] - j.off[b0] < kUploadChunk) b1++;
-        const uint64_t lo = j.off[b0], hi = b1 == nb ? nbytes : std::min<uint64_t>(j.off[b1], nbytes);
+        // the first chunk starts at 0: the bytes in front of the first block are the caller's too (pgs_run_download returns them)
+        const uint64_t lo = b0 ? j.off[b0] : 0, hi = b1 == nb ? nbytes : std::min<uint64_t>(j.off[b1], nbytes);
         if (hi > lo) PGS_CUDA(cudaMemcpyAsync(r->d_data + lo, data + lo, hi - lo, cudaMemcpyHostToDevice, cp));
         cudaEvent_t ev;
         PGS_CUDA(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));

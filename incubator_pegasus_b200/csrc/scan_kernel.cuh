@@ -129,6 +129,13 @@ PGS_DEV ScanDir scan_dir(const ScanParams &P, const ScanReqDev &Q, uint32_t rq)
 PGS_DEV uint32_t run_of(const uint32_t *base, uint32_t NR, uint32_t i) { uint32_t j = 0; while (j + 1 < NR && i >= base[j + 1]) j++; return j; }
 // the first (lowest) of the m blocks a run loads from its cursor c: forward c is that block, reverse the last one
 PGS_DEV uint32_t first_block(bool rev, uint32_t c, uint32_t m) { return rev ? c + 1 - m : c; }
+// bytes staged for blocks [lo_b, lo_b + m): up to the 16-aligned end of the last of them, so that a gap behind it (an upload
+// takes any offsets) is not loaded -- a gap of 4 GiB would otherwise wrap the 32-bit size or overflow the pool
+PGS_DEV uint32_t stage_bytes(const RunDev &r, uint32_t lo_b, uint32_t m)
+{
+    const uint32_t last = lo_b + m - 1;
+    return (uint32_t)(((r.blk_off[last] + r.blk_size[last] + 15) & ~15ull) - r.blk_off[lo_b]);
+}
 
 // ---- request setup -----------------------------------------------------------------------------------------------------------
 // initial cursors (one warp per run, 33-ary index search): first block whose last key >= the seek key (reverse: the last block
@@ -243,7 +250,7 @@ PGS_DEV void choose_blocks(ScanShared &S, const ScanParams &P, bool rev, uint32_
             }
         }
         const uint32_t lo_b = first_block(rev, c, m);
-        bytes_j = (uint32_t)(r.blk_off[lo_b + m] - r.blk_off[lo_b]);
+        bytes_j = stage_bytes(r, lo_b, m);
         const uint32_t g0 = r.blk_rec[lo_b];
         recs_j = r.blk_rec[lo_b + m] - g0;
         S.grec0[j] = g0;
@@ -281,7 +288,7 @@ PGS_DEV void stage_blocks(ScanShared &S, const ScanSlots &K, const ScanArrays &A
             if (!m) continue;
             const RunDev &r = P.rr.runs[j];
             const uint32_t lo_b = first_block(rev, S.cur[j], m);
-            tma_load_1d(A.in + S.in_off[j], r.data + r.blk_off[lo_b], (uint32_t)(r.blk_off[lo_b + m] - r.blk_off[lo_b]), (uint64_t *)&S.mbar);
+            tma_load_1d(A.in + S.in_off[j], r.data + r.blk_off[lo_b], stage_bytes(r, lo_b, m), (uint64_t *)&S.mbar);
         }
     }
     for (uint32_t t = tid; t < S.n_blk; t += kScanThreads) {

@@ -67,9 +67,10 @@ INFO_FIELDS = ("n_blocks", "n_records", "n_tombstones", "data_bytes", "raw_key_b
                "max_block_size", "max_block_records", "smallest_seq", "largest_seq")
 
 
-def check_split(pgs, ssim, br, src, dst, want=None, **kw):
-    """split br in the simulator and compare every built child with the model; returns the children"""
-    items = fb.decode(br).to_list()
+def check_split(pgs, ssim, br, src, dst, want=None, items=None, **kw):
+    """split br in the simulator and compare every built child with the model; returns the children.  items: br's records
+    when the caller has them (decoding a run that spans gigabytes copies all of it)"""
+    items = fb.decode(br).to_list() if items is None else items
     want_items, want_dropped = sm.split_items(items, src, dst)
     S = dst // src
     mask = (1 << S) - 1 if want is None else want

@@ -13,6 +13,8 @@
 #include "../../incubator_pegasus_b200/csrc/sort_kernels.cuh"
 #include "../../incubator_pegasus_b200/csrc/split_kernels.cuh"
 
+#include <sys/mman.h>
+
 #include <cstdarg>
 #include <memory>
 #include <new>
@@ -49,6 +51,34 @@ T *host_alloc(HostMem &mem, T *&p, uint64_t n, int fill)
     return p = (T *)b;
 }
 
+// A run's data of kSparseLoad bytes or more (runs placed past 4 GiB) lives in an anonymous mapping, zero until written, and
+// only the source pages that hold a non-zero byte are copied into it: the copy equals the caller's bytes everywhere, but the
+// gigabytes of zeros in front of or between such a run's blocks cost neither host memory nor copy time.  Scratch of that size
+// (a merge's key-stream bound grows with the span of its inputs, gaps included) is such a mapping too, zero rather than
+// poisoned.  AddressSanitizer checks these buffers at page granularity only.
+constexpr uint64_t kSparseLoad = 1ull << 30;
+template <class T>
+T *sparse_alloc(HostMem &mem, T *&p, uint64_t n)
+{
+    const uint64_t bytes = sizeof(T) * n;
+    void *b = mmap(nullptr, bytes, PROT_READ | PROT_WRITE, MAP_PRIVATE | MAP_ANONYMOUS | MAP_NORESERVE, -1, 0);
+    if (b == MAP_FAILED) throw std::bad_alloc();
+    mem.emplace_back(b, [bytes](void *x) { munmap(x, bytes); });
+    return p = (T *)b;
+}
+void sparse_copy(uint8_t *dst, const uint8_t *src, uint64_t n)
+{
+    constexpr uint64_t kPage = 4096;
+    for (uint64_t o = 0; o < n; o += kPage) {
+        const uint64_t len = std::min(kPage, n - o);
+        const uint64_t *w = (const uint64_t *)(src + o); // src is at least 8-aligned (a numpy buffer or the library's)
+        bool zero = true;
+        for (uint64_t i = 0; i < len / 8 && zero; i++) zero = w[i] == 0;
+        for (uint64_t i = len / 8 * 8; i < len && zero; i++) zero = src[o + i] == 0;
+        if (!zero) memcpy(dst + o, src + o, len);
+    }
+}
+
 // a run in host memory, with the buffer fields of the library's Run (engine.h)
 struct HostRun {
     HostMem mem;
@@ -65,10 +95,13 @@ struct HostRun {
 };
 
 // the (pointer, count, fill[, out]) buffers of a launch plan in mem at the library's sizes; what the library leaves unset
-// (kNoFill) is poisoned until the kernels write it
+// (kNoFill) is poisoned until the kernels write it, unless the buffer takes kSparseLoad bytes or more
 auto host_count_buffers(HostMem &mem)
 {
-    return [&mem](auto *&p, uint64_t count, int fill, bool = false) { host_alloc(mem, p, count, fill == kNoFill ? 0xEE : fill); };
+    return [&mem](auto *&p, uint64_t count, int fill, bool = false) {
+        if (fill == kNoFill && sizeof(*p) * count >= kSparseLoad) sparse_alloc(mem, p, count);
+        else host_alloc(mem, p, count, fill == kNoFill ? 0xEE : fill);
+    };
 }
 
 // the run's index and Bloom filter as pgs_run_upload builds them (engine.cu): index_scratch, pass 1, index_buffers, pass 2.
@@ -99,7 +132,8 @@ int32_t load_run(HostRun &r, const uint8_t *data, uint64_t data_bytes, const uin
     uint32_t max_blk = 0;
     if (run_handles_check(blk_off, blk_size, nb, data_bytes, last_end, max_blk) < nb) return PGS_INVALID_ARGUMENT;
     const uint64_t end = block_pad(last_end);
-    memcpy(host_alloc(r.mem, r.d_data, end + 256, 0), data, std::min(data_bytes, end));
+    if (end < kSparseLoad) memcpy(host_alloc(r.mem, r.d_data, end + 256, 0), data, std::min(data_bytes, end));
+    else sparse_copy(sparse_alloc(r.mem, r.d_data, end + 256), data, std::min(data_bytes, end));
     memcpy(host_alloc(r.mem, r.d_blk_off, nb + 1, 0), blk_off, 8 * (size_t)nb);
     memcpy(host_alloc(r.mem, r.d_blk_size, nb, 0), blk_size, 4 * (size_t)nb);
     r.d_blk_off[nb] = end;
