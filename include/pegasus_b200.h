@@ -255,6 +255,42 @@ PGS_API int32_t pgs_compact_ex(pgs_partition *p, const uint64_t *run_ids, uint32
                                int32_t out_level, int32_t bottommost, const pgs_filter_params *fp,
                                uint32_t now, uint32_t flags, pgs_compact_result *out);
 
+/* One compaction job of pgs_compact_many: the arguments pgs_compact_ex takes for one partition. */
+typedef struct {
+    pgs_partition *part;
+    const uint64_t *run_ids;     /* the job's input runs, as pgs_compact takes them                 */
+    uint32_t k;
+    int32_t out_level;
+    int32_t bottommost;          /* -1: derived per partition, as pgs_compact derives it            */
+    const pgs_filter_params *fp; /* per job: pidx, partition_version, default_ttl, ops ... (may be NULL) */
+} pgs_compact_job;
+#define PGS_COMPACT_MANY_MAX_JOBS 4096u
+/* Compactions of many partitions of one engine in one plan and one set of kernel launches on the engine stream.  Job i is by
+ * definition pgs_compact_ex(jobs[i].part, jobs[i].run_ids, jobs[i].k, jobs[i].out_level, jobs[i].bottommost, jobs[i].fp, now,
+ * flags, &out[i]): the same records, counters and run info, and the same reads afterwards.  Only the block layout may differ:
+ * the segments are sized by the whole launch's weight and every segment starts a block, so block cuts (n_blocks, data_bytes,
+ * max_block_size, max_block_records, out_block_bytes) can differ from a pgs_compact of the same job.
+ *   launches: six, whatever n is (out[i].n_launches);
+ *   out (n entries, may be NULL): out[i] = job i's own counters, run id and n_tiles (its segments); device_ms, merge_kernel_ms,
+ *     walk_ms and emit_ms are the call's, repeated in every entry;
+ *   installed runs: as pgs_compact, per job (inputs removed, the merged run installed only when non-empty); flags apply to
+ *     every job.
+ * Statuses, checked before anything is allocated or launched:
+ *   jobs == NULL with n > 0, a job without a partition or run ids, k == 0, out_level < 0, a run given twice, the same partition
+ *   in two jobs, partitions of different engines, a malformed ops table: PGS_INVALID_ARGUMENT;
+ *   an unknown run: PGS_NOT_FOUND;
+ *   n > PGS_COMPACT_MANY_MAX_JOBS, a job of more than 16 runs, a user key over 4096 bytes, or jobs whose joint geometry does not
+ *   fit one launch (the widest user key of any job sizes the key rows of all of them): PGS_NOT_SUPPORTED -- split the call;
+ *   n == 0: PGS_OK, nothing launched.
+ * pgs_last_error() names the failing job.  All or nothing: on any error (a device allocation failure is PGS_IO_ERROR) no
+ * partition's run list changes.
+ * Device memory, all of it allocated before the first launch and held until the call returns: every job's merged run (about
+ * its inputs' raw key and value bytes plus 23 bytes per record and 20 per block) and every job's scratch (about 16 +
+ * (27 + the launch's widest user key, rounded up to 4) bytes per input record, plus the input blocks of two segments'
+ * boundaries), a MergeParams (about 1.8 KB) per job. */
+PGS_API int32_t pgs_compact_many(const pgs_compact_job *jobs, uint32_t n, uint32_t now, uint32_t flags,
+                                 pgs_compact_result *out);
+
 /* ---- partition split ------------------------------------------------------------------------
  * Splits partition `src` (index pidx of `src_count`) into its dst_count / src_count children on the
  * device.  Child i is partition pidx + i * src_count and receives, for every run of the parent, one
@@ -657,6 +693,14 @@ PGS_API int32_t pgs_rrdb_flush(pgs_server *s, uint32_t now);
 /* do_manual_compact (pegasus_server_impl.cpp:3373-3456): whole-CF CompactRange, bottommost
  * level forced. */
 PGS_API int32_t pgs_rrdb_manual_compact(pgs_server *s, uint32_t now, pgs_compact_result *out);
+/* pgs_rrdb_manual_compact of n replicas of one engine, the merges in one pgs_compact_many: every replica's memtable is
+ * flushed, a stack deeper than 16 runs folded first, then its whole run list merged at the deepest level present (at least
+ * 1), bottommost forced, and manual_compact_last_finish_ms set.  The replicas' writer locks are taken in address order and
+ * held until the runs are installed.  out: n entries (may be NULL), replica i's result.  Replicas on different engines, or
+ * one given twice: PGS_INVALID_ARGUMENT.  If the joint merge fails no replica's runs change; a memtable already flushed
+ * stays flushed and a deep stack already folded stays folded, as with pgs_rrdb_manual_compact. */
+PGS_API int32_t pgs_rrdb_manual_compact_many(pgs_server *const *servers, uint32_t n, uint32_t now,
+                                             pgs_compact_result *out);
 /* last_flushed_decree: the newest decree whose data lives in an HBM run (advanced by a memtable flush, like the decree the
  * reference persists in the SST meta CF); last_committed_decree: the newest decree applied to the memtable.  Nothing here is
  * durable across a process crash (no WAL / checkpoint yet: SURVEY 8 f4), so neither may drive replication-log GC. */

@@ -74,6 +74,11 @@ class CompactResult(C.Structure):
                 ("reserved", C.c_uint32)]
 
 
+class CompactJob(C.Structure):
+    _fields_ = [("part", C.c_void_p), ("run_ids", C.POINTER(C.c_uint64)), ("k", C.c_uint32), ("out_level", C.c_int32),
+                ("bottommost", C.c_int32), ("fp", C.POINTER(FilterParams))]
+
+
 SPLIT_MAX_CHILDREN = 32
 
 
@@ -257,6 +262,8 @@ def lib() -> C.CDLL:
         "pgs_rrdb_multi_remove": [vp, Blob, C.POINTER(Blob), C.c_uint32, C.c_int64, C.POINTER(C.c_int64), C.c_uint32],
         "pgs_rrdb_flush": [vp, C.c_uint32],
         "pgs_rrdb_manual_compact": [vp, C.c_uint32, C.POINTER(CompactResult)],
+        "pgs_rrdb_manual_compact_many": [C.POINTER(vp), C.c_uint32, C.c_uint32, C.POINTER(CompactResult)],
+        "pgs_compact_many": [C.POINTER(CompactJob), C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(CompactResult)],
         "pgs_rrdb_detect_hotkey": [vp, C.c_int32, C.c_int32, C.c_uint32, C.c_char_p, C.c_uint32, u32p],
         "pgs_rrdb_hotkey_analyse": [vp, C.c_uint32],
         "pgs_rrdb_hotkey_state": [vp, C.c_int32],
@@ -392,6 +399,23 @@ def parse_ops(json_text: str, data_version: int = 1) -> np.ndarray:
     return buf[:n].copy()
 
 
+def _filter_params(enabled: bool = True, default_ttl: int = 0, validate_hash: bool = False, pidx: int = 0,
+                   partition_version: int = -1, ops: np.ndarray | None = None, data_version: int = 1) -> FilterParams:
+    """the FilterParams of Engine.compact_many's filter kwargs; the struct keeps its ops table alive (fp._ops)"""
+    fp = FilterParams()
+    fp.enabled = 1 if enabled else 0
+    fp.validate_hash = 1 if validate_hash else 0
+    fp.data_version = data_version
+    fp.default_ttl = default_ttl
+    fp.pidx = pidx
+    fp.partition_version = partition_version
+    if ops is not None and ops.shape[0] >= 4:
+        fp._ops = np.ascontiguousarray(ops)
+        fp.ops = fp._ops.ctypes.data_as(u8p)
+        fp.ops_len = fp._ops.shape[0]
+    return fp
+
+
 class Engine:
     def __init__(self, device: int = -1, ctas_per_sm: int = 0, block_size: int = 0, restart_interval: int = 0):
         cfg = EngineConfig(device, block_size, restart_interval, ctas_per_sm, 0)
@@ -428,6 +452,23 @@ class Engine:
 
     def partition(self, app_id: int = 1, pidx: int = 0, data_version: int = 1) -> "Partition":
         return Partition(self, app_id, pidx, data_version)
+
+    def compact_many(self, jobs, now: int, flags: int = 0) -> list[CompactResult]:
+        """pgs_compact_many: the compactions of many partitions of this engine in one launch.  A job is (partition, run_ids,
+        out_level, bottommost, filter kwargs as Partition.compact takes them -- enabled, default_ttl, validate_hash, pidx,
+        partition_version, ops, data_version); returns one CompactResult per job."""
+        n = len(jobs)
+        arr = (CompactJob * max(1, n))()
+        keep = []  # the id arrays, filter params and ops tables must outlive the call
+        for i, (part, run_ids, out_level, bottommost, kw) in enumerate(jobs):
+            ids = np.array(list(run_ids), np.uint64)
+            fp = _filter_params(**(kw or {}))
+            keep += [ids, fp]
+            arr[i] = CompactJob(part.h.value if part is not None else None, ids.ctypes.data_as(u64p), ids.shape[0], out_level,
+                                bottommost, C.pointer(fp))
+        res = (CompactResult * max(1, n))()
+        _check(lib().pgs_compact_many(arr if n else None, n, now, flags, res), "compact_many")
+        return [res[i] for i in range(n)]
 
     def __enter__(self):
         return self

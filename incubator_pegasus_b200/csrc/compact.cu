@@ -23,6 +23,12 @@ int32_t compact_init_kernels(int max_smem)
     }
     PGS_CUDA(cudaFuncGetAttributes(&a, k_emit));
     PGS_CUDA(cudaFuncSetAttribute(k_emit, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem - (int)a.sharedSizeBytes));
+    for (uint32_t G : kWalkGs) {
+        PGS_CUDA(cudaFuncGetAttributes(&a, walk_many_kernel(G)));
+        PGS_CUDA(cudaFuncSetAttribute(walk_many_kernel(G), cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem - (int)a.sharedSizeBytes));
+    }
+    PGS_CUDA(cudaFuncGetAttributes(&a, k_emit_many));
+    PGS_CUDA(cudaFuncSetAttribute(k_emit_many, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem - (int)a.sharedSizeBytes));
     return PGS_OK;
 }
 } // namespace pgs
@@ -154,6 +160,228 @@ extern "C" int32_t pgs_compact_ex(pgs_partition *ph, const uint64_t *run_ids, ui
         }
     }
     if (out) *out = res;
+    return PGS_OK;
+}
+
+// ---- pgs_compact_many --------------------------------------------------------------------------------------------------------
+// The jobs of many partitions planned together (compact_many_geometry) and launched once (compact_launch_many).  The jobs'
+// scratch shares one allocation; each merged run keeps buffers of its own, as pgs_compact's does.
+extern "C" int32_t pgs_compact_many(const pgs_compact_job *jobs, uint32_t n, uint32_t now, uint32_t flags, pgs_compact_result *out)
+{
+    if (n == 0) return PGS_OK;
+    if (!jobs) { set_error("compact_many: %u jobs and no job array", n); return PGS_INVALID_ARGUMENT; }
+    if (n > kMaxCompactJobs) { set_error("compact_many: %u jobs > %u per call", n, kMaxCompactJobs); return PGS_NOT_SUPPORTED; }
+    Engine *e = nullptr;
+    std::vector<Partition *> parts(n);
+    for (uint32_t i = 0; i < n; i++) {
+        const pgs_compact_job &J = jobs[i];
+        if (!J.part || !J.run_ids || J.k == 0 || J.out_level < 0) {
+            set_error("compact_many: job %u: no partition, no runs or a negative output level", i);
+            return PGS_INVALID_ARGUMENT;
+        }
+        parts[i] = &J.part->p;
+        if (!e) e = parts[i]->eng;
+        if (parts[i]->eng != e) { set_error("compact_many: job %u: its partition is on another engine than job 0's", i); return PGS_INVALID_ARGUMENT; }
+    }
+    std::vector<Partition *> order = parts; // the install locks them in this order
+    std::sort(order.begin(), order.end());
+    for (uint32_t i = 1; i < n; i++)
+        if (order[i] == order[i - 1]) {
+            const uint32_t j = (uint32_t)(std::find(parts.begin(), parts.end(), order[i]) - parts.begin());
+            set_error("compact_many: job %u: its partition is in another job too", j);
+            return PGS_INVALID_ARGUMENT;
+        }
+
+    // the inputs and the bottommost rule of every job, as pgs_compact_ex finds them
+    std::vector<std::vector<std::shared_ptr<Run>>> in(n);
+    std::vector<int32_t> bottom(n);
+    for (uint32_t i = 0; i < n; i++) {
+        const pgs_compact_job &J = jobs[i];
+        Partition &part = *parts[i];
+        std::lock_guard<std::mutex> g(part.mu);
+        for (uint32_t x = 0; x < J.k; x++) {
+            auto r = part.find(J.run_ids[x]);
+            if (!r) { set_error("compact_many: job %u: unknown run %llu", i, (unsigned long long)J.run_ids[x]); return PGS_NOT_FOUND; }
+            for (auto &y : in[i])
+                if (y == r) { set_error("compact_many: job %u: run %llu given twice", i, (unsigned long long)J.run_ids[x]); return PGS_INVALID_ARGUMENT; }
+            in[i].push_back(r);
+        }
+        bottom[i] = J.bottommost;
+        if (bottom[i] < 0) {
+            size_t first_in = part.runs.size();
+            for (size_t x = 0; x < part.runs.size(); x++)
+                if (std::find(in[i].begin(), in[i].end(), part.runs[x]) != in[i].end()) { first_in = x; break; }
+            bottom[i] = 1;
+            for (size_t x = first_in; x < part.runs.size(); x++)
+                if (std::find(in[i].begin(), in[i].end(), part.runs[x]) == in[i].end()) bottom[i] = 0;
+        }
+    }
+    std::vector<MergeParams> P(n);
+    std::vector<CompactTotals> T(n);
+    std::vector<uint32_t> ops_len(n);
+    uint64_t ops_total = 0;
+    uint32_t any_hash = 0;
+    for (uint32_t i = 0; i < n; i++) {
+        const pgs_compact_job &J = jobs[i];
+        if (J.k > kMaxRuns) { set_error("compact_many: job %u: %u runs > %u per merge", i, J.k, kMaxRuns); return PGS_NOT_SUPPORTED; }
+        MergeParams &p = P[i];
+        p.k = J.k;
+        for (uint32_t x = 0; x < J.k; x++) {
+            p.runs[x] = in[i][x]->dev();
+            const pgs_run_info &fi = in[i][x]->info;
+            T[i].add(fi, in[i][x]->n_bloom_entries);
+            if (fi.n_blocks >= (1u << 28) || fi.data_bytes >= (1ull << 40)) { set_error("compact_many: job %u: a run too large for a merge", i); return PGS_NOT_SUPPORTED; }
+        }
+        if (T[i].max_ukey > kMaxUkeyLen) { set_error("compact_many: job %u: user key of %u bytes > %u", i, T[i].max_ukey, kMaxUkeyLen); return PGS_NOT_SUPPORTED; }
+        p.block_size = e->cfg.block_size;
+        p.restart_interval = e->cfg.restart_interval;
+        p.bottommost = bottom[i] ? 1 : 0;
+        p.now = now;
+        p.data_version = parts[i]->data_version;
+        if (!compact_filter(p, J.fp, ops_len[i])) { set_error("compact_many: job %u: malformed ops table of %u bytes", i, J.fp->ops_len); return PGS_INVALID_ARGUMENT; }
+        if (p.validate_hash) { p.crc_table = (const unsigned long long *)e->d_crc; any_hash = 1; }
+        ops_total += (ops_len[i] + 15) & ~15u;
+    }
+    MergeJobs M{};
+    CompactGeometry shared{};
+    std::vector<CompactGeometry> geo(n);
+    uint32_t force_G = 0; // diagnostics: PGS_WALK_G, as pgs_compact_ex
+    if (const char *ev = getenv("PGS_WALK_G")) { const int v = atoi(ev); if (v == 1 || v == 2 || v == 4 || v == 8 || v == 16) force_G = (uint32_t)v; }
+    const uint32_t smem = compact_smem_budget((uint32_t)e->max_smem_optin);
+    bool geo_ok = compact_many_geometry(P.data(), T.data(), geo.data(), n, smem, M, shared, force_G);
+    if (geo_ok) { // second pass: the segment weight follows from how many groups the device runs at once
+        int occ = 0;
+        PGS_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, walk_many_kernel(shared.G), (int)kWalkThreads, (size_t)shared.walk_dyn));
+        const uint64_t groups = (uint64_t)std::max(1, occ) * e->sm_count * (kWalkThreads / shared.G);
+        geo_ok = compact_many_geometry(P.data(), T.data(), geo.data(), n, smem, M, shared, shared.G, 0, groups);
+    }
+    if (!geo_ok) {
+        uint32_t widest = 0;
+        for (auto &t : T) widest = std::max(widest, t.max_ukey);
+        set_error("compact_many: %u jobs (user keys up to %u bytes) do not fit one merge launch; split the call", n, widest);
+        return PGS_NOT_SUPPORTED;
+    }
+
+    PGS_CUDA(cudaSetDevice(e->device));
+    cudaStream_t st = e->stream;
+    LaunchScratch S(st);
+    // the merged runs' buffers, one set per job; the scratch of every job is laid out in one allocation, grouped by fill byte
+    struct Slice { void **p; uint64_t bytes; int fill; };
+    std::vector<Slice> slices;
+    std::vector<std::shared_ptr<Run>> outr(n);
+    cudaError_t ce = cudaSuccess;
+    for (uint32_t i = 0; i < n; i++) {
+        outr[i] = std::make_shared<Run>(e);
+        outr[i]->level = jobs[i].out_level;
+        Run &r = *outr[i];
+        compact_buffers(P[i], geo[i], T[i], r, [&](auto *&p, uint64_t cnt, int fill, bool is_out) {
+            const size_t bytes = sizeof(*p) * cnt;
+            if (!is_out) { slices.push_back(Slice{(void **)&p, bytes, fill}); return; }
+            if (ce != cudaSuccess) return;
+            if ((void *)&p == (void *)&r.d_data) ce = e->alloc_data(r, bytes);
+            else ce = cudaMallocAsync((void **)&p, bytes, st); // ~Run frees the run's buffers
+            if (ce == cudaSuccess && fill != kNoFill) ce = cudaMemsetAsync(p, fill, bytes, st);
+        });
+    }
+    PGS_CUDA(ce);
+    slices.push_back(Slice{(void **)&M.ticket, 2 * sizeof(uint32_t), 0});
+    std::vector<int> fills;
+    for (auto &s : slices)
+        if (std::find(fills.begin(), fills.end(), s.fill) == fills.end()) fills.push_back(s.fill);
+    std::vector<uint64_t> offs(slices.size());
+    std::vector<std::pair<uint64_t, uint64_t>> fill_range(fills.size());
+    uint64_t arena_bytes = 0;
+    for (size_t f = 0; f < fills.size(); f++) {
+        fill_range[f].first = arena_bytes;
+        for (size_t x = 0; x < slices.size(); x++)
+            if (slices[x].fill == fills[f]) { offs[x] = arena_bytes; arena_bytes += (std::max<uint64_t>(slices[x].bytes, 16) + 255) & ~255ull; }
+        fill_range[f].second = arena_bytes;
+    }
+    uint8_t *arena = nullptr;
+    PGS_CUDA(S.alloc(arena, arena_bytes));
+    for (size_t f = 0; f < fills.size(); f++)
+        if (fills[f] != kNoFill) PGS_CUDA(cudaMemsetAsync(arena + fill_range[f].first, fills[f], fill_range[f].second - fill_range[f].first, st));
+    for (size_t x = 0; x < slices.size(); x++) *slices[x].p = arena + offs[x];
+
+    // the job table: MergeParams[n] | MergeStats[n] | seg_base[n + 1] | blk_base[n + 1] | the ops tables, in one upload
+    const uint64_t o_stats = sizeof(MergeParams) * (uint64_t)n, o_seg = (o_stats + sizeof(MergeStats) * (uint64_t)n + 15) & ~15ull;
+    const uint64_t o_blk = (o_seg + 4ull * (n + 1) + 15) & ~15ull, o_ops = (o_blk + 4ull * (n + 1) + 15) & ~15ull;
+    const uint64_t tab_bytes = o_ops + ops_total;
+    uint8_t *tab = nullptr;
+    PGS_CUDA(S.alloc(tab, tab_bytes));
+    std::vector<uint8_t> h(tab_bytes, 0);
+    uint64_t ops_at = o_ops;
+    for (uint32_t i = 0; i < n; i++) {
+        P[i].stats = (MergeStats *)(tab + o_stats) + i;
+        if (ops_len[i]) {
+            memcpy(h.data() + ops_at, jobs[i].fp->ops, ops_len[i]);
+            P[i].ops = tab + ops_at;
+            ops_at += (ops_len[i] + 15) & ~15u;
+        }
+        const MergeStats s0 = merge_stats_init();
+        memcpy(h.data() + o_stats + sizeof(MergeStats) * i, &s0, sizeof s0);
+    }
+    memcpy(h.data(), P.data(), sizeof(MergeParams) * (size_t)n);
+    compact_many_bases(P.data(), n, (uint32_t *)(h.data() + o_seg), (uint32_t *)(h.data() + o_blk));
+    PGS_CUDA(cudaMemcpyAsync(tab, h.data(), tab_bytes, cudaMemcpyHostToDevice, st));
+    M.job = (const MergeParams *)tab;
+    M.seg_base = (const uint32_t *)(tab + o_seg);
+    M.blk_base = (const uint32_t *)(tab + o_blk);
+    M.validate_hash = any_hash;
+    M.crc_table = (const unsigned long long *)e->d_crc;
+
+    cudaEvent_t ev[4];
+    for (auto &x : ev) PGS_CUDA(S.event(x));
+    int occ_w = 0, occ_e = 0;
+    PGS_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_w, walk_many_kernel(shared.G), (int)kWalkThreads, (size_t)shared.walk_dyn));
+    PGS_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_e, k_emit_many, (int)(shared.emit_warps * 32), (size_t)shared.emit_dyn));
+    const uint32_t launches = compact_launch_many(M, shared, (uint64_t)std::max(1, occ_w) * e->sm_count, (uint64_t)std::max(1, occ_e) * e->sm_count,
+                                                  st, [&](int i) { if (ce == cudaSuccess) ce = cudaEventRecord(ev[i], st); });
+    e->launches += launches;
+    PGS_CUDA(ce);
+    std::vector<MergeStats> hs(n);
+    PGS_CUDA(cudaMemcpyAsync(hs.data(), tab + o_stats, sizeof(MergeStats) * (size_t)n, cudaMemcpyDeviceToHost, st));
+    cudaError_t se = cudaStreamSynchronize(st);
+    if (se != cudaSuccess) return cuda_fail(se, "multi-job compaction kernels");
+    for (uint32_t i = 0; i < n; i++)
+        if (hs[i].error) {
+            set_error("compact_many: job %u: compaction kernel failed with status %u at segment %u of %u", i, hs[i].error, hs[i].error_seg, P[i].Q);
+            return (int32_t)hs[i].error;
+        }
+    float ms_total = 0, ms_merge = 0, ms_walk = 0, ms_emit = 0;
+    cudaEventElapsedTime(&ms_total, ev[0], ev[3]);
+    cudaEventElapsedTime(&ms_merge, ev[1], ev[3]);
+    cudaEventElapsedTime(&ms_walk, ev[1], ev[2]);
+    cudaEventElapsedTime(&ms_emit, ev[2], ev[3]);
+    std::vector<pgs_compact_result> res(n);
+    for (uint32_t i = 0; i < n; i++) {
+        outr[i]->n_bloom_entries = compact_result_stats(hs[i], T[i].in_block_bytes, res[i], outr[i]->info);
+        outr[i]->info.level = jobs[i].out_level;
+        res[i].n_tiles = P[i].Q; res[i].n_launches = launches;
+        res[i].device_ms = ms_total; res[i].merge_kernel_ms = ms_merge;
+        res[i].walk_ms = ms_walk; res[i].emit_ms = ms_emit;
+    }
+    // all partitions or none: every lock is held (in address order) from the check that the inputs are still there to the install
+    std::vector<std::unique_lock<std::mutex>> held;
+    for (Partition *p : order) held.emplace_back(p->mu);
+    for (uint32_t i = 0; i < n; i++)
+        for (auto &r : in[i])
+            if (std::find(parts[i]->runs.begin(), parts[i]->runs.end(), r) == parts[i]->runs.end()) {
+                set_error("compact_many: job %u: run %llu left the partition during the merge", i, (unsigned long long)r->id);
+                return PGS_ABORTED;
+            }
+    for (uint32_t i = 0; i < n; i++) {
+        Partition &part = *parts[i];
+        if (!(flags & PGS_COMPACT_KEEP_INPUTS))
+            for (auto &r : in[i]) part.runs.erase(std::find(part.runs.begin(), part.runs.end(), r));
+        if (hs[i].tot_blocks > 0 && !(flags & PGS_COMPACT_DISCARD_OUTPUT)) {
+            outr[i]->id = e->next_run_id++;
+            outr[i]->info.run_id = outr[i]->id;
+            part.insert(outr[i]);
+            res[i].new_run_id = outr[i]->id;
+        }
+    }
+    if (out) memcpy(out, res.data(), sizeof(pgs_compact_result) * (size_t)n);
     return PGS_OK;
 }
 

@@ -213,6 +213,15 @@ PGS_HD uint64_t walk_dyn_smem(uint32_t G, uint32_t group_smem, uint32_t k)
 {
     return walk_win_off(G, group_smem) + (uint64_t)(kWalkThreads / G) * walk_win_stride(k);
 }
+// k_walk_many (several jobs per launch) has no CTA-wide run table: a group reads its job's runs through the cache, and keeps
+// its counters in a WalkCtaStats of its own, which it hands to its job's MergeStats after every segment.  Its layout: crc table
+// (2 KB) | one WalkCtaStats per group | the groups' states and key rows | their head windows.
+PGS_HD uint32_t walk_many_fixed_smem(uint32_t G) { return 2048 + (kWalkThreads / G) * (uint32_t)sizeof(WalkCtaStats); }
+PGS_HD uint32_t walk_many_win_off(uint32_t G, uint32_t group_smem) { return (walk_many_fixed_smem(G) + (kWalkThreads / G) * group_smem + 15) & ~15u; }
+PGS_HD uint64_t walk_many_dyn_smem(uint32_t G, uint32_t group_smem, uint32_t k)
+{
+    return walk_many_win_off(G, group_smem) + (uint64_t)(kWalkThreads / G) * walk_win_stride(k);
+}
 // k_emit's shared memory per warp, every part 16-aligned: output buffer (ob) | key-stream stage (ks) | value stage (vs) | the
 // stages' mbarrier | restart offsets.  The 32 bytes behind each buffer take the whole 16-byte chunks read or written past its end.
 PGS_HD uint32_t emit_vs_off(uint32_t ob, uint32_t ks) { return ob + 32 + ks + 32; }
@@ -231,11 +240,15 @@ PGS_HD uint32_t emit_warp_layout(uint32_t bb, uint32_t RI, uint32_t ks, uint32_t
 // fills the derived fields of P (P.k, P.block_size, P.restart_interval must be set); false = not supported
 constexpr uint32_t kWalkMinG = 4; // default lanes per merge group (see group.cuh)
 // walk_groups = merge groups the device runs at the same time (0: not known yet, the default segment budget is used);
-// force_Q = the segment count of a plan made elsewhere (a partition split's child is emitted over its parent's segments)
+// force_Q = the segment count of a plan made elsewhere (a partition split's child is emitted over its parent's segments);
+// many = the shared memory of k_walk_many rather than k_walk's
 inline bool compact_geometry(MergeParams &P, const CompactTotals &T, uint32_t max_smem, CompactGeometry &geo, uint32_t force_G = 0,
-                             uint64_t force_weight = 0, uint64_t walk_groups = 0, uint32_t force_Q = 0)
+                             uint64_t force_weight = 0, uint64_t walk_groups = 0, uint32_t force_Q = 0, bool many = false)
 {
     const uint32_t k = P.k;
+    auto walk_dyn_smem = [many](uint32_t G, uint32_t group_smem, uint32_t k) {
+        return many ? walk_many_dyn_smem(G, group_smem, k) : pgs::walk_dyn_smem(G, group_smem, k);
+    };
     P.total_blocks = (uint32_t)T.total_blocks;
     P.KS = T.max_ukey < 4 ? 4u : ((T.max_ukey + 3) & ~3u);
     P.KSW = (P.KS + 8) / 4 + 1;
@@ -396,10 +409,9 @@ PGS_DEV unsigned long long run_weight(const RunDev &r, uint32_t pos, uint32_t re
     return r.blk_off[pos] + (unsigned long long)r.blk_rec[pos] * rec_cost;
 }
 
-__global__ void __launch_bounds__(256) k_plan(const __grid_constant__ MergeParams P)
+// input block gt (over all of P's runs, < P.total_blocks): the segment boundaries its last user key sets
+PGS_DEV void plan_block(const MergeParams &P, uint32_t gt)
 {
-    uint32_t gt = blockIdx.x * blockDim.x + threadIdx.x;
-    if (gt >= P.total_blocks) return;
     uint32_t i = 0, b = gt;
     while (b >= P.runs[i].nb) { b -= P.runs[i].nb; i++; }
     const RunDev &ri = P.runs[i];
@@ -443,6 +455,13 @@ __global__ void __launch_bounds__(256) k_plan(const __grid_constant__ MergeParam
     }
 }
 
+__global__ void __launch_bounds__(256) k_plan(const __grid_constant__ MergeParams P)
+{
+    uint32_t gt = blockIdx.x * blockDim.x + threadIdx.x;
+    if (gt >= P.total_blocks) return;
+    plan_block(P, gt);
+}
+
 // slice of run j that segment q may touch: blocks [lo, hi_ex); blocks >= chk may hold keys above the upper bound
 PGS_DEV bool seg_slice(const MergeParams &P, uint32_t q, uint32_t j, uint32_t &lo, uint32_t &hi_ex, uint32_t &chk)
 {
@@ -469,10 +488,8 @@ PGS_HD unsigned long long ks_bound(unsigned long long n_in, unsigned long long i
 // k_seg_bounds + k_seg_layout: where each segment's descriptor array and key stream live.  One thread per segment computes
 // the bounds of what it may emit (from its input slice); one CTA turns them into offsets with an exclusive scan.
 // ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) k_seg_bounds(const __grid_constant__ MergeParams P)
+PGS_DEV void seg_bound(const MergeParams &P, uint32_t q)
 {
-    const uint32_t q = blockIdx.x * blockDim.x + threadIdx.x;
-    if (q >= P.Q) return;
     unsigned long long n_in = 0, in_bytes = 0;
     bool ok = true;
     for (uint32_t j = 0; j < P.k; j++) {
@@ -485,8 +502,15 @@ __global__ void __launch_bounds__(256) k_seg_bounds(const __grid_constant__ Merg
     P.seg[q].desc_off = n_in;
     P.seg[q].ks_off = ks_bound(n_in, in_bytes, P.KS, P.block_size);
 }
+__global__ void __launch_bounds__(256) k_seg_bounds(const __grid_constant__ MergeParams P)
+{
+    const uint32_t q = blockIdx.x * blockDim.x + threadIdx.x;
+    if (q >= P.Q) return;
+    seg_bound(P, q);
+}
 
-__global__ void __launch_bounds__(1024) k_seg_layout(const __grid_constant__ MergeParams P)
+// the whole CTA: P's segment bounds become offsets
+PGS_DEV void seg_layout(const MergeParams &P)
 {
     uint32_t q0, q1;
     unsigned long long pre[2], tot[2];
@@ -500,6 +524,7 @@ __global__ void __launch_bounds__(1024) k_seg_layout(const __grid_constant__ Mer
         pre[1] += b;
     }
 }
+__global__ void __launch_bounds__(1024) k_seg_layout(const __grid_constant__ MergeParams P) { seg_layout(P); }
 
 // ------------------------------------------------------------------------------------------------
 // compaction filter on the device
@@ -640,9 +665,12 @@ PGS_DEV unsigned long long adj_head_to(unsigned long long a, uint32_t pos, uint3
 
 // One segment per group, all groups of the warp in lock step (see group.cuh): every statement outside an `if (en...)` body is
 // executed by all 32 lanes; `act` marks the groups that still have records.
-template <uint32_t G>
+// MANY: the groups of a warp may walk segments of different jobs (k_walk_many), whose run counts differ; the cursors are
+// opened in a loop of k_open (warp-uniform, at least every group's P.k) steps, and a group takes part in those past its P.k
+// with nothing enabled.
+template <uint32_t G, bool MANY = false>
 PGS_DEV void walk_segment(const MergeParams &P, const RunDev *runs, const Grp<G> &g, bool seg_en, uint32_t q, CurState *cs, uint32_t *rows,
-                          uint8_t *wins, const unsigned long long *crc, WalkAcc &acc, WalkCtaStats *cta)
+                          uint8_t *wins, const unsigned long long *crc, WalkAcc &acc, WalkCtaStats *cta, uint32_t k_open = 0)
 {
     const uint32_t k = P.k, KS = P.KS, KSW = P.KSW, RI = P.restart_interval, BS = P.block_size;
     uint32_t *rowA = rows + k * KSW, *rowB = rowA + KSW, *rowLO = rowB + KSW, *rowHI = rowLO + KSW;
@@ -673,8 +701,9 @@ PGS_DEV void walk_segment(const MergeParams &P, const RunDev *runs, const Grp<G>
     unsigned long long order = 0; // entries 0..live-1: the group's runs in merge order
     uint32_t dpos = 0;
 #pragma unroll 1
-    for (uint32_t j = 0; j < k; j++) {
-        const bool en = seg_en && !err;
+    for (uint32_t j = 0; j < (MANY ? k_open : k); j++) {
+        const bool run_en = seg_en && (!MANY || j < k); // (a group past its own runs takes part with nothing enabled)
+        const bool en = run_en && !err;
         uint32_t lo = 0, hi_ex = 0, chk = 0;
         if (en && !seg_slice(P, q, j, lo, hi_ex, chk)) err = PGS_ABORTED;
         CurState *C = &cs[j];
@@ -683,20 +712,20 @@ PGS_DEV void walk_segment(const MergeParams &P, const RunDev *runs, const Grp<G>
         if (en && !err) err = e1;
 #pragma unroll 1
         for (;;) { // records at or below U_lo belong to the previous segment
-            const bool sk = seg_en && !err && !first && C->live;
+            const bool sk = run_en && !err && !first && C->live;
             const int c = row_cmp(g, sk, row, sk ? C->klen - 8 : 0u, rowLO, ulo_len, dpos);
             const bool more = sk && c <= 0;
             if (!g.any(more)) break;
             const uint32_t e2 = cur_next<G, true>(g, more, runs[j], C, row, KS, wins + j * kHeadWin);
             if (more) err = e2;
         }
-        const bool hi = seg_en && !err && C->live && !last && C->b >= C->chk_from;
+        const bool hi = run_en && !err && C->live && !last && C->b >= C->chk_from;
         const int ch = row_cmp(g, hi, row, hi ? C->klen - 8 : 0u, rowHI, uhi_len, dpos);
         g.sync();
         if (hi && ch > 0 && g.gl == 0) C->live = 0;
         g.sync();
         // insert into the order
-        const bool ins = seg_en && !err && C->live;
+        const bool ins = run_en && !err && C->live;
         uint32_t pos = live;
         bool searching = ins;
 #pragma unroll 1
@@ -1023,6 +1052,35 @@ __global__ void __launch_bounds__(kWalkThreads, 4) k_walk(const __grid_constant_
 // k_seg_scan: one CTA; exclusive prefixes of the segments' output sizes, totals, index sentinels
 // ------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(1024) k_seg_scan(const __grid_constant__ MergeParams P)
+{
+    uint32_t q0, q1;
+    unsigned long long pre[4], tot[4];
+    cta_excl_scan<4>(P.Q, [&](uint32_t q, unsigned long long (&v)[4]) {
+        const SegAgg a = P.agg[q];
+        v[0] += a.out_bytes; v[1] += a.n_blocks; v[2] += a.n_entries; v[3] += a.keyb;
+    }, q0, q1, pre, tot);
+    const uint32_t tid = threadIdx.x;
+    for (uint32_t q = q0; q < q1; q++) {
+        const SegAgg a = P.agg[q];
+        SegBase b;
+        b.bytes = pre[0]; b.blocks = (uint32_t)pre[1]; b.recs = (uint32_t)pre[2]; b.keyb = (uint32_t)pre[3]; b.pad = 0;
+        P.base[q] = b;
+        pre[0] += a.out_bytes; pre[1] += a.n_blocks; pre[2] += a.n_entries; pre[3] += a.keyb;
+    }
+    if (tid == 0) {
+        P.stats->tot_bytes = tot[0]; P.stats->tot_blocks = tot[1]; P.stats->tot_recs = tot[2]; P.stats->tot_keyb = tot[3];
+        if (tot[0] > P.out_cap || tot[1] > P.out_blk_cap || tot[2] > P.out_rec_cap || tot[3] > P.out_ikey_cap) {
+            atomicMax(&P.stats->error, (uint32_t)PGS_ABORTED);
+        } else { // sentinels of the new run's index
+            P.out_blk_off[tot[1]] = tot[0];
+            P.out_blk_rec[tot[1]] = (uint32_t)tot[2];
+            P.out_ikey_off[tot[1]] = (uint32_t)tot[3];
+        }
+    }
+}
+// k_seg_scan's body for one job of a multi-job launch (k_seg_scan_many), by the whole CTA.  k_seg_scan keeps its own copy of
+// these lines: moved into a function they schedule differently, and the single-partition kernels keep their machine code.
+PGS_DEV void seg_scan(const MergeParams &P)
 {
     uint32_t q0, q1;
     unsigned long long pre[4], tot[4];
@@ -1520,6 +1578,43 @@ PGS_DEV void carry_over(const MergeParams &P, EmitSeg &S, const EmitWarp &W, con
     S.cv = lane < S.carry ? W.obuf[whole + lane] : (uint8_t)0;
 }
 
+// segment q of P, by the whole warp: its blocks, index entries and Bloom filter bits.  This is k_emit's loop body, which k_emit
+// keeps written out for the same reason as k_seg_scan (k_emit_many calls this one).
+PGS_DEV void emit_segment(const MergeParams &P, EmitWarp &W, uint32_t q)
+{
+    const uint32_t lane = W.lane;
+    const SegAgg A = P.agg[q];
+    if (A.n_entries == 0) return;
+    const SegBase B = P.base[q];
+    EmitSeg S;
+    emit_seg(S, P, q, A, B);
+    uint32_t err = 0;
+    uint4 dn = make_uint4(0u, 0u, 0u, 0u); // the next batch's descriptors, fetched while this batch's values are copied
+    uint32_t dn_e0 = 0xFFFFFFFFu;
+    for (uint32_t e0 = 0; e0 < S.n && !err;) {
+        EmitBatch b;
+        batch_desc(b, S, W, e0, dn, dn_e0);
+        const uint32_t first_fl = __shfl_sync(kFull, b.fl, 0);
+        if (first_fl & DF_BIG) { emit_big(P, S, W, b, first_fl); e0++; continue; }
+        if (batch_fit(P, S, W, b) == 0) { err = PGS_ABORTED; break; }
+        stage_batch(P, S, W, b, e0, dn, dn_e0);
+        batch_offsets(P, S, W, b);
+        mbar_wait(W.bar, W.phase); // the one wait of a batch for global memory
+        W.phase ^= 1;
+        b.staged = W.stage + ((uintptr_t)(S.ks + S.kpos) & 15);
+        obuf_reclaim(S, W);
+        restart_points(P, S, W, b);
+        write_entries(P, W, b);
+        __syncwarp();
+        close_blocks(P, S, W, b);
+        carry_over(P, S, W, b);
+        e0 += b.cnt;
+    }
+    if (!err && S.open) finish_open(P, S, W); // the segment's last block
+    if (!err && (S.blk_start != B.bytes + A.out_bytes || S.blk_idx != B.blocks + A.n_blocks || S.keyb != B.keyb + A.keyb)) err = PGS_CORRUPTION; // the two passes disagree
+    if (err && lane == 0) { atomicMax(&P.stats->error, err); atomicMin(&P.stats->error_seg, q); }
+}
+
 // three CTAs per SM: what shared memory allows with an 8 KB output buffer and an 8 KB value stage per warp
 __global__ void __launch_bounds__(kEmitThreads, 3) k_emit(const __grid_constant__ MergeParams P)
 {
@@ -1605,6 +1700,244 @@ inline uint32_t compact_launch(const MergeParams &P, const CompactGeometry &geo,
     mark(2);
     PGS_LAUNCH(k_seg_scan, 1, 1024, 0, st, P);
     PGS_LAUNCH(k_emit, grid_e, geo.emit_warps * 32, geo.emit_dyn, st, P);
+    mark(3);
+    return 6;
+}
+
+// ================================================================================================================================
+// Several compactions in one launch (pgs_compact_many): the jobs of many partitions of one engine share one plan and one set of
+// six launches.  Every job keeps its own MergeParams -- runs, policy and filter, scratch, output run, MergeStats -- in device
+// memory; the launch numbers the jobs' segments one after the other (job j owns the launch's segments [seg_base[j],
+// seg_base[j + 1])) and k_plan's threads likewise over the jobs' input blocks.  A kernel maps its global index to (job, local
+// index) with job_of and runs the single-job code on that job's parameters: k_plan, k_seg_bounds and k_walk's segment walk are
+// the same device functions as in the single launch, k_seg_layout and k_seg_scan give every job a CTA of its own, k_emit's
+// warps draw global segments.  What the jobs share is the launch's shape: the widest user key sizes every job's key rows and
+// k_emit's stages, the deepest job sizes the groups' cursor states, and one segment weight cuts every job (compact_many_geometry).
+// ================================================================================================================================
+constexpr uint32_t kMaxCompactJobs = 4096; // jobs of one multi-job launch
+
+struct MergeJobs {
+    const MergeParams *job;   // [n] in device memory
+    const uint32_t *seg_base; // [n + 1]: job j's segments are the launch's segments [seg_base[j], seg_base[j + 1])
+    const uint32_t *blk_base; // [n + 1]: job j's input blocks are k_plan's threads [blk_base[j], blk_base[j + 1])
+    uint32_t n, Q, total_blocks;
+    uint32_t k_max;           // the deepest job: every group's cursor states and head windows are sized for it
+    uint32_t group_smem;      // one group's shared memory (every job's P.group_smem)
+    uint32_t validate_hash;   // some job checks partition hashes: k_walk_many loads the crc table
+    const unsigned long long *crc_table;
+    uint32_t *ticket;         // [0] k_walk_many, [1] k_emit_many
+};
+
+// the job whose range [base[j], base[j + 1]) holds x (base[0] = 0 <= x < base[n]; empty ranges are skipped)
+PGS_HD uint32_t job_of(const uint32_t *base, uint32_t n, uint32_t x)
+{
+    uint32_t lo = 0, hi = n; // base[lo] <= x < base[hi]
+    while (hi - lo > 1) {
+        const uint32_t mid = (lo + hi) >> 1;
+        if (base[mid] <= x) lo = mid; else hi = mid;
+    }
+    return lo;
+}
+
+__global__ void __launch_bounds__(256) k_plan_many(const __grid_constant__ MergeJobs M)
+{
+    const uint32_t gt = blockIdx.x * blockDim.x + threadIdx.x;
+    if (gt >= M.total_blocks) return;
+    const uint32_t j = job_of(M.blk_base, M.n, gt);
+    plan_block(M.job[j], gt - M.blk_base[j]); // ranked against its own job's runs, cut by the launch's one segment weight
+}
+
+__global__ void __launch_bounds__(256) k_seg_bounds_many(const __grid_constant__ MergeJobs M)
+{
+    const uint32_t q = blockIdx.x * blockDim.x + threadIdx.x;
+    if (q >= M.Q) return;
+    const uint32_t j = job_of(M.seg_base, M.n, q);
+    seg_bound(M.job[j], q - M.seg_base[j]);
+}
+
+// one CTA per job: a segmented scan of the launch's segment list, each job's offsets from its own scratch's start
+__global__ void __launch_bounds__(1024) k_seg_layout_many(const __grid_constant__ MergeJobs M) { seg_layout(M.job[blockIdx.x]); }
+__global__ void __launch_bounds__(1024) k_seg_scan_many(const __grid_constant__ MergeJobs M) { seg_scan(M.job[blockIdx.x]); }
+
+// A group's counters after a segment of a multi-job launch go to that segment's job: the events it kept in gst (its own
+// WalkCtaStats, only its lane 0 touches it) and in acc, the byte sums and maxima in acc.  acc and gst start over.
+PGS_DEV void walk_stats_flush(WalkAcc &acc, WalkCtaStats *gst, MergeStats *st, bool lane0)
+{
+    acc_flush_events(acc, gst, lane0);
+    if (lane0) {
+        for (uint32_t i = 0; i < 12; i++)
+            if (gst->cnt[i]) { atomicAdd(&st->cnt[i], (unsigned long long)gst->cnt[i]); gst->cnt[i] = 0; }
+        if (acc.b_in) atomicAdd(&st->bytes[SB_IN], acc.b_in);
+        if (acc.b_key + acc.b_val) atomicAdd(&st->bytes[SB_OUT], acc.b_key + acc.b_val);
+        if (acc.b_key) atomicAdd(&st->bytes[SB_OUT_KEY], acc.b_key);
+        if (acc.b_val) atomicAdd(&st->bytes[SB_OUT_VAL], acc.b_val);
+        if (acc.m_ukey) atomicMax(&st->mx[SM_UKEY], (unsigned long long)acc.m_ukey);
+        if (acc.m_vlen) atomicMax(&st->mx[SM_VLEN], (unsigned long long)acc.m_vlen);
+        if (acc.m_seq) atomicMax(&st->mx[SM_MAX_SEQ], acc.m_seq);
+        if (acc.m_seq_inv) atomicMax(&st->mx[SM_MIN_SEQ_INV], acc.m_seq_inv);
+        if (acc.m_bsize) atomicMax(&st->mx[SM_BLK_SIZE], (unsigned long long)acc.m_bsize);
+        if (acc.m_brec) atomicMax(&st->mx[SM_BLK_REC], (unsigned long long)acc.m_brec);
+    }
+    acc.b_in = acc.b_key = acc.b_val = 0;
+    acc.m_ukey = acc.m_vlen = acc.m_bsize = acc.m_brec = 0;
+    acc.m_seq = acc.m_seq_inv = 0;
+}
+
+// k_walk over the segments of every job.  The groups of a warp may draw segments of different jobs, so there is no CTA-wide
+// run table: a group reads its job's run table (MergeParams::runs) through the L1 cache -- a few hundred bytes per job, the
+// same lines for the whole segment -- where k_walk copies its one table into shared memory.
+template <uint32_t G>
+__global__ void __launch_bounds__(kWalkThreads, 4) k_walk_many(const __grid_constant__ MergeJobs M)
+{
+    PGS_SMEM_DYN(dyn);
+    const Grp<G> g;
+    constexpr uint32_t NGW = 32 / G; // groups per warp
+    const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const uint32_t gi = warp * NGW + g.shift / G; // the group inside the CTA
+    unsigned long long *crc = (unsigned long long *)dyn;
+    WalkCtaStats *gst = (WalkCtaStats *)(dyn + 2048) + gi;
+    if (M.validate_hash)
+        for (uint32_t i = threadIdx.x; i < 256; i += blockDim.x) crc[i] = M.crc_table[i];
+    for (uint32_t i = g.gl; i < sizeof(WalkCtaStats) / 4; i += G) ((uint32_t *)gst)[i] = 0;
+    __syncthreads();
+    uint8_t *gs = dyn + walk_many_fixed_smem(G) + (size_t)gi * M.group_smem;
+    CurState *cs = (CurState *)gs;
+    uint32_t *rows = (uint32_t *)(gs + (size_t)M.k_max * sizeof(CurState));
+    uint8_t *wins = dyn + walk_many_win_off(G, M.group_smem) + (size_t)gi * walk_win_stride(M.k_max);
+    WalkAcc acc;
+    acc.e0 = acc.e1 = acc.e2 = acc.n = 0;
+    acc.b_in = acc.b_key = acc.b_val = 0;
+    acc.m_ukey = acc.m_vlen = acc.m_bsize = acc.m_brec = 0;
+    acc.m_seq = acc.m_seq_inv = 0;
+#pragma unroll 1
+    for (;;) {
+        uint32_t t0 = 0;
+        if (lane == 0) t0 = atomicAdd(M.ticket, NGW);
+        t0 = __shfl_sync(kFull, t0, 0);
+        if (t0 >= M.Q) break;
+        const uint32_t q = t0 + g.shift / G;
+        const uint32_t j = q < M.Q ? job_of(M.seg_base, M.n, q) : 0u;
+        const MergeParams &P = M.job[j];
+        // a job whose plan failed is not walked (its output is discarded); one lane reads the flag for the whole group
+        const uint32_t failed = g.shfl(g.gl == 0 ? P.stats->error : 0u, 0);
+        const bool en = q < M.Q && failed == 0;
+        walk_segment<G, true>(P, P.runs, g, en, en ? q - M.seg_base[j] : 0u, cs, rows, wins, crc, acc, gst, M.k_max);
+        walk_stats_flush(acc, gst, P.stats, en && g.gl == 0);
+    }
+}
+
+// k_emit over the segments of every job: a warp draws global segments and writes each into its own job's run, index and
+// Bloom filter; the filter counts go to that job's MergeStats after every segment
+__global__ void __launch_bounds__(kEmitThreads, 3) k_emit_many(const __grid_constant__ MergeJobs M)
+{
+    PGS_SMEM_DYN(dyn);
+    const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const MergeParams &P0 = M.job[0]; // the stages' layout is the launch's, the same in every job
+    EmitWarp W;
+    emit_warp(W, P0, dyn + (size_t)warp * P0.emit_warp_smem, lane);
+    for (;;) {
+        uint32_t t = 0;
+        if (lane == 0) t = atomicAdd(M.ticket + 1, 1u);
+        t = __shfl_sync(kFull, t, 0);
+        if (t >= M.Q) break;
+        const uint32_t j = job_of(M.seg_base, M.n, t);
+        const MergeParams &P = M.job[j];
+        if (__shfl_sync(kFull, lane == 0 ? P.stats->error : 0u, 0)) continue; // its plan or walk failed: discarded
+        emit_segment(P, W, t - M.seg_base[j]);
+        if (lane == 0) {
+            if (W.n_bloom_keys) atomicAdd(&P.stats->cnt[EV_BLOOM_KEY], (unsigned long long)W.n_bloom_keys);
+            if (W.n_bloom_prefixes) atomicAdd(&P.stats->cnt[EV_BLOOM_PREFIX], (unsigned long long)W.n_bloom_prefixes);
+        }
+        W.n_bloom_keys = W.n_bloom_prefixes = 0;
+    }
+    if (lane == 0) tma_store_wait_all();
+}
+
+typedef void (*walk_many_kernel_t)(const MergeJobs);
+inline walk_many_kernel_t walk_many_kernel(uint32_t G)
+{
+    switch (G) {
+    case 1: return k_walk_many<1>;
+    case 2: return k_walk_many<2>;
+    case 4: return k_walk_many<4>;
+    case 8: return k_walk_many<8>;
+    default: return k_walk_many<16>;
+    }
+}
+
+// The joint plan of n jobs (host side).  P[i] holds job i's k, runs, block_size, restart_interval, policy and filter fields,
+// T[i] its totals.  The widest user key sizes every job's key rows and k_emit's stages, the deepest job every group's cursor
+// states, and one segment weight is sized from the whole launch's weight (walk_groups and force_* as in compact_geometry).
+// Then every job gets its own segments and output bounds (geo[i]); shared = the launch's walk and emit shape.  M gets the
+// launch's counts and shape, no pointers.  false: the jobs do not fit one launch (the caller can split them).
+inline bool compact_many_geometry(MergeParams *P, const CompactTotals *T, CompactGeometry *geo, uint32_t n, uint32_t max_smem,
+                                  MergeJobs &M, CompactGeometry &shared, uint32_t force_G = 0, uint64_t force_weight = 0,
+                                  uint64_t walk_groups = 0)
+{
+    if (n == 0 || n > kMaxCompactJobs) return false;
+    CompactTotals J{};
+    uint32_t k_max = 0;
+    for (uint32_t i = 0; i < n; i++) {
+        J.max_ukey = std::max(J.max_ukey, T[i].max_ukey);
+        J.max_blk = std::max(J.max_blk, T[i].max_blk);
+        J.max_blk_rec = std::max(J.max_blk_rec, T[i].max_blk_rec);
+        J.total_blocks += T[i].total_blocks;
+        J.n_rec += T[i].n_rec;
+        J.raw_key += T[i].raw_key;
+        J.raw_val += T[i].raw_val;
+        J.in_block_bytes += T[i].in_block_bytes;
+        J.bloom_entries += T[i].bloom_entries;
+        k_max = std::max(k_max, P[i].k);
+    }
+    MergeParams L = P[0];
+    L.k = k_max;
+    if (!compact_geometry(L, J, max_smem, shared, force_G, force_weight, walk_groups, 0, true)) return false;
+    uint64_t Q = 0, blocks = 0;
+    for (uint32_t i = 0; i < n; i++) {
+        CompactTotals t = T[i];
+        t.max_ukey = J.max_ukey; // the key rows of the widest key
+        if (!compact_geometry(P[i], t, max_smem, geo[i], shared.G, L.tile_weight, 0, 0, true)) return false;
+        if (P[i].KS != L.KS || P[i].blk_buf != L.blk_buf || P[i].emit_warp_smem != L.emit_warp_smem || P[i].block_size != L.block_size) return false;
+        P[i].group_smem = L.group_smem;
+        Q += P[i].Q;
+        blocks += P[i].total_blocks;
+    }
+    if (Q > 0x7FFFFFF0ull || blocks > 0xFFFFFFF0ull) return false;
+    M.n = n;
+    M.Q = (uint32_t)Q;
+    M.total_blocks = (uint32_t)blocks;
+    M.k_max = k_max;
+    M.group_smem = L.group_smem;
+    return true;
+}
+// the exclusive prefixes of the jobs' segments and input blocks (n + 1 entries each)
+inline void compact_many_bases(const MergeParams *P, uint32_t n, uint32_t *seg_base, uint32_t *blk_base)
+{
+    seg_base[0] = blk_base[0] = 0;
+    for (uint32_t i = 0; i < n; i++) {
+        seg_base[i + 1] = seg_base[i] + P[i].Q;
+        blk_base[i + 1] = blk_base[i] + P[i].total_blocks;
+    }
+}
+
+// The six kernels of a multi-job compaction on stream st, as compact_launch (the same marks, the same launch count).
+template <class Mark>
+inline uint32_t compact_launch_many(const MergeJobs &M, const CompactGeometry &geo, uint64_t walk_ctas, uint64_t emit_ctas, cudaStream_t st,
+                                    Mark &&mark)
+{
+    const walk_many_kernel_t walk = walk_many_kernel(geo.G);
+    const uint32_t seg_per_cta = kWalkThreads / geo.G;
+    const uint32_t grid_w = (uint32_t)std::min<uint64_t>((M.Q + seg_per_cta - 1) / seg_per_cta, walk_ctas);
+    const uint32_t grid_e = (uint32_t)std::min<uint64_t>((M.Q + geo.emit_warps - 1) / geo.emit_warps, emit_ctas);
+    mark(0);
+    PGS_LAUNCH(k_plan_many, std::max(1ull, (M.total_blocks + 255ull) / 256), 256, 0, st, M);
+    PGS_LAUNCH(k_seg_bounds_many, (M.Q + 255ull) / 256, 256, 0, st, M);
+    PGS_LAUNCH(k_seg_layout_many, M.n, 1024, 0, st, M);
+    mark(1);
+    PGS_LAUNCH(walk, grid_w, kWalkThreads, geo.walk_dyn, st, M);
+    mark(2);
+    PGS_LAUNCH(k_seg_scan_many, M.n, 1024, 0, st, M);
+    PGS_LAUNCH(k_emit_many, grid_e, geo.emit_warps * 32, geo.emit_dyn, st, M);
     mark(3);
     return 6;
 }

@@ -1043,6 +1043,60 @@ int32_t pgs_rrdb_manual_compact(pgs_server *h, uint32_t now, pgs_compact_result 
     if (st == PGS_OK) h->s.manual_compact_last_finish_ms = ((uint64_t)now + kEpochBegin) * 1000;
     return st;
 }
+// The same manual-compaction decision on many replicas (the app envs reach every replica of the app at once): each replica is
+// prepared as do_manual_compact prepares it, and the merges go to the GPU in one pgs_compact_many.
+int32_t pgs_rrdb_manual_compact_many(pgs_server *const *servers, uint32_t n, uint32_t now, pgs_compact_result *out)
+{
+    if (n == 0) return PGS_OK;
+    if (!servers) return PGS_INVALID_ARGUMENT;
+    std::vector<Server *> order;
+    for (uint32_t i = 0; i < n; i++) {
+        if (!servers[i]) return PGS_INVALID_ARGUMENT;
+        if (servers[i]->s.part->p.eng != servers[0]->s.part->p.eng) {
+            set_error("rrdb_manual_compact_many: replica %u is on another engine than replica 0", i);
+            return PGS_INVALID_ARGUMENT;
+        }
+        order.push_back(&servers[i]->s);
+    }
+    std::sort(order.begin(), order.end());
+    if (std::adjacent_find(order.begin(), order.end()) != order.end()) {
+        set_error("rrdb_manual_compact_many: a replica given twice");
+        return PGS_INVALID_ARGUMENT;
+    }
+    std::vector<std::unique_lock<std::shared_mutex>> held;
+    for (Server *s : order) held.emplace_back(s->mu);
+    if (out) memset(out, 0, sizeof(pgs_compact_result) * (size_t)n);
+    // do_manual_compact's preparation per replica: flush, fold a stack deeper than one merge, the level of the merge
+    std::vector<std::vector<uint64_t>> ids(n);
+    std::vector<pgs_filter_params> fps(n);
+    std::vector<pgs_compact_job> jobs;
+    std::vector<uint32_t> which; // the replica of each job (a replica without runs has none)
+    for (uint32_t i = 0; i < n; i++) {
+        Server &s = servers[i]->s;
+        if (const int32_t st = s.flush_mem()) return st;
+        auto rs = s.runs();
+        if (rs.empty()) continue;
+        int32_t level = 1;
+        for (auto &r : rs) { level = std::max(level, r->level); ids[i].push_back(r->id); }
+        while (ids[i].size() > kMaxRuns) {
+            std::vector<uint64_t> tail(ids[i].end() - kMaxRuns, ids[i].end());
+            pgs_filter_params fp = s.filter();
+            pgs_compact_result cr{};
+            if (const int32_t st = pgs_compact(s.part, tail.data(), kMaxRuns, level, 1, &fp, now, &cr)) return st;
+            ids[i].resize(ids[i].size() - kMaxRuns);
+            if (cr.new_run_id) ids[i].push_back(cr.new_run_id);
+        }
+        fps[i] = s.filter();
+        jobs.push_back(pgs_compact_job{s.part, ids[i].data(), (uint32_t)ids[i].size(), level, 1, &fps[i]});
+        which.push_back(i);
+    }
+    std::vector<pgs_compact_result> res(jobs.size());
+    if (const int32_t st = pgs_compact_many(jobs.data(), (uint32_t)jobs.size(), now, 0, res.data())) return st;
+    for (uint32_t i = 0; i < n; i++) servers[i]->s.manual_compact_last_finish_ms = ((uint64_t)now + kEpochBegin) * 1000;
+    if (out)
+        for (size_t j = 0; j < jobs.size(); j++) out[which[j]] = res[j];
+    return PGS_OK;
+}
 // ---- checkpoints (pegasus_server_impl.cpp:1951-2336: sync_checkpoint, get_checkpoint, storage_apply_checkpoint) ---------------
 // The directory protocol (temporary name, MANIFEST last, rename) lives in checkpoint_dir.h.
 int32_t pgs_rrdb_sync_checkpoint(pgs_server *h, const char *dir, uint32_t now, int64_t *decree_out)

@@ -148,6 +148,8 @@ struct Merged { // the output of the last sim_compact call
     uint32_t Q = 0;
 } g_res;
 
+std::vector<Merged> g_many; // the outputs of the last sim_compact_many call, one per job
+
 struct Built { // the run of the last sim_run_build call
     HostRun run;
     uint64_t data_bytes = 0;
@@ -210,6 +212,90 @@ int32_t sim_compact(uint32_t k, const uint8_t **data, const uint64_t *data_bytes
     R.st = st;
     R.Q = P.Q;
     if (st.error) { fprintf(stderr, "sim_compact: status %u at segment %u of %u\n", st.error, st.error_seg, P.Q); return (int32_t)st.error; }
+    return PGS_OK;
+}
+
+// n jobs through compact_many_geometry / compact_buffers / compact_launch_many, as pgs_compact_many runs them.  Job i merges
+// k[i] runs, taken in order from the flat run arrays; bottommost[i] and fp[i] are its policy and filter.  group_lanes and
+// seg_weight as sim_compact (seg_weight: the launch's one segment weight).  Returns a status; *launches = the launches made.
+// Every job's output stays until the next call: sim_compact_many_select(i) makes job i's the one sim_result_* read.
+int32_t sim_compact_many(uint32_t n, const uint32_t *k, const uint8_t **data, const uint64_t *data_bytes, const uint64_t **blk_off,
+                         const uint32_t **blk_size, const uint32_t *n_blocks, uint32_t block_size, uint32_t restart_interval,
+                         const int32_t *bottommost, const pgs_filter_params *fp, uint32_t now, uint32_t group_lanes, uint64_t seg_weight,
+                         uint32_t *launches)
+{
+    g_many.clear();
+    *launches = 0;
+    uint32_t total = 0;
+    for (uint32_t i = 0; i < n; i++) total += k[i];
+    std::vector<HostRun> runs(total);
+    for (uint32_t i = 0; i < total; i++)
+        if (const int32_t rc = load_run(runs[i], data[i], data_bytes[i], blk_off[i], blk_size[i], n_blocks[i])) return rc;
+    if (group_lanes && group_lanes != 1 && group_lanes != 2 && group_lanes != 4 && group_lanes != 8 && group_lanes != 16) return PGS_INVALID_ARGUMENT;
+    crc64_make_table(crc_tab);
+    HostMem scratch;
+    std::vector<MergeParams> P(n);
+    std::vector<CompactTotals> T(n);
+    uint32_t any_hash = 0;
+    for (uint32_t i = 0, r = 0; i < n; r += k[i], i++) {
+        if (k[i] == 0) return PGS_INVALID_ARGUMENT;
+        if (k[i] > kMaxRuns) return PGS_NOT_SUPPORTED;
+        P[i].k = k[i];
+        for (uint32_t x = 0; x < k[i]; x++) {
+            P[i].runs[x] = runs[r + x].dev();
+            T[i].add(runs[r + x].info, runs[r + x].n_bloom_entries);
+        }
+        P[i].block_size = block_size;
+        P[i].restart_interval = restart_interval;
+        P[i].bottommost = bottommost[i] ? 1 : 0;
+        P[i].now = now;
+        P[i].data_version = fp[i].data_version;
+        uint32_t len = 0;
+        if (!compact_filter(P[i], &fp[i], len)) return PGS_INVALID_ARGUMENT;
+        if (len) {
+            uint8_t *ops;
+            memcpy(host_alloc(scratch, ops, len, 0), fp[i].ops, len);
+            P[i].ops = ops;
+        }
+        if (P[i].validate_hash) { P[i].crc_table = (const unsigned long long *)crc_tab; any_hash = 1; }
+    }
+    MergeJobs M{};
+    CompactGeometry shared{};
+    std::vector<CompactGeometry> geo(n);
+    if (!compact_many_geometry(P.data(), T.data(), geo.data(), n, compact_smem_budget(kSimSmemOptin), M, shared, group_lanes, seg_weight))
+        return PGS_NOT_SUPPORTED;
+    g_many.resize(n);
+    std::vector<MergeStats> st(n, merge_stats_init());
+    for (uint32_t i = 0; i < n; i++) {
+        HostRun &run = g_many[i].run;
+        compact_buffers(P[i], geo[i], T[i], run, [&](auto *&p, uint64_t cnt, int fill, bool out) { host_count_buffers(out ? run.mem : scratch)(p, cnt, fill); });
+        P[i].stats = &st[i];
+    }
+    std::vector<uint32_t> seg_base(n + 1), blk_base(n + 1);
+    compact_many_bases(P.data(), n, seg_base.data(), blk_base.data());
+    host_alloc(scratch, M.ticket, 2, 0);
+    M.job = P.data();
+    M.seg_base = seg_base.data();
+    M.blk_base = blk_base.data();
+    M.validate_hash = any_hash;
+    M.crc_table = (const unsigned long long *)crc_tab;
+    *launches = compact_launch_many(M, shared, 2, 2, nullptr, [](int) {});
+    for (uint32_t i = 0; i < n; i++) {
+        Merged &R = g_many[i];
+        pgs_compact_result res{};
+        R.run.n_bloom_entries = compact_result_stats(st[i], T[i].in_block_bytes, res, R.run.info);
+        R.st = st[i];
+        R.Q = P[i].Q;
+    }
+    for (uint32_t i = 0; i < n; i++)
+        if (st[i].error) { fprintf(stderr, "sim_compact_many: job %u: status %u at segment %u of %u\n", i, st[i].error, st[i].error_seg, P[i].Q); return (int32_t)st[i].error; }
+    return PGS_OK;
+}
+// job i of the last sim_compact_many becomes the output sim_result_* read
+int32_t sim_compact_many_select(uint32_t i)
+{
+    if (i >= g_many.size()) return PGS_INVALID_ARGUMENT;
+    g_res = g_many[i];
     return PGS_OK;
 }
 
