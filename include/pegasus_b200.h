@@ -192,6 +192,37 @@ PGS_API void pgs_run_build_last_ms(float *ms4);
 /* device time (ms) of the sort and the gather of the sorted copy in the calling thread's last successful pgs_run_build_unsorted
  */
 PGS_API float pgs_run_build_last_sort_ms(void);
+/* One job of pgs_run_build_many: the arguments pgs_run_build takes for one partition. */
+typedef struct {
+    pgs_partition *part;
+    int32_t level;
+    uint64_t n;
+    const uint8_t *keys;
+    const uint64_t *key_off;
+    const uint8_t *vals;
+    const uint64_t *val_off;
+    const uint64_t *seq;
+    const uint8_t *type;
+} pgs_run_build_job;
+#define PGS_RUN_BUILD_MANY_MAX_JOBS 4096u
+/* The runs of many partitions of one engine built in one set of kernel launches on the engine stream.  Job i is by definition
+ * pgs_run_build(jobs[i].part, jobs[i].level, jobs[i].n, ...): its blocks, blk_off, blk_size and pgs_run_info (all but the run
+ * id) are byte for byte the same.  The jobs' records form one record space of N = sum(n) records; a block never crosses a job.
+ *   run_ids_out (n entries, may be NULL): job i's run id, 0 for a job with n == 0 (nothing installed for it).
+ *   launches: 2 * R + 7 with R = max(1, ceil(log2 N)), whatever n is; none when N == 0.
+ *   host waits: three (the block plan, index pass 1, index pass 2).
+ * Statuses, checked before anything is allocated or launched:
+ *   n > PGS_RUN_BUILD_MANY_MAX_JOBS, a job of more than 0xFFFFFFF0 records, or N > 0xFFFFFFF0 - PGS_RUN_BUILD_MANY_MAX_JOBS (the
+ *   32-bit record indices of one launch): PGS_NOT_SUPPORTED -- split the call;
+ *   jobs == NULL with n > 0, a job without a partition, level < 0, a job with records and a NULL array, the same partition in
+ *   two jobs, partitions of different engines: PGS_INVALID_ARGUMENT.
+ * Found on the device, per job, with pgs_run_build's statuses and precedence: offsets out of range or records out of order
+ * (PGS_INVALID_ARGUMENT), a user key over 4096 bytes or a block of 4 GB or more (PGS_NOT_SUPPORTED).  The call returns the status
+ * of the lowest-numbered failing job, and pgs_last_error() names it.
+ * All or nothing: on any error no partition's run list changes, and every device buffer of the call is freed.
+ * Device memory: every job's input and pgs_run_build's scratch for N records, the runs, and per block 8 bytes of index scratch.
+ * pgs_run_build_last_ms reports the call's four phases. */
+PGS_API int32_t pgs_run_build_many(const pgs_run_build_job *jobs, uint32_t n, uint64_t *run_ids_out);
 PGS_API int32_t pgs_run_drop(pgs_partition *p, uint64_t run_id);
 PGS_API int32_t pgs_run_info_get(pgs_partition *p, uint64_t run_id, pgs_run_info *out);
 /* run ids in read order (newest first: L0 by recency, then L1, L2, ...) */
@@ -690,6 +721,15 @@ PGS_API int32_t pgs_rrdb_multi_remove(pgs_server *s, pgs_blob hash_key, const pg
  * L0 trigger check (L0 count >= trigger -> L0(+L1) -> L1 compaction with the filter at `now`).
  * `now` (epoch_now) also feeds the default-TTL substitution of puts (rocksdb_wrapper.cpp:280-288). */
 PGS_API int32_t pgs_rrdb_flush(pgs_server *s, uint32_t now);
+/* pgs_rrdb_flush of n replicas of one engine, in the resulting records, decrees and reads.  The replicas' writer locks are
+ * taken in address order.  The non-empty memtables are packed in the given order into calls of at most 256 MB of staged
+ * memtable bytes and PGS_RUN_BUILD_MANY_MAX_JOBS replicas (a larger memtable goes alone), each call one pgs_run_build_many;
+ * then the flushed replicas whose L0 count reached l0_compaction_trigger are compacted L0(+L1) -> L1 in one pgs_compact_many
+ * (the block layout of those runs may differ from a per-replica compaction, as pgs_compact_many documents).  A failed build
+ * call flushes none of its replicas nor any later one; the replicas in front of it stay flushed and are compacted, and the
+ * call returns the build's status.  A failed compaction leaves the flushes done.  Replicas on different engines, or one given
+ * twice: PGS_INVALID_ARGUMENT. */
+PGS_API int32_t pgs_rrdb_flush_many(pgs_server *const *servers, uint32_t n, uint32_t now);
 /* do_manual_compact (pegasus_server_impl.cpp:3373-3456): whole-CF CompactRange, bottommost
  * level forced. */
 PGS_API int32_t pgs_rrdb_manual_compact(pgs_server *s, uint32_t now, pgs_compact_result *out);

@@ -79,6 +79,17 @@ class CompactJob(C.Structure):
                 ("bottommost", C.c_int32), ("fp", C.POINTER(FilterParams))]
 
 
+class RunBuildJob(C.Structure):
+    _fields_ = [("part", C.c_void_p), ("level", C.c_int32), ("n", C.c_uint64), ("keys", C.c_void_p), ("key_off", C.c_void_p),
+                ("vals", C.c_void_p), ("val_off", C.c_void_p), ("seq", C.c_void_p), ("type", C.c_void_p)]
+
+    @staticmethod
+    def of(part, recs: "Records", level: int = 0) -> "RunBuildJob":
+        """the job of `recs` for `part` (a Partition or None); the arrays of recs must outlive the call"""
+        return RunBuildJob(part.h.value if part is not None else None, level, recs.n, recs.keys.ctypes.data, recs.key_off.ctypes.data,
+                           recs.vals.ctypes.data, recs.val_off.ctypes.data, recs.seq.ctypes.data, recs.type.ctypes.data)
+
+
 SPLIT_MAX_CHILDREN = 32
 
 
@@ -261,6 +272,8 @@ def lib() -> C.CDLL:
                                C.c_uint64, C.c_uint32],
         "pgs_rrdb_multi_remove": [vp, Blob, C.POINTER(Blob), C.c_uint32, C.c_int64, C.POINTER(C.c_int64), C.c_uint32],
         "pgs_rrdb_flush": [vp, C.c_uint32],
+        "pgs_rrdb_flush_many": [C.POINTER(vp), C.c_uint32, C.c_uint32],
+        "pgs_run_build_many": [C.POINTER(RunBuildJob), C.c_uint32, u64p],
         "pgs_rrdb_manual_compact": [vp, C.c_uint32, C.POINTER(CompactResult)],
         "pgs_rrdb_manual_compact_many": [C.POINTER(vp), C.c_uint32, C.c_uint32, C.POINTER(CompactResult)],
         "pgs_compact_many": [C.POINTER(CompactJob), C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(CompactResult)],
@@ -469,6 +482,17 @@ class Engine:
         res = (CompactResult * max(1, n))()
         _check(lib().pgs_compact_many(arr if n else None, n, now, flags, res), "compact_many")
         return [res[i] for i in range(n)]
+
+    def build_many(self, jobs) -> list[int]:
+        """pgs_run_build_many: the runs of many partitions of this engine built in one set of launches.  A job is (partition,
+        records in internal-key order, level); returns one run id per job (0 for a job without records)."""
+        n = len(jobs)
+        arr = (RunBuildJob * max(1, n))()
+        for i, (part, recs, level) in enumerate(jobs):
+            arr[i] = RunBuildJob.of(part, recs, level)
+        ids = np.zeros(max(1, n), np.uint64)
+        _check(lib().pgs_run_build_many(arr if n else None, n, ids.ctypes.data_as(u64p)), "run_build_many")
+        return [int(x) for x in ids[:n]]
 
     def __enter__(self):
         return self

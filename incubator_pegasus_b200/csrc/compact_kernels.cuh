@@ -1728,17 +1728,6 @@ struct MergeJobs {
     uint32_t *ticket;         // [0] k_walk_many, [1] k_emit_many
 };
 
-// the job whose range [base[j], base[j + 1]) holds x (base[0] = 0 <= x < base[n]; empty ranges are skipped)
-PGS_HD uint32_t job_of(const uint32_t *base, uint32_t n, uint32_t x)
-{
-    uint32_t lo = 0, hi = n; // base[lo] <= x < base[hi]
-    while (hi - lo > 1) {
-        const uint32_t mid = (lo + hi) >> 1;
-        if (base[mid] <= x) lo = mid; else hi = mid;
-    }
-    return lo;
-}
-
 __global__ void __launch_bounds__(256) k_plan_many(const __grid_constant__ MergeJobs M)
 {
     const uint32_t gt = blockIdx.x * blockDim.x + threadIdx.x;

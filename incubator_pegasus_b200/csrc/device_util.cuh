@@ -33,6 +33,17 @@ struct ReadInit {
 constexpr ReadInit kZero{nullptr, 0, 0};
 void set_error(const char *fmt, ...); // the message of a refused call (engine.cu; the simulator prints it)
 
+// the job whose range [base[j], base[j + 1]) holds x (base[0] = 0 <= x < base[n]; empty ranges are skipped)
+PGS_HD uint32_t job_of(const uint32_t *base, uint32_t n, uint32_t x)
+{
+    uint32_t lo = 0, hi = n; // base[lo] <= x < base[hi]
+    while (hi - lo > 1) {
+        const uint32_t mid = (lo + hi) >> 1;
+        if (base[mid] <= x) lo = mid; else hi = mid;
+    }
+    return lo;
+}
+
 // ---- shared-memory addressing / mbarrier / TMA bulk (cp.async.bulk) ----------------------------
 #ifdef PGS_SIM
 // The stand-ins check what the device would fault on or hang at: a bulk copy's addresses and size, and an mbarrier whose

@@ -172,6 +172,8 @@ int32_t index_init_kernels()
     const int smem = (int)(kIdxWarps * kIdxScratch);
     PGS_CUDA(cudaFuncSetAttribute(k_index_walk<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     PGS_CUDA(cudaFuncSetAttribute(k_index_walk<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    PGS_CUDA(cudaFuncSetAttribute(k_index_walk_many<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    PGS_CUDA(cudaFuncSetAttribute(k_index_walk_many<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     return PGS_OK;
 }
 
@@ -649,6 +651,194 @@ int32_t pgs_run_build_unsorted(pgs_partition *ph, int32_t level, uint64_t n, con
         cudaEventElapsedTime(&t_sort_ms, ev_copied, ev[1]);
         for (int i = 1; i < 4; i++) cudaEventElapsedTime(&t_build_ms[i], ev[i], ev[i + 1]);
     }
+    return PGS_OK;
+}
+
+// The nonempty jobs planned as one record space (build_many_plan) and built in one set of launches: the plan, one wait for the
+// summary and every job's status, every job's run allocated, the blocks and index pass 1 over all runs, one wait, index_buffers
+// per run, pass 2, one wait, and every run installed under all the partitions' locks.
+int32_t pgs_run_build_many(const pgs_run_build_job *jobs, uint32_t n, uint64_t *run_ids_out)
+{
+    memset(t_build_ms, 0, sizeof t_build_ms);
+    if (n == 0) return PGS_OK;
+    if (!jobs) { set_error("run build many: %u jobs and no job array", n); return PGS_INVALID_ARGUMENT; }
+    if (n > PGS_RUN_BUILD_MANY_MAX_JOBS) { set_error("run build many: %u jobs > %u per call", n, PGS_RUN_BUILD_MANY_MAX_JOBS); return PGS_NOT_SUPPORTED; }
+    Engine *e = nullptr;
+    std::vector<Partition *> parts(n);
+    for (uint32_t i = 0; i < n; i++) {
+        const pgs_run_build_job &x = jobs[i];
+        if (!x.part || x.level < 0 || (x.n && (!x.key_off || !x.val_off || !x.seq || !x.type)) ||
+            (x.n && ((!x.keys && x.key_off[x.n]) || (!x.vals && x.val_off[x.n])))) {
+            set_error("run build many: job %u: no partition, a negative level or a missing array", i);
+            return PGS_INVALID_ARGUMENT;
+        }
+        parts[i] = &x.part->p;
+        if (!e) e = parts[i]->eng;
+        if (parts[i]->eng != e) { set_error("run build many: job %u: its partition is on another engine than job 0's", i); return PGS_INVALID_ARGUMENT; }
+    }
+    {
+        std::vector<Partition *> order = parts;
+        std::sort(order.begin(), order.end());
+        for (uint32_t i = 1; i < n; i++)
+            if (order[i] == order[i - 1]) {
+                const uint32_t j = (uint32_t)(std::find(parts.begin(), parts.end(), order[i]) - parts.begin());
+                set_error("run build many: job %u: its partition is in another job too", j);
+                return PGS_INVALID_ARGUMENT;
+            }
+    }
+    std::vector<const pgs_run_build_job *> J; // the nonempty jobs, and which job each one is
+    std::vector<uint32_t> which;
+    uint64_t total = 0;
+    for (uint32_t i = 0; i < n; i++) {
+        if (jobs[i].n > kBuildMaxRecords) {
+            set_error("run build many: job %u: %llu records exceed the index's 32-bit record offsets", i, (unsigned long long)jobs[i].n);
+            return PGS_NOT_SUPPORTED;
+        }
+        total += jobs[i].n;
+        if (jobs[i].n) { J.push_back(&jobs[i]); which.push_back(i); }
+    }
+    if (total > kBuildMaxRecords - PGS_RUN_BUILD_MANY_MAX_JOBS) {
+        set_error("run build many: %llu records exceed one launch's 32-bit record indices; split the call", (unsigned long long)total);
+        return PGS_NOT_SUPPORTED;
+    }
+    if (run_ids_out) memset(run_ids_out, 0, sizeof(uint64_t) * n);
+    const uint32_t jn = (uint32_t)J.size();
+    if (jn == 0) return PGS_OK;
+
+    PGS_CUDA(cudaSetDevice(e->device));
+    cudaStream_t st = e->stream;
+    struct Pinned { // pinned staging of the engine, given back when the call ends
+        Engine *e; size_t need; size_t cap = 0; uint8_t *p = (uint8_t *)e->take_pinned(need, &cap);
+        ~Pinned() { if (p) e->give_pinned(p, cap); }
+    };
+    struct Drain { // on an error, nothing of the call may still be in flight when its staging and buffers go
+        Engine *e; bool armed = true;
+        ~Drain() { if (armed) upload_abandon(e); }
+    };
+    auto a16 = [](uint64_t x) { return (x + 15) & ~15ull; };
+    LaunchScratch S(st);
+    std::vector<std::shared_ptr<Run>> runs(jn);
+    // the plan's staging: job_rec [jn + 1] | job [jn] | summary | job_out [3 jn] | job_off [jn]
+    const uint64_t o_job = a16(4ull * (jn + 1)), o_sum = a16(o_job + sizeof(BuildJob) * jn), o_out = a16(o_sum + sizeof(BuildSummary));
+    const uint64_t o_off = a16(o_out + 12ull * jn);
+    Pinned pa{e, o_off + 8ull * jn};
+    if (!pa.p) { set_error("run build many: no pinned staging memory"); return PGS_IO_ERROR; }
+    Drain drain{e};
+    uint32_t *job_rec = (uint32_t *)pa.p, *job_out = (uint32_t *)(pa.p + o_out);
+    BuildJob *job = (BuildJob *)(pa.p + o_job);
+    const BuildSummary &sum = *(const BuildSummary *)(pa.p + o_sum);
+    const unsigned long long *job_off = (const unsigned long long *)(pa.p + o_off);
+    cudaEvent_t ev[5], ev_read;
+    for (auto &x : ev) PGS_CUDA(S.event(x));
+    PGS_CUDA(S.event(ev_read));
+    PGS_CUDA(cudaEventRecord(ev[0], st));
+    BuildManyParams M{};
+    build_many_plan(M, J.data(), jn, job_rec, job, e->cfg.block_size, e->cfg.restart_interval);
+    cudaError_t ce = cudaSuccess;
+    build_many_stage(M, J.data(), job_rec, job, device_buffers(S, ce), [&](const void *dst, const void *src, uint64_t bytes) {
+        if (ce == cudaSuccess && bytes) ce = cudaMemcpyAsync((void *)dst, src, bytes, cudaMemcpyHostToDevice, st);
+    });
+    PGS_CUDA(ce);
+    build_many_buffers(M, scratch_buffers(S, ce));
+    PGS_CUDA(ce);
+    PGS_CUDA(cudaEventRecord(ev[1], st));
+    e->launches += build_many_launch_plan(M, 0, st, [](int) {});
+    PGS_CUDA(cudaMemcpyAsync(pa.p + o_sum, M.B.sum, sizeof(BuildSummary), cudaMemcpyDeviceToHost, st));
+    PGS_CUDA(cudaMemcpyAsync(job_out, M.job_out, 12ull * jn, cudaMemcpyDeviceToHost, st));
+    PGS_CUDA(cudaMemcpyAsync(pa.p + o_off, M.job_off, 8ull * jn, cudaMemcpyDeviceToHost, st));
+    PGS_CUDA(cudaEventRecord(ev[2], st));
+    PGS_CUDA(cudaEventSynchronize(ev[2]));
+    std::vector<uint32_t> nb(jn);
+    std::vector<uint64_t> bytes(jn);
+    for (uint32_t d = 0; d < jn; d++)
+        if (const int32_t rc = build_many_job(M, sum, job_out, job_off, d, nb[d], bytes[d])) {
+            if (rc == PGS_INVALID_ARGUMENT) set_error("run build many: job %u: records out of internal-key order, or offsets out of range", which[d]);
+            else set_error("run build many: job %u: a user key over %u bytes, or a block over 4 GB", which[d], kMaxUkeyLen);
+            return rc;
+        }
+
+    // every job's run, and the index staging: nrec [nb] | lastlen [nb] | rec_cum [nb + jn] | key_cum [nb + jn] | then the table
+    // the device reads: stats [jn] | out [jn] | X [jn]
+    const uint32_t NB = (uint32_t)sum.n_blocks;
+    const uint64_t o_rc = 8ull * NB, o_kc = o_rc + 4ull * (NB + jn), o_tab = a16(o_kc + 4ull * (NB + jn));
+    const uint64_t t_out = a16(sizeof(IndexStats) * jn), t_x = a16(t_out + sizeof(BuildRunOut) * jn), t_end = t_x + sizeof(IndexParams) * jn;
+    Pinned pb{e, o_tab + t_end};
+    if (!pb.p) { set_error("run build many: no pinned staging memory"); return PGS_IO_ERROR; }
+    Drain drain_b{e};
+    uint32_t *h_nrec = (uint32_t *)pb.p, *h_lastlen = h_nrec + NB, *rec_cum = (uint32_t *)(pb.p + o_rc), *key_cum = (uint32_t *)(pb.p + o_kc);
+    IndexStats *hs = (IndexStats *)(pb.p + o_tab);
+    BuildRunOut *outs = (BuildRunOut *)(pb.p + o_tab + t_out);
+    IndexParams *X = (IndexParams *)(pb.p + o_tab + t_x);
+    uint32_t *d_nrec = nullptr, *d_lastlen = nullptr;
+    uint8_t *d_tab = nullptr;
+    PGS_CUDA(S.alloc(d_nrec, 4ull * NB));
+    PGS_CUDA(S.alloc(d_lastlen, 4ull * NB));
+    PGS_CUDA(S.alloc(d_tab, t_end));
+    for (uint32_t d = 0; d < jn; d++) {
+        runs[d] = std::make_shared<Run>(e);
+        Run &r = *runs[d];
+        r.level = r.info.level = J[d]->level;
+        PGS_CUDA(e->alloc_data(r, bytes[d] + 256));
+        PGS_CUDA(cudaMemsetAsync(r.d_data + bytes[d], 0, r.data_cap - bytes[d], st));
+        PGS_CUDA(cudaMallocAsync(&r.d_blk_off, sizeof(uint64_t) * (nb[d] + 1), st));
+        PGS_CUDA(cudaMallocAsync(&r.d_blk_size, sizeof(uint32_t) * nb[d], st));
+        outs[d] = BuildRunOut{r.d_data, (unsigned long long *)r.d_blk_off, r.d_blk_size};
+        X[d] = IndexParams{r.d_data, r.d_blk_off, r.d_blk_size, nb[d]};
+        X[d].nrec = d_nrec + job_out[d];
+        X[d].lastlen = d_lastlen + job_out[d];
+        X[d].stats = (IndexStats *)d_tab + d;
+        hs[d] = index_stats_init();
+    }
+    PGS_CUDA(cudaMemcpyAsync(d_tab, hs, t_end, cudaMemcpyHostToDevice, st));
+    M.out = (const BuildRunOut *)(d_tab + t_out);
+    const IndexParams *d_X = (const IndexParams *)(d_tab + t_x);
+    e->launches += build_many_launch_blocks(M, NB, 0, st);
+    PGS_CUDA(cudaEventRecord(ev[3], st));
+    e->launches += index_launch_many<false>(d_X, M.job_out, jn, NB, st);
+    PGS_CUDA(cudaMemcpyAsync(h_nrec, d_nrec, 4ull * NB, cudaMemcpyDeviceToHost, st));
+    PGS_CUDA(cudaMemcpyAsync(h_lastlen, d_lastlen, 4ull * NB, cudaMemcpyDeviceToHost, st));
+    PGS_CUDA(cudaMemcpyAsync(hs, d_tab, sizeof(IndexStats) * jn, cudaMemcpyDeviceToHost, st));
+    PGS_CUDA(cudaEventRecord(ev_read, st));
+    PGS_CUDA(cudaEventSynchronize(ev_read));
+    for (uint32_t d = 0; d < jn; d++) {
+        const uint32_t b0 = job_out[d];
+        const int32_t rc = index_buffers(X[d], *runs[d], h_nrec + b0, h_lastlen + b0, hs[d], rec_cum + b0 + d, key_cum + b0 + d,
+                                         [&](auto *&p, uint64_t cnt, int fill) {
+                                             const size_t sz = sizeof(*p) * cnt;
+                                             if (ce == cudaSuccess) ce = cudaMallocAsync((void **)&p, sz, st); // ~Run frees them
+                                             if (ce == cudaSuccess && fill != kNoFill) ce = cudaMemsetAsync(p, fill, sz, st);
+                                         });
+        if (rc) {
+            const std::string m = g_last_error;
+            set_error("run build many: job %u: %s", which[d], m.c_str());
+            return rc;
+        }
+        PGS_CUDA(ce);
+        PGS_CUDA(cudaMemcpyAsync(X[d].blk_rec, rec_cum + b0 + d, sizeof(uint32_t) * (nb[d] + 1), cudaMemcpyHostToDevice, st));
+        PGS_CUDA(cudaMemcpyAsync(X[d].ikey_off, key_cum + b0 + d, sizeof(uint32_t) * (nb[d] + 1), cudaMemcpyHostToDevice, st));
+    }
+    PGS_CUDA(cudaMemcpyAsync(d_tab + t_x, X, sizeof(IndexParams) * jn, cudaMemcpyHostToDevice, st));
+    e->launches += index_launch_many<true>(d_X, M.job_out, jn, NB, st);
+    PGS_CUDA(cudaEventRecord(ev[4], st));
+    PGS_CUDA(cudaEventSynchronize(ev[4]));
+    {
+        // all partitions or none: every lock is held, in address order, while the runs go in
+        std::vector<Partition *> order;
+        for (auto *x : J) order.push_back(&x->part->p);
+        std::sort(order.begin(), order.end());
+        std::vector<std::unique_lock<std::mutex>> held;
+        for (Partition *p : order) held.emplace_back(p->mu);
+        for (uint32_t d = 0; d < jn; d++) {
+            Run &r = *runs[d];
+            run_info_from_index(hs[d], nb[d], bytes[d], job_out[jn + d], r.info);
+            r.id = e->next_run_id++;
+            r.info.run_id = r.id;
+            J[d]->part->p.insert(runs[d]);
+            if (run_ids_out) run_ids_out[which[d]] = r.id;
+        }
+    }
+    drain.armed = drain_b.armed = false;
+    for (int i = 0; i < 4; i++) cudaEventElapsedTime(&t_build_ms[i], ev[i], ev[i + 1]);
     return PGS_OK;
 }
 

@@ -19,19 +19,15 @@ struct IndexStats {
 constexpr uint32_t kIdxWarps = 8;
 constexpr uint32_t kIdxScratch = kMaxUkeyLen + 16;
 
+// one warp walks block b (of the run at data / blk_off / blk_size): both passes' work on it.  Pass 1 (!kEmitKey) writes
+// nrec_out[b] / lastlen_out[b] and adds into *stats; pass 2 writes the block's index key, entry offsets and Bloom bits.
 template <bool kEmitKey>
-__global__ void __launch_bounds__(kIdxWarps * 32)
-k_index_walk(const uint8_t *__restrict__ data, const uint64_t *__restrict__ blk_off,
-             const uint32_t *__restrict__ blk_size, uint32_t nb, uint32_t *__restrict__ nrec_out,
-             uint32_t *__restrict__ lastlen_out, const uint32_t *__restrict__ ikey_off,
-             uint8_t *__restrict__ ikeys, const uint32_t *__restrict__ blk_rec, uint32_t *__restrict__ rec_off,
-             uint32_t *__restrict__ bloom, uint32_t bloom_lines, IndexStats *__restrict__ stats, uint32_t b_begin)
+PGS_DEV void index_walk_block(const Grp<32> &g, uint8_t *smem, uint32_t warp, uint32_t lane, const uint8_t *__restrict__ data, const uint64_t *__restrict__ blk_off,
+                              const uint32_t *__restrict__ blk_size, uint32_t b, uint32_t *__restrict__ nrec_out,
+                              uint32_t *__restrict__ lastlen_out, const uint32_t *__restrict__ ikey_off, uint8_t *__restrict__ ikeys,
+                              const uint32_t *__restrict__ blk_rec, uint32_t *__restrict__ rec_off, uint32_t *__restrict__ bloom,
+                              uint32_t bloom_lines, IndexStats *__restrict__ stats)
 {
-    const Grp<32> g;
-    PGS_SMEM_DYN(smem);
-    uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    uint32_t b = b_begin + blockIdx.x * kIdxWarps + warp; // blocks [b_begin, nb)
-    if (b >= nb) return;
     uint8_t *scr = smem + warp * kIdxScratch;
     const uint8_t *base = data + blk_off[b];
     uint32_t size = blk_size[b];
@@ -115,6 +111,23 @@ k_index_walk(const uint8_t *__restrict__ data, const uint64_t *__restrict__ blk_
         atomicMax(&stats->max_blk_rec, nrec);
     }
     if (err && lane == 0) atomicMax(&stats->error, err);
+}
+
+template <bool kEmitKey>
+__global__ void __launch_bounds__(kIdxWarps * 32)
+k_index_walk(const uint8_t *__restrict__ data, const uint64_t *__restrict__ blk_off,
+             const uint32_t *__restrict__ blk_size, uint32_t nb, uint32_t *__restrict__ nrec_out,
+             uint32_t *__restrict__ lastlen_out, const uint32_t *__restrict__ ikey_off,
+             uint8_t *__restrict__ ikeys, const uint32_t *__restrict__ blk_rec, uint32_t *__restrict__ rec_off,
+             uint32_t *__restrict__ bloom, uint32_t bloom_lines, IndexStats *__restrict__ stats, uint32_t b_begin)
+{
+    const Grp<32> g;
+    PGS_SMEM_DYN(smem);
+    uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    uint32_t b = b_begin + blockIdx.x * kIdxWarps + warp; // blocks [b_begin, nb)
+    if (b >= nb) return;
+    index_walk_block<kEmitKey>(g, smem, warp, lane, data, blk_off, blk_size, b, nrec_out, lastlen_out, ikey_off, ikeys, blk_rec, rec_off,
+                               bloom, bloom_lines, stats);
 }
 
 // host, before anything is copied: the handle rule of pgs_run_upload.  Every block starts on a multiple of kBlockAlign, at or
@@ -217,6 +230,38 @@ inline uint32_t index_launch_pass2(const IndexParams &X, cudaStream_t st)
     if (!X.nb) return 0;
     PGS_LAUNCH(k_index_walk<true>, (X.nb + kIdxWarps - 1) / kIdxWarps, kIdxWarps * 32, kIdxWarps * kIdxScratch, st, X.data, X.blk_off,
                X.blk_size, X.nb, nullptr, nullptr, X.ikey_off, X.ikeys, X.blk_rec, X.rec_off, X.bloom, X.bloom_lines, X.stats, 0u);
+    return 1;
+}
+
+// Both passes over the blocks of several runs in one launch (pgs_run_build_many): run j is X[j], and its blocks are the launch's
+// blocks [blk0[j], blk0[j + 1]) (blk0[0] = 0, nb in all).  Each run keeps its own statistics and index buffers.
+// (a register cap instead of launch bounds: with the bounds ptxas kept pass 2 at 40 registers and spilled two of the run's
+// pointers it needs only at the end of the walk; 48 is pass 1's count and allows 5 CTAs per SM, the shared memory 6)
+template <bool kEmitKey>
+__global__ void __maxnreg__(48) k_index_walk_many(const IndexParams *__restrict__ X, const uint32_t *__restrict__ blk0,
+                                                                    uint32_t runs, uint32_t nb)
+{
+    const Grp<32> g;
+    PGS_SMEM_DYN(smem);
+    const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31, b = blockIdx.x * kIdxWarps + warp;
+    if (b >= nb) return;
+    const uint32_t j = job_of(blk0, runs, b);
+    const IndexParams &x = X[j];
+    // each pass reads only its own buffers of the run, as index_launch_pass1 / index_launch_pass2 pass them
+    if (kEmitKey)
+        index_walk_block<true>(g, smem, warp, lane, x.data, x.blk_off, x.blk_size, b - blk0[j], nullptr, nullptr, x.ikey_off, x.ikeys,
+                               x.blk_rec, x.rec_off, x.bloom, x.bloom_lines, x.stats);
+    else
+        index_walk_block<false>(g, smem, warp, lane, x.data, x.blk_off, x.blk_size, b - blk0[j], x.nrec, x.lastlen, nullptr, nullptr,
+                                nullptr, nullptr, nullptr, 0u, x.stats);
+}
+// pass 1 (kEmitKey false: X[j]'s scratch set) or pass 2 (true: X[j]'s index buffers set) of the nb blocks of every run of X
+// (a device table); returns the launches
+template <bool kEmitKey>
+inline uint32_t index_launch_many(const IndexParams *X, const uint32_t *blk0, uint32_t runs, uint32_t nb, cudaStream_t st)
+{
+    if (!nb) return 0;
+    PGS_LAUNCH(k_index_walk_many<kEmitKey>, (nb + kIdxWarps - 1) / kIdxWarps, kIdxWarps * 32, kIdxWarps * kIdxScratch, st, X, blk0, runs, nb);
     return 1;
 }
 

@@ -128,18 +128,22 @@ struct Server {
         std::lock_guard<std::mutex> g(part->p.mu);
         return part->p.runs;
     }
-    int32_t flush_mem()
+    // flush_mem in two halves, shared with flush_many: the memtable (sorted, one version per key) flattened at `at`
+    // (flush_staging_bytes() of them) as key_off | val_off | seq | type | keys | values, the job that builds its L0 run on the
+    // device (pgs_run_build); and the replica's state once that run is installed
+    uint64_t flush_staging_bytes() const
     {
-        if (mem.empty()) return PGS_OK;
-        // the memtable (sorted, one version per key) flattened into pinned staging: key_off | val_off | seq | type | keys | values;
-        // the device encodes the blocks (pgs_run_build)
         const uint64_t n = mem.size();
         uint64_t kb = 0, vb = 0;
         for (auto &kv : mem) { kb += kv.first.size(); vb += kv.second.value.size(); }
-        size_t cap = 0;
-        uint8_t *pin = (uint8_t *)eng->take_pinned(8 * (3 * n + 2) + n + kb + vb, &cap);
-        if (!pin) { set_error("flush: no pinned staging memory"); return PGS_IO_ERROR; }
-        uint64_t *key_off = (uint64_t *)pin, *val_off = key_off + n + 1, *seq = val_off + n + 1;
+        return 8 * (3 * n + 2) + n + kb + vb;
+    }
+    pgs_run_build_job flush_stage(uint8_t *at) const
+    {
+        const uint64_t n = mem.size();
+        uint64_t *key_off = (uint64_t *)at, *val_off = key_off + n + 1, *seq = val_off + n + 1;
+        uint64_t kb = 0;
+        for (auto &kv : mem) kb += kv.first.size();
         uint8_t *type = (uint8_t *)(seq + n), *keys = type + n, *vals = keys + kb;
         uint64_t i = 0, ko = 0, vo = 0;
         for (auto &kv : mem) {
@@ -155,33 +159,52 @@ struct Server {
         }
         key_off[n] = ko;
         val_off[n] = vo;
-        uint64_t id = 0;
-        int32_t st = pgs_run_build(part, 0, n, keys, key_off, vals, val_off, seq, type, &id);
-        eng->give_pinned(pin, cap);
-        if (st != PGS_OK) return st;
+        return pgs_run_build_job{part, 0, n, keys, key_off, vals, val_off, seq, type};
+    }
+    void flush_commit()
+    {
         mem.clear();
         mem_bytes = 0;
         last_flushed_decree = last_committed_decree; // everything applied so far now lives in an HBM run
+    }
+    int32_t flush_mem()
+    {
+        if (mem.empty()) return PGS_OK;
+        size_t cap = 0;
+        uint8_t *pin = (uint8_t *)eng->take_pinned(flush_staging_bytes(), &cap);
+        if (!pin) { set_error("flush: no pinned staging memory"); return PGS_IO_ERROR; }
+        const pgs_run_build_job j = flush_stage(pin);
+        uint64_t id = 0;
+        int32_t st = pgs_run_build(part, 0, j.n, j.keys, j.key_off, j.vals, j.val_off, j.seq, j.type, &id);
+        eng->give_pinned(pin, cap);
+        if (st != PGS_OK) return st;
+        flush_commit();
         return PGS_OK;
     }
-    // L0 (+ the L1 run) -> L1, the engine's stand-in for RocksDB's level0_file_num_compaction_trigger
-    int32_t compact_l0(uint32_t now)
+    // compact_l0's job: the ids of L0 and L1 (ids empty: nothing to merge)
+    void l0_job(std::vector<uint64_t> &ids)
     {
-        auto rs = runs();
-        std::vector<uint64_t> ids;
-        for (auto &r : rs)
+        for (auto &r : runs())
             if (r->level <= 1) ids.push_back(r->id);
-        if (ids.size() < 2) return PGS_OK;
-        pgs_filter_params fp = filter();
-        return pgs_compact(part, ids.data(), (uint32_t)ids.size(), 1, -1, &fp, now, nullptr);
+        if (ids.size() < 2) ids.clear();
     }
-    int32_t maybe_compact(uint32_t now)
+    bool l0_triggered()
     {
         uint32_t trigger = opt.l0_compaction_trigger ? opt.l0_compaction_trigger : 4;
         uint32_t l0 = 0;
         for (auto &r : runs()) l0 += r->level == 0;
-        return l0 >= trigger ? compact_l0(now) : PGS_OK;
+        return l0 >= trigger;
     }
+    // L0 (+ the L1 run) -> L1, the engine's stand-in for RocksDB's level0_file_num_compaction_trigger
+    int32_t compact_l0(uint32_t now)
+    {
+        std::vector<uint64_t> ids;
+        l0_job(ids);
+        if (ids.empty()) return PGS_OK;
+        pgs_filter_params fp = filter();
+        return pgs_compact(part, ids.data(), (uint32_t)ids.size(), 1, -1, &fp, now, nullptr);
+    }
+    int32_t maybe_compact(uint32_t now) { return l0_triggered() ? compact_l0(now) : PGS_OK; }
     // range reads: the memtable becomes an L0 run, and L0 is folded once the run list grows past kReadMaxRuns, or when the
     // reverse-scan kernel could not stage one block of every run (many L0 runs of small records, such as tombstones)
     bool needs_fold(bool reverse) { return runs().size() > kReadMaxRuns || (reverse && !scan_stages_every_run(part)); }
@@ -647,6 +670,72 @@ static void parse_envs(const char *envs, uint32_t n, std::vector<std::pair<std::
 
 using namespace pgs;
 struct pgs_server { Server s; };
+
+namespace pgs {
+// The writer locks of n replicas of one engine, taken in address order into held; PGS_INVALID_ARGUMENT for a null replica,
+// replicas on different engines or one given twice (nothing locked then).
+static int32_t lock_replicas(pgs_server *const *servers, uint32_t n, const char *what, std::vector<std::unique_lock<std::shared_mutex>> &held)
+{
+    if (!servers) return PGS_INVALID_ARGUMENT;
+    std::vector<Server *> order;
+    for (uint32_t i = 0; i < n; i++) {
+        if (!servers[i]) return PGS_INVALID_ARGUMENT;
+        if (servers[i]->s.part->p.eng != servers[0]->s.part->p.eng) {
+            set_error("%s: replica %u is on another engine than replica 0", what, i);
+            return PGS_INVALID_ARGUMENT;
+        }
+        order.push_back(&servers[i]->s);
+    }
+    std::sort(order.begin(), order.end());
+    if (std::adjacent_find(order.begin(), order.end()) != order.end()) {
+        set_error("%s: a replica given twice", what);
+        return PGS_INVALID_ARGUMENT;
+    }
+    for (Server *s : order) held.emplace_back(s->mu);
+    return PGS_OK;
+}
+
+constexpr uint64_t kFlushManyBytes = 256ull << 20; // staged memtable bytes per pgs_run_build_many call of flush_many
+
+// flush_mem of n replicas (their writer locks held): the non-empty memtables, in the given order, packed into calls of at most
+// kFlushManyBytes of staging (a larger memtable goes alone) and PGS_RUN_BUILD_MANY_MAX_JOBS replicas, each call one
+// pgs_run_build_many, and the replicas of a successful call committed.  A failed call commits none of its replicas and ends the
+// flush; *done (if not null) = the replicas in front of it, all of them on success.
+static int32_t flush_many(pgs_server *const *servers, uint32_t n, uint32_t *done = nullptr)
+{
+    uint32_t i = 0;
+    if (done) *done = 0;
+    while (i < n) {
+        const uint32_t first = i;
+        std::vector<Server *> batch;
+        std::vector<uint64_t> at;
+        uint64_t bytes = 0;
+        for (; i < n; i++) {
+            Server &s = servers[i]->s;
+            if (s.mem.empty()) continue;
+            const uint64_t b = (s.flush_staging_bytes() + 15) & ~15ull;
+            if (!batch.empty() && (bytes + b > kFlushManyBytes || batch.size() == PGS_RUN_BUILD_MANY_MAX_JOBS)) break;
+            batch.push_back(&s);
+            at.push_back(bytes);
+            bytes += b;
+        }
+        if (batch.empty()) break;
+        if (done) *done = first;
+        Engine *e = batch[0]->eng;
+        size_t cap = 0;
+        uint8_t *pin = (uint8_t *)e->take_pinned(bytes, &cap);
+        if (!pin) { set_error("flush_many: no pinned staging memory"); return PGS_IO_ERROR; }
+        std::vector<pgs_run_build_job> jobs;
+        for (size_t k = 0; k < batch.size(); k++) jobs.push_back(batch[k]->flush_stage(pin + at[k]));
+        const int32_t st = pgs_run_build_many(jobs.data(), (uint32_t)jobs.size(), nullptr);
+        e->give_pinned(pin, cap);
+        if (st != PGS_OK) return st;
+        for (Server *s : batch) s->flush_commit();
+    }
+    if (done) *done = n;
+    return PGS_OK;
+}
+} // namespace pgs
 struct pgs_response_buf { Resp r; };
 
 extern "C" {
@@ -1036,6 +1125,29 @@ int32_t pgs_rrdb_flush(pgs_server *h, uint32_t now)
     if (st != PGS_OK) return st;
     return h->s.maybe_compact(now);
 }
+// The replicas' memtables built together (flush_many), then the L0 compactions the flushes triggered in one pgs_compact_many.
+int32_t pgs_rrdb_flush_many(pgs_server *const *servers, uint32_t n, uint32_t now)
+{
+    if (n == 0) return PGS_OK;
+    std::vector<std::unique_lock<std::shared_mutex>> held;
+    if (const int32_t st = lock_replicas(servers, n, "rrdb_flush_many", held)) return st;
+    // as pgs_rrdb_flush of each replica in turn: when a build call fails, the replicas in front of it are still compacted
+    uint32_t done = 0;
+    const int32_t flushed = flush_many(servers, n, &done);
+    std::vector<std::vector<uint64_t>> ids(n);
+    std::vector<pgs_filter_params> fps(n);
+    std::vector<pgs_compact_job> jobs;
+    for (uint32_t i = 0; i < done; i++) {
+        Server &s = servers[i]->s;
+        if (!s.l0_triggered()) continue;
+        s.l0_job(ids[i]);
+        if (ids[i].empty()) continue;
+        fps[i] = s.filter();
+        jobs.push_back(pgs_compact_job{s.part, ids[i].data(), (uint32_t)ids[i].size(), 1, -1, &fps[i]});
+    }
+    const int32_t compacted = pgs_compact_many(jobs.data(), (uint32_t)jobs.size(), now, 0, nullptr);
+    return flushed != PGS_OK ? flushed : compacted;
+}
 int32_t pgs_rrdb_manual_compact(pgs_server *h, uint32_t now, pgs_compact_result *out)
 {
     WLOCKED(h);
@@ -1048,32 +1160,18 @@ int32_t pgs_rrdb_manual_compact(pgs_server *h, uint32_t now, pgs_compact_result 
 int32_t pgs_rrdb_manual_compact_many(pgs_server *const *servers, uint32_t n, uint32_t now, pgs_compact_result *out)
 {
     if (n == 0) return PGS_OK;
-    if (!servers) return PGS_INVALID_ARGUMENT;
-    std::vector<Server *> order;
-    for (uint32_t i = 0; i < n; i++) {
-        if (!servers[i]) return PGS_INVALID_ARGUMENT;
-        if (servers[i]->s.part->p.eng != servers[0]->s.part->p.eng) {
-            set_error("rrdb_manual_compact_many: replica %u is on another engine than replica 0", i);
-            return PGS_INVALID_ARGUMENT;
-        }
-        order.push_back(&servers[i]->s);
-    }
-    std::sort(order.begin(), order.end());
-    if (std::adjacent_find(order.begin(), order.end()) != order.end()) {
-        set_error("rrdb_manual_compact_many: a replica given twice");
-        return PGS_INVALID_ARGUMENT;
-    }
     std::vector<std::unique_lock<std::shared_mutex>> held;
-    for (Server *s : order) held.emplace_back(s->mu);
+    if (const int32_t st = lock_replicas(servers, n, "rrdb_manual_compact_many", held)) return st;
     if (out) memset(out, 0, sizeof(pgs_compact_result) * (size_t)n);
-    // do_manual_compact's preparation per replica: flush, fold a stack deeper than one merge, the level of the merge
+    // do_manual_compact's preparation: every memtable flushed (together), then per replica a stack deeper than one merge folded
+    // and the level of the merge chosen
     std::vector<std::vector<uint64_t>> ids(n);
     std::vector<pgs_filter_params> fps(n);
     std::vector<pgs_compact_job> jobs;
     std::vector<uint32_t> which; // the replica of each job (a replica without runs has none)
+    if (const int32_t st = flush_many(servers, n)) return st;
     for (uint32_t i = 0; i < n; i++) {
         Server &s = servers[i]->s;
-        if (const int32_t st = s.flush_mem()) return st;
         auto rs = s.runs();
         if (rs.empty()) continue;
         int32_t level = 1;

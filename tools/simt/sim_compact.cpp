@@ -155,6 +155,8 @@ struct Built { // the run of the last sim_run_build call
     uint64_t data_bytes = 0;
 } g_built;
 
+std::vector<Built> g_built_many; // the runs of the last sim_run_build_many call, one per job
+
 struct Split { // the children of the last sim_split call
     std::vector<HostRun> child;
     std::vector<MergeStats> st;
@@ -762,6 +764,99 @@ void sim_run_build_copy(uint8_t *data, uint64_t *blk_off, uint32_t *blk_size)
 {
     const HostRun &r = g_built.run;
     memcpy(data, r.d_data, g_built.data_bytes);
+    memcpy(blk_off, r.d_blk_off, 8 * (size_t)r.info.n_blocks);
+    memcpy(blk_size, r.d_blk_size, 4 * (size_t)r.info.n_blocks);
+}
+
+// n jobs (their partitions unused) built through build_many_plan / build_many_stage / build_many_buffers /
+// build_many_launch_plan / build_many_launch_blocks and both index passes over every run (index_launch_many), as
+// pgs_run_build_many runs them.  Returns pgs_run_build_many's status and *failed_job (the lowest failing job), or PGS_OK with
+// every job's run kept until the next call (sim_run_build_many_info / _copy read job j's).
+int32_t sim_run_build_many(const pgs_run_build_job *jobs, uint32_t n, uint32_t block_size, uint32_t restart_interval, uint32_t grid_cap,
+                           uint32_t *failed_job)
+{
+    g_built_many.clear();
+    g_built_many.resize(n);
+    *failed_job = 0;
+    std::vector<const pgs_run_build_job *> J;
+    std::vector<uint32_t> which;
+    for (uint32_t i = 0; i < n; i++)
+        if (jobs[i].n) { J.push_back(&jobs[i]); which.push_back(i); }
+    const uint32_t jn = (uint32_t)J.size();
+    if (!jn) return PGS_OK;
+    HostMem scratch;
+    std::vector<uint32_t> job_rec(jn + 1);
+    std::vector<BuildJob> job(jn);
+    BuildManyParams M{};
+    build_many_plan(M, J.data(), jn, job_rec.data(), job.data(), block_size, restart_interval);
+    build_many_stage(M, J.data(), job_rec.data(), job.data(), host_buffers(scratch), [](const void *dst, const void *src, uint64_t bytes) {
+        if (bytes) memcpy((void *)dst, src, bytes);
+    });
+    build_many_buffers(M, host_count_buffers(scratch));
+    build_many_launch_plan(M, grid_cap, nullptr, [](int) {});
+    const BuildSummary sum = *M.B.sum;
+    std::vector<uint32_t> nb(jn);
+    std::vector<uint64_t> bytes(jn);
+    for (uint32_t d = 0; d < jn; d++)
+        if (const int32_t rc = build_many_job(M, sum, M.job_out, M.job_off, d, nb[d], bytes[d])) { *failed_job = which[d]; return rc; }
+    const uint32_t NB = (uint32_t)sum.n_blocks;
+    std::vector<BuildRunOut> outs(jn);
+    for (uint32_t d = 0; d < jn; d++) {
+        Built &R = g_built_many[which[d]];
+        HostRun &r = R.run;
+        host_alloc(r.mem, r.d_data, bytes[d] + 256, 0xEE); // the library's slack, zeroed as the library does
+        memset(r.d_data + bytes[d], 0, 256);
+        host_alloc(r.mem, r.d_blk_off, nb[d] + 1, 0xEE);
+        host_alloc(r.mem, r.d_blk_size, nb[d], 0xEE);
+        R.data_bytes = bytes[d];
+        outs[d] = BuildRunOut{r.d_data, (unsigned long long *)r.d_blk_off, r.d_blk_size};
+    }
+    M.out = outs.data();
+    build_many_launch_blocks(M, NB, grid_cap, nullptr);
+    uint32_t *nrec, *lastlen;
+    IndexStats *stats;
+    host_count_buffers(scratch)(nrec, NB, kNoFill);
+    host_count_buffers(scratch)(lastlen, NB, kNoFill);
+    host_count_buffers(scratch)(stats, jn, kNoFill);
+    std::vector<IndexParams> X(jn);
+    for (uint32_t d = 0; d < jn; d++) {
+        HostRun &r = g_built_many[which[d]].run;
+        X[d] = IndexParams{r.d_data, r.d_blk_off, r.d_blk_size, nb[d]};
+        X[d].nrec = nrec + M.job_out[d];
+        X[d].lastlen = lastlen + M.job_out[d];
+        X[d].stats = stats + d;
+        stats[d] = index_stats_init();
+    }
+    index_launch_many<false>(X.data(), M.job_out, jn, NB, nullptr);
+    for (uint32_t d = 0; d < jn; d++) {
+        HostRun &r = g_built_many[which[d]].run;
+        std::vector<uint32_t> rec_cum(nb[d] + 1), key_cum(nb[d] + 1);
+        if (const int32_t rc = index_buffers(X[d], r, X[d].nrec, X[d].lastlen, stats[d], rec_cum.data(), key_cum.data(), host_count_buffers(r.mem))) {
+            *failed_job = which[d];
+            return rc;
+        }
+        memcpy(r.d_blk_rec, rec_cum.data(), 4 * (nb[d] + 1ull));
+        memcpy(r.d_ikey_off, key_cum.data(), 4 * (nb[d] + 1ull));
+    }
+    index_launch_many<true>(X.data(), M.job_out, jn, NB, nullptr);
+    for (uint32_t d = 0; d < jn; d++) {
+        HostRun &r = g_built_many[which[d]].run;
+        if (stats[d].error) { *failed_job = which[d]; return (int32_t)stats[d].error; }
+        run_info_from_index(stats[d], nb[d], bytes[d], M.job_out[jn + d], r.info);
+    }
+    return PGS_OK;
+}
+// job j of the last sim_run_build_many: its sizes and info (level and run id zero), and its blocks and handles
+void sim_run_build_many_info(uint32_t j, uint64_t *data_bytes, uint32_t *n_blocks, pgs_run_info *info)
+{
+    *data_bytes = g_built_many[j].data_bytes;
+    *n_blocks = g_built_many[j].run.info.n_blocks;
+    *info = g_built_many[j].run.info;
+}
+void sim_run_build_many_copy(uint32_t j, uint8_t *data, uint64_t *blk_off, uint32_t *blk_size)
+{
+    const HostRun &r = g_built_many[j].run;
+    memcpy(data, r.d_data, g_built_many[j].data_bytes);
     memcpy(blk_off, r.d_blk_off, 8 * (size_t)r.info.n_blocks);
     memcpy(blk_size, r.d_blk_size, 4 * (size_t)r.info.n_blocks);
 }

@@ -170,6 +170,7 @@ inline void launch(K kernel, uint32_t grid, uint32_t block, size_t dyn_bytes, A.
 #define __forceinline__ inline
 #define __noinline__
 #define __launch_bounds__(...)
+#define __maxnreg__(...)
 #define __grid_constant__
 #define __restrict__
 #define __align__(n) __attribute__((aligned(n)))
