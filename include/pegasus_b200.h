@@ -361,6 +361,43 @@ typedef struct {
 PGS_API int32_t pgs_partition_split(pgs_partition *src, uint32_t src_count, uint32_t dst_count,
                                     pgs_partition *const *dst, uint32_t n_dst, pgs_split_result *out);
 
+/* One split job of pgs_partition_split_many: a parent partition and its children. */
+typedef struct {
+    pgs_partition *src;        /* parent: index src->pidx of src_count                                         */
+    pgs_partition *const *dst; /* dst_count / src_count children, NULL = child not built                       */
+} pgs_split_job;
+#define PGS_SPLIT_MANY_MAX_JOBS 4096u
+#define PGS_SPLIT_MANY_LAUNCHES 7u
+/* The splits of many parent partitions of one engine (one app's split: every job has the same src_count and dst_count) in one
+ * plan and one set of kernel launches on the engine stream.  Job i is by definition pgs_partition_split(jobs[i].src, src_count,
+ * dst_count, jobs[i].dst, dst_count / src_count, &out[i]): every child gets the same runs, in its parent's run order, with the
+ * same records in the same order and the same tombstones; its pgs_run_info holds the same record and byte totals, and gets and
+ * scans on it answer the same.  Only the block layout may differ: the segments are sized by the weight of the whole launch and
+ * every segment starts a block, so block_bytes, n_blocks and the largest block may differ from the single call.
+ *   launches: PGS_SPLIT_MANY_LAUNCHES (k_plan_many, k_seg_bounds_many, k_seg_layout_many, k_split_walk_many<count>, one host
+ *     wait, k_split_walk_many<write>, k_seg_scan_many, k_emit_many), whatever n is and however many runs the parents hold; four
+ *     when no child receives a record, none when no parent holds a run;
+ *   out (n entries, may be NULL): out[i] = job i's own child[], in_records, in_bytes and dropped_empty; device_ms, kernel_ms,
+ *     count_ms, walk_ms, emit_ms and n_launches are the call's, repeated in every entry.
+ * Statuses, checked before anything is allocated or launched, each with pgs_partition_split's meaning per job:
+ *   jobs == NULL with n > 0, a job without a parent or children, counts or child indices pgs_partition_split refuses, a
+ *   partition that is a parent in one job and a parent or child in another, a child in two jobs, partitions on different
+ *   engines, a child that holds runs: PGS_INVALID_ARGUMENT;
+ *   a child of another data_version, more than PGS_SPLIT_MAX_CHILDREN children, n > PGS_SPLIT_MANY_MAX_JOBS, more than
+ *   PGS_COMPACT_MANY_MAX_JOBS child runs (the sum over every parent run of its job's non-NULL children), or jobs whose joint
+ *   geometry does not fit one launch (the widest user key of any job sizes the key rows of all of them; at most
+ *   PGS_COMPACT_MANY_MAX_JOBS parent runs): PGS_NOT_SUPPORTED -- split the call;
+ *   n == 0: PGS_OK, nothing launched.
+ * pgs_last_error() names the failing job.  All or nothing: on any error (a device allocation failure is PGS_IO_ERROR) no child
+ * changes; the install holds every child's lock, in address order, from the check that it is still empty to the last install.
+ * Device memory, all of it held until the call returns: before the first launch, every parent run's scratch (about 16 +
+ * (27 + the launch's widest user key, rounded up to 4) bytes per record, plus the blocks on its segments' boundaries, plus
+ * 64 bytes per (segment, child)) and a MergeParams and a SplitParams (about 1.8 KB each) per parent run; after the counting
+ * pass, before the writing pass, every child run (about its records' raw key and value bytes plus 23 bytes per record and 20
+ * per block). */
+PGS_API int32_t pgs_partition_split_many(const pgs_split_job *jobs, uint32_t n, uint32_t src_count, uint32_t dst_count,
+                                         pgs_split_result *out);
+
 /* Parse the JSON of the `user_specified_compaction` env (compaction_operation.cpp:162-186) into
  * the binary ops table.  Invalid JSON / rules yield an empty table like the reference.  A pattern
  * longer than 65 535 bytes (it matches no key) is stored as the empty pattern; an op of more than
@@ -756,6 +793,16 @@ PGS_API int32_t pgs_rrdb_manual_compact_many(pgs_server *const *servers, uint32_
  * manual_compact_last_finish_ms.  Errors as pgs_partition_split's; on an error no child changes. */
 PGS_API int32_t pgs_rrdb_split(pgs_server *parent, uint32_t src_count, uint32_t dst_count,
                                pgs_server *const *children, uint32_t n, int64_t *decree_out);
+/* pgs_rrdb_split of each of n parent replicas of one engine, the splits in one pgs_partition_split_many.  children holds
+ * n * (dst_count / src_count) handles, row i = parent i's (NULL: not built).  The children are locked for the whole call.  The
+ * parents' writer locks are taken in address order; every parent's memtable is flushed through the build calls of
+ * pgs_rrdb_flush_many (without its L0 compaction, so each snapshot is the one pgs_rrdb_split takes); each parent's runs,
+ * decree, last_seq and manual_compact_last_finish_ms are snapshotted, and the parents are released.  Each child then gets
+ * what pgs_rrdb_split gives it.  decrees_out (n entries, may be NULL): parent i's split decree.  Refusals: pgs_rrdb_split's,
+ * per row (pgs_last_error() names it), replicas on different engines and a replica given twice: PGS_INVALID_ARGUMENT; then
+ * pgs_partition_split_many's.  On an error no child changes; a memtable already flushed stays flushed. */
+PGS_API int32_t pgs_rrdb_split_many(pgs_server *const *parents, uint32_t n, uint32_t src_count, uint32_t dst_count,
+                                    pgs_server *const *children, int64_t *decrees_out);
 PGS_API int64_t pgs_rrdb_last_flushed_decree(pgs_server *s);
 PGS_API int64_t pgs_rrdb_last_committed_decree(pgs_server *s);
 /* Checkpoints (first slice of SURVEY 8 f4; sync_checkpoint / storage_apply_checkpoint, pegasus_server_impl.cpp:1951-2336).

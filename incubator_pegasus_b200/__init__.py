@@ -104,6 +104,14 @@ class SplitResult(C.Structure):
                 ("walk_ms", C.c_float), ("emit_ms", C.c_float), ("n_launches", C.c_uint32)]
 
 
+class SplitJob(C.Structure):
+    _fields_ = [("src", C.c_void_p), ("dst", C.POINTER(C.c_void_p))]
+
+
+SPLIT_MANY_MAX_JOBS = 4096
+SPLIT_MANY_LAUNCHES = 7
+
+
 class GetResult(C.Structure):
     _fields_ = [("status", C.c_int32), ("expire_ts", C.c_uint32), ("value_off", C.c_uint32),
                 ("value_len", C.c_uint32), ("expired", C.c_uint8), ("reserved", C.c_uint8 * 3)]
@@ -254,6 +262,8 @@ def lib() -> C.CDLL:
         "pgs_get_batch": [vp, vp, vp, C.c_uint32, C.c_uint32, vp, C.c_uint64, vp, u64p],
         "pgs_partition_split": [vp, C.c_uint32, C.c_uint32, C.POINTER(vp), C.c_uint32, C.POINTER(SplitResult)],
         "pgs_rrdb_split": [vp, C.c_uint32, C.c_uint32, C.POINTER(vp), C.c_uint32, C.POINTER(C.c_int64)],
+        "pgs_partition_split_many": [C.POINTER(SplitJob), C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(SplitResult)],
+        "pgs_rrdb_split_many": [C.POINTER(vp), C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(vp), C.POINTER(C.c_int64)],
         "pgs_range_scan": [vp, C.POINTER(ScanRequest), C.c_uint32, vp, C.c_uint64, vp, C.c_uint32, vp, C.c_uint32,
                            C.POINTER(ScanResult)],
         "pgs_rrdb_start": [vp, C.c_int32, C.c_int32, C.POINTER(ServerOptions), C.c_char_p, C.c_uint32, C.POINTER(vp)],
@@ -494,6 +504,20 @@ class Engine:
         _check(lib().pgs_run_build_many(arr if n else None, n, ids.ctypes.data_as(u64p)), "run_build_many")
         return [int(x) for x in ids[:n]]
 
+    def split_many(self, jobs, src_count: int, dst_count: int) -> list[SplitResult]:
+        """pgs_partition_split_many: the splits of many parent partitions of this engine in one set of launches.  A job is
+        (parent Partition, its children as Partition.split takes them); returns one SplitResult per job."""
+        n = len(jobs)
+        arr = (SplitJob * max(1, n))()
+        keep = []  # the child arrays must outlive the call
+        for i, (parent, children) in enumerate(jobs):
+            hs = (C.c_void_p * max(1, len(children)))(*[c.h.value if c is not None else None for c in children])
+            keep.append(hs)
+            arr[i] = SplitJob(parent.h.value if parent is not None else None, C.cast(hs, C.POINTER(C.c_void_p)))
+        res = (SplitResult * max(1, n))()
+        _check(lib().pgs_partition_split_many(arr if n else None, n, src_count, dst_count, res), "partition_split_many")
+        return [res[i] for i in range(n)]
+
     def __enter__(self):
         return self
 
@@ -640,6 +664,18 @@ def rrdb_split(parent, src_count: int, dst_count: int, children) -> int:
     decree = C.c_int64()
     _check(lib().pgs_rrdb_split(parent, src_count, dst_count, handles, len(children), C.byref(decree)), "rrdb_split")
     return decree.value
+
+
+def rrdb_split_many(parents, src_count: int, dst_count: int, children) -> list[int]:
+    """pgs_rrdb_split_many: the pgs_server handles `parents` split together; children[i] is parent i's row of dst_count /
+    src_count child handles (None: not built); returns every parent's split decree"""
+    n = len(parents)
+    flat = [c for row in children for c in row]
+    ph = (C.c_void_p * max(1, n))(*parents)
+    ch = (C.c_void_p * max(1, len(flat)))(*flat)
+    decrees = (C.c_int64 * max(1, n))()
+    _check(lib().pgs_rrdb_split_many(ph, n, src_count, dst_count, ch, decrees), "rrdb_split_many")
+    return [decrees[i] for i in range(n)]
 
 
 def run_build_last_ms() -> list[float]:

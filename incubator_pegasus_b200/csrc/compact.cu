@@ -399,6 +399,8 @@ int32_t split_init_kernels(int max_smem)
         for (bool w : {false, true}) {
             PGS_CUDA(cudaFuncGetAttributes(&a, split_kernel(G, w)));
             PGS_CUDA(cudaFuncSetAttribute(split_kernel(G, w), cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem - (int)a.sharedSizeBytes));
+            PGS_CUDA(cudaFuncGetAttributes(&a, split_many_kernel(G, w)));
+            PGS_CUDA(cudaFuncSetAttribute(split_many_kernel(G, w), cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem - (int)a.sharedSizeBytes));
         }
     return PGS_OK;
 }
@@ -507,10 +509,9 @@ int32_t split_run(Engine *e, const Run &in, const SplitParams &proto, std::vecto
 
 } // namespace
 
-// pgs_partition_split over the runs `snap` of src (nullptr: its current runs); pgs_rrdb_split passes the snapshot it took
-// under the replica's writer lock
-int32_t partition_split(pgs_partition *src, const std::vector<std::shared_ptr<Run>> *snap, uint32_t src_count, uint32_t dst_count,
-                        pgs_partition *const *dst, uint32_t n_dst, pgs_split_result *out)
+namespace {
+// pgs_partition_split's argument checks: the counts, src's index, and every destination (want = bit i for a built child i)
+int32_t split_dests(pgs_partition *src, uint32_t src_count, uint32_t dst_count, pgs_partition *const *dst, uint32_t n_dst, uint32_t &want)
 {
     if (!src || !dst || src_count == 0 || dst_count <= src_count || dst_count % src_count) {
         set_error("partition_split: dst_count %u is not src_count %u times a power of two", dst_count, src_count);
@@ -523,7 +524,7 @@ int32_t partition_split(pgs_partition *src, const std::vector<std::shared_ptr<Ru
         set_error("partition_split: %u destinations for %u -> %u partitions of index %d", n_dst, src_count, dst_count, part.pidx);
         return PGS_INVALID_ARGUMENT;
     }
-    uint32_t want = 0;
+    want = 0;
     for (uint32_t i = 0; i < NC; i++) {
         if (!dst[i]) continue;
         Partition &c = dst[i]->p;
@@ -547,6 +548,20 @@ int32_t partition_split(pgs_partition *src, const std::vector<std::shared_ptr<Ru
         want |= 1u << (i & 31);
     }
     if (NC > kSplitMaxChildren) { set_error("partition_split: %u children > %u", NC, kSplitMaxChildren); return PGS_NOT_SUPPORTED; }
+    return PGS_OK;
+}
+} // namespace
+
+// pgs_partition_split over the runs `snap` of src (nullptr: its current runs); pgs_rrdb_split passes the snapshot it took
+// under the replica's writer lock
+int32_t partition_split(pgs_partition *src, const std::vector<std::shared_ptr<Run>> *snap, uint32_t src_count, uint32_t dst_count,
+                        pgs_partition *const *dst, uint32_t n_dst, pgs_split_result *out)
+{
+    uint32_t want = 0;
+    if (const int32_t rc = split_dests(src, src_count, dst_count, dst, n_dst, want)) return rc;
+    const uint32_t NC = dst_count / src_count;
+    Partition &part = src->p;
+    Engine *e = part.eng;
     std::vector<std::shared_ptr<Run>> runs;
     if (snap) runs = *snap;
     else {
@@ -610,6 +625,302 @@ int32_t partition_split(pgs_partition *src, const std::vector<std::shared_ptr<Ru
     if (out) *out = res;
     return PGS_OK;
 }
+
+// ---- pgs_partition_split_many -------------------------------------------------------------------------------------------------
+// Every run of every parent planned together (split_many_plan) and launched once per phase (split_many_launch).  The parent
+// runs' scratch shares one allocation; each child run keeps buffers of its own, as pgs_partition_split's do.
+int32_t partition_split_many(const pgs_split_job *jobs, uint32_t n, uint32_t src_count, uint32_t dst_count,
+                             const std::vector<std::shared_ptr<Run>> *snaps, pgs_split_result *out)
+{
+    if (n == 0) return PGS_OK;
+    if (!jobs) { set_error("partition_split_many: %u jobs and no job array", n); return PGS_INVALID_ARGUMENT; }
+    if (n > PGS_SPLIT_MANY_MAX_JOBS) { set_error("partition_split_many: %u jobs > %u per call", n, PGS_SPLIT_MANY_MAX_JOBS); return PGS_NOT_SUPPORTED; }
+    const uint32_t n_dst = src_count ? dst_count / src_count : 0;
+    std::vector<uint32_t> want(n);
+    Engine *e = nullptr;
+    for (uint32_t i = 0; i < n; i++) {
+        if (const int32_t rc = split_dests(jobs[i].src, src_count, dst_count, jobs[i].dst, n_dst, want[i])) {
+            const std::string why = pgs_last_error();
+            set_error("partition_split_many: job %u: %s", i, why.c_str());
+            return rc;
+        }
+        if (!e) e = jobs[i].src->p.eng;
+        if (jobs[i].src->p.eng != e) { set_error("partition_split_many: job %u: its parent is on another engine than job 0's", i); return PGS_INVALID_ARGUMENT; }
+    }
+    const uint32_t NC = n_dst;
+    // every partition in one job only: a parent is no other job's parent or child, a child no other job's child
+    std::vector<std::pair<Partition *, uint32_t>> seen;
+    for (uint32_t i = 0; i < n; i++) {
+        seen.emplace_back(&jobs[i].src->p, i);
+        for (uint32_t c = 0; c < NC; c++)
+            if (jobs[i].dst[c]) seen.emplace_back(&jobs[i].dst[c]->p, i);
+    }
+    std::sort(seen.begin(), seen.end());
+    for (size_t x = 1; x < seen.size(); x++)
+        if (seen[x].first == seen[x - 1].first) {
+            set_error("partition_split_many: job %u: a partition of job %u is in job %u too", std::max(seen[x].second, seen[x - 1].second),
+                      std::min(seen[x].second, seen[x - 1].second), std::max(seen[x].second, seen[x - 1].second));
+            return PGS_INVALID_ARGUMENT;
+        }
+
+    // the parent runs, job by job in each parent's order; run x belongs to job run_job[x]
+    std::vector<std::shared_ptr<Run>> in;
+    std::vector<uint32_t> run_job;
+    uint64_t child_runs = 0, emit_segments = 0;
+    for (uint32_t i = 0; i < n; i++) {
+        std::vector<std::shared_ptr<Run>> runs;
+        if (snaps) runs = snaps[i];
+        else {
+            std::lock_guard<std::mutex> g(jobs[i].src->p.mu);
+            runs = jobs[i].src->p.runs;
+        }
+        for (auto &r : runs) {
+            if (r->info.n_records == 0 || r->info.n_blocks == 0) continue;
+            if (r->info.n_blocks >= (1u << 28) || r->info.data_bytes >= (1ull << 40)) {
+                set_error("partition_split_many: job %u: run %llu is too large for a split", i, (unsigned long long)r->id);
+                return PGS_NOT_SUPPORTED;
+            }
+            in.push_back(r);
+            run_job.push_back(i);
+            child_runs += __builtin_popcount(want[i]);
+        }
+    }
+    if (child_runs > kMaxCompactJobs) {
+        set_error("partition_split_many: %llu child runs > %u per call; split the call", (unsigned long long)child_runs, kMaxCompactJobs);
+        return PGS_NOT_SUPPORTED;
+    }
+    const uint32_t nr = (uint32_t)in.size();
+    std::vector<SplitParams> SP(nr);
+    std::vector<CompactTotals> T(nr);
+    for (uint32_t x = 0; x < nr; x++) {
+        SplitParams &s = SP[x];
+        s.M.runs[0] = in[x]->dev();
+        s.M.block_size = e->cfg.block_size;
+        s.M.restart_interval = e->cfg.restart_interval;
+        s.M.data_version = jobs[run_job[x]].src->p.data_version;
+        s.M.crc_table = (const unsigned long long *)e->d_crc;
+        s.S = NC;
+        s.src_count = src_count;
+        s.dst_count = dst_count;
+        s.want = want[run_job[x]];
+        T[x].add(in[x]->info, in[x]->n_bloom_entries);
+    }
+    PGS_CUDA(cudaSetDevice(e->device));
+    cudaStream_t st = e->stream;
+    const uint32_t smem = compact_smem_budget((uint32_t)e->max_smem_optin);
+    SplitJobs J{};
+    MergeJobs M{};
+    SplitGeometry geo{};
+    int occ_w = 0;
+    if (nr) {
+        int32_t rc = split_many_plan(SP.data(), T.data(), nr, smem, J, M, geo);
+        if (rc == PGS_OK) { // second pass: segments sized by the groups the device runs at once
+            PGS_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_w, split_many_kernel(geo.G, false), (int)kSplitThreads, (size_t)geo.walk_dyn));
+            const uint64_t groups = (uint64_t)std::max(1, occ_w) * e->sm_count * (kSplitThreads / geo.G);
+            rc = split_many_plan(SP.data(), T.data(), nr, smem, J, M, geo, groups);
+        }
+        for (uint32_t x = 0; x < nr && rc == PGS_OK; x++) emit_segments += (uint64_t)SP[x].M.Q * __builtin_popcount(SP[x].want);
+        if (rc == PGS_OK && emit_segments > 0x7FFFFFF0ull) rc = PGS_NOT_SUPPORTED;
+        if (rc != PGS_OK) {
+            uint32_t widest = 0;
+            for (auto &t : T) widest = std::max(widest, t.max_ukey);
+            set_error("partition_split_many: %u parent runs (user keys up to %u bytes) into %u children do not fit one launch; split the call", nr, widest, NC);
+            return rc;
+        }
+    }
+
+    pgs_split_result all{}; // the call's timings and launches
+    LaunchScratch S(st);
+    cudaEvent_t t0, t1, ev[5];
+    PGS_CUDA(S.event(t0));
+    PGS_CUDA(S.event(t1));
+    for (auto &x : ev) PGS_CUDA(S.event(x));
+    PGS_CUDA(cudaEventRecord(t0, st));
+    std::vector<MergeStats> hs((size_t)nr * NC, merge_stats_init());
+    std::vector<unsigned long long> prefixes((size_t)nr * NC), dropped(nr);
+    std::vector<std::vector<std::shared_ptr<Run>>> outs(nr, std::vector<std::shared_ptr<Run>>(NC));
+    cudaError_t ce = cudaSuccess;
+    if (nr) {
+        // the scratch in one allocation grouped by fill byte: one pass of split_many_buffers sizes it, a second hands it out
+        std::vector<std::pair<uint64_t, int>> sl;
+        split_many_buffers(SP.data(), nr, J, [&](auto *&p, uint64_t cnt, int fill, bool) { sl.emplace_back(sizeof(*p) * cnt, fill); p = nullptr; });
+        std::vector<int> fills;
+        for (auto &s : sl)
+            if (std::find(fills.begin(), fills.end(), s.second) == fills.end()) fills.push_back(s.second);
+        std::vector<uint64_t> offs(sl.size());
+        std::vector<std::pair<uint64_t, uint64_t>> fill_range(fills.size());
+        uint64_t arena_bytes = 0;
+        for (size_t f = 0; f < fills.size(); f++) {
+            fill_range[f].first = arena_bytes;
+            for (size_t x = 0; x < sl.size(); x++)
+                if (sl[x].second == fills[f]) { offs[x] = arena_bytes; arena_bytes += (std::max<uint64_t>(sl[x].first, 16) + 255) & ~255ull; }
+            fill_range[f].second = arena_bytes;
+        }
+        uint8_t *arena = nullptr;
+        PGS_CUDA(S.alloc(arena, arena_bytes));
+        for (size_t f = 0; f < fills.size(); f++)
+            if (fills[f] != kNoFill) PGS_CUDA(cudaMemsetAsync(arena + fill_range[f].first, fills[f], fill_range[f].second - fill_range[f].first, st));
+        size_t at = 0;
+        split_many_buffers(SP.data(), nr, J, [&](auto *&p, uint64_t, int, bool) { *(void **)&p = arena + offs[at++]; });
+        PGS_CUDA(cudaMemcpyAsync(J.stats, hs.data(), sizeof(MergeStats) * hs.size(), cudaMemcpyHostToDevice, st));
+
+        // the job tables: MergeParams[nr] (the planner's) | SplitParams[nr] | seg_base[nr + 1] | blk_base[nr + 1], in one upload
+        std::vector<MergeParams> MP(nr);
+        for (uint32_t x = 0; x < nr; x++) MP[x] = SP[x].M;
+        const uint64_t o_split = (sizeof(MergeParams) * (uint64_t)nr + 15) & ~15ull;
+        const uint64_t o_seg = (o_split + sizeof(SplitParams) * (uint64_t)nr + 15) & ~15ull, o_blk = (o_seg + 4ull * (nr + 1) + 15) & ~15ull;
+        const uint64_t tab_bytes = o_blk + 4ull * (nr + 1);
+        std::vector<uint8_t> h(tab_bytes, 0);
+        memcpy(h.data(), MP.data(), sizeof(MergeParams) * (size_t)nr);
+        memcpy(h.data() + o_split, SP.data(), sizeof(SplitParams) * (size_t)nr);
+        compact_many_bases(MP.data(), nr, (uint32_t *)(h.data() + o_seg), (uint32_t *)(h.data() + o_blk));
+        uint8_t *tab = nullptr;
+        PGS_CUDA(S.upload(tab, h.data(), tab_bytes));
+        M.job = (const MergeParams *)tab;
+        M.seg_base = J.seg_base = (const uint32_t *)(tab + o_seg);
+        M.blk_base = (const uint32_t *)(tab + o_blk);
+        J.job = (const SplitParams *)(tab + o_split);
+        J.crc_table = (const unsigned long long *)e->d_crc;
+
+        // counting phase, then one read-back of every (job, child) counter, prefix count and dropped count
+        const uint64_t walk_ctas = (uint64_t)std::max(1, occ_w) * e->sm_count;
+        all.n_launches += split_many_launch(J, M, geo, nullptr, CompactGeometry{}, walk_ctas, 0, st,
+                                            [&](int i) { if (ce == cudaSuccess) ce = cudaEventRecord(ev[i], st); });
+        PGS_CUDA(ce);
+        PGS_CUDA(cudaMemcpyAsync(hs.data(), J.stats, sizeof(MergeStats) * hs.size(), cudaMemcpyDeviceToHost, st));
+        PGS_CUDA(cudaMemcpyAsync(prefixes.data(), J.prefixes, 8 * prefixes.size(), cudaMemcpyDeviceToHost, st));
+        PGS_CUDA(cudaMemcpyAsync(dropped.data(), J.dropped, 8 * dropped.size(), cudaMemcpyDeviceToHost, st));
+        cudaError_t se = cudaStreamSynchronize(st);
+        if (se != cudaSuccess) return cuda_fail(se, "multi-job split counting pass");
+        for (size_t y = 0; y < hs.size(); y++)
+            if (hs[y].error) {
+                set_error("partition_split_many: job %u: counting pass failed with status %u (child %u)", run_job[y / NC], hs[y].error, (uint32_t)(y % NC));
+                return (int32_t)hs[y].error;
+            }
+
+        // the children's outputs, sized by what the counting pass found; every (parent run, built child) is a job of k_emit_many
+        std::vector<MergeParams> Pc;
+        std::vector<uint32_t> emit_base(1, 0);
+        CompactGeometry shape{};
+        for (uint32_t x = 0; x < nr; x++)
+            for (uint32_t c = 0; c < NC; c++) {
+                const size_t y = (size_t)x * NC + c;
+                if (!((SP[x].want >> c) & 1u) || hs[y].cnt[EV_OUT] == 0) continue;
+                MergeParams P{};
+                CompactGeometry g{};
+                CompactTotals Tc{};
+                if (!split_many_child(SP[x], c, hs[y], prefixes[y], smem, P, g, Tc, Pc.empty() ? nullptr : &Pc[0], &shape)) {
+                    set_error("partition_split_many: job %u: child %u's run is too large, or not of the launch's shape", run_job[x], c);
+                    return PGS_NOT_SUPPORTED;
+                }
+                auto r = std::make_shared<Run>(e);
+                r->level = in[x]->level;
+                compact_buffers(P, g, Tc, *r, [&](auto *&p, uint64_t cnt, int fill, bool is_out) {
+                    const size_t bytes = sizeof(*p) * cnt;
+                    if (!is_out || ce != cudaSuccess) return; // the scratch is the split's
+                    if ((void *)&p == (void *)&r->d_data) ce = e->alloc_data(*r, bytes);
+                    else ce = cudaMallocAsync((void **)&p, bytes, st); // ~Run frees the run's buffers
+                    if (ce == cudaSuccess && fill != kNoFill) ce = cudaMemsetAsync(p, fill, bytes, st);
+                });
+                PGS_CUDA(ce);
+                if (Pc.empty()) shape = g;
+                Pc.push_back(P);
+                emit_base.push_back(emit_base.back() + P.Q);
+                outs[x][c] = r;
+            }
+        if (!Pc.empty()) { // writing phase
+            const uint32_t nc = (uint32_t)Pc.size();
+            const uint64_t o_base = (sizeof(MergeParams) * (uint64_t)nc + 15) & ~15ull;
+            std::vector<uint8_t> hc(o_base + 4ull * (nc + 1), 0);
+            memcpy(hc.data(), Pc.data(), sizeof(MergeParams) * (size_t)nc);
+            memcpy(hc.data() + o_base, emit_base.data(), 4ull * (nc + 1));
+            uint8_t *ctab = nullptr;
+            PGS_CUDA(S.upload(ctab, hc.data(), hc.size()));
+            MergeJobs E{};
+            E.job = (const MergeParams *)ctab;
+            E.seg_base = (const uint32_t *)(ctab + o_base);
+            E.n = nc;
+            E.Q = emit_base.back();
+            E.ticket = J.ticket + 2;
+            int occ_e = 0;
+            PGS_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_e, k_emit_many, (int)(shape.emit_warps * 32), (size_t)shape.emit_dyn));
+            all.n_launches += split_many_launch(J, M, geo, &E, shape, walk_ctas, (uint64_t)std::max(1, occ_e) * e->sm_count, st,
+                                                [&](int i) { if (ce == cudaSuccess) ce = cudaEventRecord(ev[2 + i], st); });
+            PGS_CUDA(ce);
+            PGS_CUDA(cudaMemcpyAsync(hs.data(), J.stats, sizeof(MergeStats) * hs.size(), cudaMemcpyDeviceToHost, st));
+            se = cudaStreamSynchronize(st);
+            if (se != cudaSuccess) return cuda_fail(se, "multi-job split writing pass");
+            for (size_t y = 0; y < hs.size(); y++)
+                if (hs[y].error) {
+                    set_error("partition_split_many: job %u: writing pass failed with status %u at segment %u (child %u)", run_job[y / NC], hs[y].error,
+                              hs[y].error_seg, (uint32_t)(y % NC));
+                    return (int32_t)hs[y].error;
+                }
+            float ms_walk = 0, ms_emit = 0;
+            cudaEventElapsedTime(&ms_walk, ev[2], ev[4]);
+            cudaEventElapsedTime(&ms_emit, ev[4], ev[3]);
+            all.walk_ms = ms_walk;
+            all.emit_ms = ms_emit;
+        }
+        cudaEventElapsedTime(&all.count_ms, ev[0], ev[1]);
+    }
+    PGS_CUDA(cudaEventRecord(t1, st));
+    PGS_CUDA(cudaEventSynchronize(t1));
+    cudaEventElapsedTime(&all.device_ms, t0, t1);
+    all.kernel_ms = all.count_ms + all.walk_ms + all.emit_ms;
+
+    std::vector<pgs_split_result> res(n, all);
+    for (uint32_t x = 0; x < nr; x++) {
+        pgs_split_result &r = res[run_job[x]];
+        r.in_records += in[x]->info.n_records;
+        r.in_bytes += in[x]->info.raw_key_bytes + in[x]->info.raw_value_bytes;
+        r.dropped_empty += dropped[x];
+        for (uint32_t c = 0; c < NC; c++)
+            if (outs[x][c]) {
+                Run &o = *outs[x][c];
+                pgs_compact_result cr{};
+                o.n_bloom_entries = compact_result_stats(hs[(size_t)x * NC + c], 0, cr, o.info);
+                o.info.level = in[x]->level;
+            }
+    }
+    // all children of all jobs, or none: every child's lock is held (in address order) from the check to the last install
+    std::vector<Partition *> kids;
+    for (uint32_t i = 0; i < n; i++)
+        for (uint32_t c = 0; c < NC; c++)
+            if (jobs[i].dst[c]) kids.push_back(&jobs[i].dst[c]->p);
+    std::sort(kids.begin(), kids.end());
+    std::vector<std::unique_lock<std::mutex>> held;
+    for (Partition *k : kids) held.emplace_back(k->mu);
+    for (uint32_t i = 0; i < n; i++)
+        for (uint32_t c = 0; c < NC; c++)
+            if (jobs[i].dst[c] && !jobs[i].dst[c]->p.runs.empty()) {
+                set_error("partition_split_many: job %u: destination %u took runs during the split", i, c);
+                return PGS_ABORTED;
+            }
+    std::vector<std::vector<std::shared_ptr<Run>>> built((size_t)n * NC); // job i's child c at i * NC + c, in the parent's run order
+    for (uint32_t x = 0; x < nr; x++)
+        for (uint32_t c = 0; c < NC; c++)
+            if (outs[x][c]) built[(size_t)run_job[x] * NC + c].push_back(outs[x][c]);
+    for (uint32_t i = 0; i < n; i++)
+        for (uint32_t c = 0; c < NC; c++) {
+            if (!jobs[i].dst[c]) continue;
+            pgs_split_child_result &cr = res[i].child[c];
+            auto &b = built[(size_t)i * NC + c];
+            for (auto &r : b) {
+                r->id = e->next_run_id++;
+                r->info.run_id = r->id;
+                cr.records += r->info.n_records;
+                cr.tombstones += r->info.n_tombstones;
+                cr.raw_bytes += r->info.raw_key_bytes + r->info.raw_value_bytes;
+                cr.block_bytes += r->info.data_bytes;
+                cr.runs++;
+            }
+            jobs[i].dst[c]->p.runs = b;
+        }
+    e->launches += all.n_launches;
+    if (out) memcpy(out, res.data(), sizeof(pgs_split_result) * (size_t)n);
+    return PGS_OK;
+}
 } // namespace pgs
 
 using namespace pgs;
@@ -618,4 +929,9 @@ extern "C" int32_t pgs_partition_split(pgs_partition *src, uint32_t src_count, u
                                        pgs_split_result *out)
 {
     return partition_split(src, nullptr, src_count, dst_count, dst, n_dst, out);
+}
+
+extern "C" int32_t pgs_partition_split_many(const pgs_split_job *jobs, uint32_t n, uint32_t src_count, uint32_t dst_count, pgs_split_result *out)
+{
+    return partition_split_many(jobs, n, src_count, dst_count, nullptr, out);
 }

@@ -134,6 +134,9 @@ bool scan_stages_every_run(pgs_partition *ph);
 // pgs_partition_split over the runs `snap` of src (nullptr: its current runs)
 int32_t partition_split(pgs_partition *src, const std::vector<std::shared_ptr<Run>> *snap, uint32_t src_count, uint32_t dst_count,
                         pgs_partition *const *dst, uint32_t n_dst, pgs_split_result *out);
+// pgs_partition_split_many over the runs snaps[i] of job i's parent (snaps null: the parents' current runs)
+int32_t partition_split_many(const pgs_split_job *jobs, uint32_t n, uint32_t src_count, uint32_t dst_count,
+                             const std::vector<std::shared_ptr<Run>> *snaps, pgs_split_result *out);
 
 void set_error(const char *fmt, ...);
 int32_t cuda_fail(cudaError_t e, const char *what);

@@ -17,6 +17,9 @@
 //   k_split_walk<write>   the same walk again; each segment's region is divided among the children by the counts, and every
 //                 record leaves as a Desc + key-stream record of its child in the format k_walk hands to k_emit.
 //   k_seg_scan, k_emit    unchanged, once per child over that child's segment aggregates, descriptors and key stream.
+// pgs_partition_split_many runs the same steps over every run of many parents at once: the *_many planner kernels, then
+// k_split_walk_many<count / write> over the launch's segment list, then k_seg_scan_many and k_emit_many over every built child
+// (the end of this file).
 // Nothing is filtered: versions, tombstones, trailers and values stay as they are.  Records with an empty user key (the empty
 // write) are dropped and counted.
 #pragma once
@@ -91,14 +94,14 @@ inline int32_t split_plan(SplitParams &S, const CompactTotals &T, uint32_t max_s
     return PGS_OK;
 }
 
-// The scratch of one parent run's split, as compact_buffers hands it out: buf(pointer, elements, fill, out = false).
+// The per-segment scratch of one parent run's split (its plan, descriptors, key stream and the children's segment tables), as
+// compact_buffers hands it out: buf(pointer, elements, fill, out = false).
 template <class F>
-inline void split_buffers(SplitParams &S, F &&buf)
+inline void split_scratch(SplitParams &S, F &&buf)
 {
     const uint64_t Q = S.M.Q, C = S.S;
     buf(S.M.split_pos, Q + 1, 0xFF, false);
     buf(S.M.split_ref, Q + 1, 0xFF, false);
-    buf(S.M.ticket, 4 + 2 * C, 0, false); // [0] counting walk, [2] writing walk, 4 + 2c: child c's k_emit (its ticket[1])
     buf(S.M.seg, Q, kNoFill, false);
     buf(S.M.desc, S.M.desc_cap, kNoFill, false);
     buf(S.M.kstream, S.M.ks_cap + 64, kNoFill, false);
@@ -106,6 +109,14 @@ inline void split_buffers(SplitParams &S, F &&buf)
     buf(S.lay, C * Q, kNoFill, false);
     buf(S.agg, C * Q, 0, false); // a child that gets nothing from a segment has an empty aggregate
     buf(S.base, C * Q, kNoFill, false);
+}
+// The scratch of one parent run's split: split_scratch, the tickets and the children's counters.
+template <class F>
+inline void split_buffers(SplitParams &S, F &&buf)
+{
+    const uint64_t C = S.S;
+    split_scratch(S, buf);
+    buf(S.M.ticket, 4 + 2 * C, 0, false); // [0] counting walk, [2] writing walk, 4 + 2c: child c's k_emit (its ticket[1])
     buf(S.stats, C, kNoFill, false); // the caller sets every child's to merge_stats_init()
     buf(S.prefixes, C, 0, false);
     buf(S.dropped, 1, 0, false);
@@ -465,6 +476,175 @@ inline uint32_t split_launch(const SplitParams &S, const SplitGeometry &geo, con
             PGS_LAUNCH(k_emit, grid_e, child_geo[i].emit_warps * 32, child_geo[i].emit_dyn, st, Pc);
             n += 2;
         }
+    }
+    mark(1);
+    return n;
+}
+
+// ================================================================================================================================
+// Several splits in one launch (pgs_partition_split_many): every run of every parent partition of one engine is a job, planned
+// with k = 1 by compaction's multi-job planner (compact_many_geometry, k_plan_many, k_seg_bounds_many, k_seg_layout_many), so
+// one segment weight cuts every run.  k_split_walk_many numbers the jobs' segments one after the other, as k_walk_many does,
+// and runs split_segment on each segment's job.  Every (parent run, built child) pair is then one job of k_seg_scan_many and
+// k_emit_many.  The jobs share the launch's shape: the child count S (one app's split per call), and the key rows of the
+// widest user key of any job, so that one group_smem serves the walker and every child's k_emit has the same stages.
+// ================================================================================================================================
+struct SplitJobs {
+    const SplitParams *job;   // [n] in device memory
+    const uint32_t *seg_base; // [n + 1]: job j's segments are the launch's segments [seg_base[j], seg_base[j + 1])
+    uint32_t n, Q;
+    uint32_t S, KSW, group_smem; // every job's
+    const unsigned long long *crc_table;
+    uint32_t *ticket;             // [0] counting walk, [1] writing walk, [2..3] the children's MergeJobs::ticket
+    MergeStats *stats;            // [n * S]: job j's children at j * S (its SplitParams::stats), as are prefixes
+    unsigned long long *prefixes; // [n * S]
+    unsigned long long *dropped;  // [n]
+};
+
+// k_split_walk over the segments of every job.  The groups of a warp may draw segments of different jobs: a group reads its
+// job's SplitParams (and the run table inside it) through the L1 cache, where k_split_walk has its one job as a kernel
+// parameter.  A job whose plan failed is not walked.
+template <uint32_t G, bool WRITE>
+__global__ void __launch_bounds__(kSplitThreads) k_split_walk_many(const __grid_constant__ SplitJobs J)
+{
+    PGS_SMEM_DYN(dyn);
+    const Grp<G> g;
+    constexpr uint32_t NGW = 32 / G; // groups per warp
+    const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    unsigned long long *crc = (unsigned long long *)dyn; // pegasus_key_hash's table, 2 KB
+    for (uint32_t i = threadIdx.x; i < 256; i += blockDim.x) crc[i] = J.crc_table[i];
+    __syncthreads();
+    const uint32_t gi = warp * NGW + g.shift / G;
+    uint8_t *gs = dyn + 2048 + (size_t)gi * J.group_smem;
+    SplitChild *ch = (SplitChild *)gs;
+    CurState *C = (CurState *)(gs + (size_t)J.S * sizeof(SplitChild));
+    uint32_t *row = (uint32_t *)((uint8_t *)C + ((sizeof(CurState) + 15) & ~(size_t)15));
+    uint32_t *prow = row + J.KSW, *rowLO = prow + J.KSW, *rowHI = rowLO + J.KSW;
+#pragma unroll 1
+    for (;;) {
+        uint32_t t0 = 0;
+        if (lane == 0) t0 = atomicAdd(J.ticket + (WRITE ? 1 : 0), NGW);
+        t0 = __shfl_sync(kFull, t0, 0);
+        if (t0 >= J.Q) break;
+        const uint32_t q = t0 + g.shift / G;
+        const uint32_t j = q < J.Q ? job_of(J.seg_base, J.n, q) : 0u;
+        const SplitParams &S = J.job[j];
+        const uint32_t failed = g.shfl(g.gl == 0 ? S.M.stats->error : 0u, 0); // one lane reads the flag for the group
+        const bool en = q < J.Q && failed == 0;
+        split_segment<G, WRITE>(S, g, en, en ? q - J.seg_base[j] : 0u, C, row, prow, rowLO, rowHI, ch, crc);
+    }
+}
+
+typedef void (*split_many_kernel_t)(const SplitJobs);
+inline split_many_kernel_t split_many_kernel(uint32_t G, bool write)
+{
+    switch (G) {
+    case 4: return write ? k_split_walk_many<4, true> : k_split_walk_many<4, false>;
+    case 8: return write ? k_split_walk_many<8, true> : k_split_walk_many<8, false>;
+    case 16: return write ? k_split_walk_many<16, true> : k_split_walk_many<16, false>;
+    default: return write ? k_split_walk_many<32, true> : k_split_walk_many<32, false>;
+    }
+}
+
+// The joint plan of n parent runs (host side).  S[i] holds job i's run (M.runs[0]), block_size, restart_interval, S, counts and
+// want; T[i] its run's totals.  compact_many_geometry sizes every job's key rows by the widest user key and cuts every run by
+// one segment weight from the whole launch's weight (walk_groups = split groups the device runs at once, 0: not known yet;
+// force_weight overrides it); then the narrowest split group that fits, as split_plan chooses it.  J and M (the planner
+// kernels' jobs) get the launch's counts and shape, no pointers.  Returns a status: PGS_NOT_SUPPORTED when the jobs do not fit
+// one launch (the caller can split them).
+inline int32_t split_many_plan(SplitParams *S, const CompactTotals *T, uint32_t n, uint32_t max_smem, SplitJobs &J, MergeJobs &M,
+                               SplitGeometry &geo, uint64_t walk_groups = 0, uint64_t force_weight = 0)
+{
+    if (n == 0 || n > kMaxCompactJobs) return PGS_NOT_SUPPORTED;
+    const uint32_t NC = S[0].S;
+    if (NC < 2 || NC > kSplitMaxChildren) return PGS_NOT_SUPPORTED;
+    std::vector<MergeParams> P(n);
+    std::vector<CompactGeometry> cg(n);
+    for (uint32_t i = 0; i < n; i++) {
+        if (S[i].S != NC) return PGS_INVALID_ARGUMENT;
+        if (T[i].max_ukey > kMaxUkeyLen) return PGS_NOT_SUPPORTED;
+        S[i].M.k = 1;
+        P[i] = S[i].M;
+    }
+    if (!compact_many_geometry(P.data(), T, cg.data(), n, max_smem, M, geo.cg, 0, force_weight, walk_groups)) return PGS_NOT_SUPPORTED;
+    for (uint32_t i = 0; i < n; i++) {
+        S[i].M = P[i];
+        S[i].group_smem = split_group_smem(NC, P[i].KSW);
+    }
+    const uint32_t group_smem = S[0].group_smem;
+    geo.G = 0;
+    for (uint32_t G = 4; G <= 32 && !geo.G; G *= 2) // as split_plan
+        if (split_dyn_smem(G, group_smem) <= max_smem / 2) geo.G = G;
+    for (uint32_t G = 4; G <= 32 && !geo.G; G *= 2)
+        if (split_dyn_smem(G, group_smem) <= max_smem) geo.G = G;
+    if (!geo.G) return PGS_NOT_SUPPORTED;
+    geo.walk_dyn = (uint32_t)split_dyn_smem(geo.G, group_smem);
+    J.n = n;
+    J.Q = M.Q;
+    J.S = NC;
+    J.KSW = S[0].M.KSW;
+    J.group_smem = group_smem;
+    return PGS_OK;
+}
+
+// The scratch of a joint split, every buffer through buf(pointer, elements, fill, out = false) as split_buffers hands them out,
+// in an order that depends only on the plan (the library sizes an arena with one pass and hands it out with a second).
+template <class F>
+inline void split_many_buffers(SplitParams *S, uint32_t n, SplitJobs &J, F &&buf)
+{
+    const uint64_t C = J.S;
+    buf(J.ticket, 4, 0, false);
+    buf(J.stats, n * C, kNoFill, false); // the caller sets every one to merge_stats_init()
+    buf(J.prefixes, n * C, 0, false);
+    buf(J.dropped, n, 0, false);
+    for (uint32_t i = 0; i < n; i++) {
+        split_scratch(S[i], buf);
+        S[i].stats = J.stats + i * C;
+        S[i].prefixes = J.prefixes + i * C;
+        S[i].dropped = J.dropped + i;
+        S[i].M.stats = S[i].stats;
+        S[i].M.ticket = nullptr; // the launch's tickets are J's
+    }
+}
+
+// Child c of job S's k_seg_scan_many / k_emit_many parameters: split_child and split_child_scratch, and the emit shape every
+// child of the launch shares (shape = the first child's; false: this child's differs, or split_child refuses it).
+inline bool split_many_child(const SplitParams &S, uint32_t c, const MergeStats &st, unsigned long long prefixes, uint32_t max_smem,
+                             MergeParams &Pc, CompactGeometry &geo, CompactTotals &T, const MergeParams *shape, const CompactGeometry *shape_geo)
+{
+    if (!split_child(S, st, prefixes, max_smem, Pc, geo, T)) return false;
+    split_child_scratch(S, c, Pc);
+    Pc.ticket = nullptr; // k_emit_many draws from MergeJobs::ticket
+    return !shape || (Pc.KS == shape->KS && Pc.blk_buf == shape->blk_buf && Pc.emit_warp_smem == shape->emit_warp_smem &&
+                      Pc.emit_obuf == shape->emit_obuf && Pc.ks_stage == shape->ks_stage && geo.emit_warps == shape_geo->emit_warps &&
+                      geo.emit_dyn == shape_geo->emit_dyn);
+}
+
+// The launches of a joint split on stream st.  emit == nullptr: the counting phase (k_plan_many, k_seg_bounds_many,
+// k_seg_layout_many over the planner's jobs M, then k_split_walk_many<count>).  Otherwise the writing phase:
+// k_split_walk_many<write>, then k_seg_scan_many and k_emit_many over the children (*emit, every child's shape emit_geo).
+// walk_ctas / emit_ctas = CTAs the device runs at once.  mark(i) as split_launch.  Returns the number of launches.
+template <class Mark>
+inline uint32_t split_many_launch(const SplitJobs &J, const MergeJobs &M, const SplitGeometry &geo, const MergeJobs *emit,
+                                  const CompactGeometry &emit_geo, uint64_t walk_ctas, uint64_t emit_ctas, cudaStream_t st, Mark &&mark)
+{
+    const uint32_t seg_per_cta = kSplitThreads / geo.G;
+    const uint32_t grid_w = (uint32_t)std::min<uint64_t>((J.Q + seg_per_cta - 1) / seg_per_cta, walk_ctas);
+    uint32_t n = 0;
+    mark(0);
+    if (!emit) {
+        PGS_LAUNCH(k_plan_many, std::max(1ull, (M.total_blocks + 255ull) / 256), 256, 0, st, M);
+        PGS_LAUNCH(k_seg_bounds_many, (M.Q + 255ull) / 256, 256, 0, st, M);
+        PGS_LAUNCH(k_seg_layout_many, M.n, 1024, 0, st, M);
+        PGS_LAUNCH(split_many_kernel(geo.G, false), grid_w, kSplitThreads, geo.walk_dyn, st, J);
+        n = 4;
+    } else {
+        PGS_LAUNCH(split_many_kernel(geo.G, true), grid_w, kSplitThreads, geo.walk_dyn, st, J);
+        mark(2);
+        const uint32_t grid_e = (uint32_t)std::min<uint64_t>((emit->Q + emit_geo.emit_warps - 1) / emit_geo.emit_warps, emit_ctas);
+        PGS_LAUNCH(k_seg_scan_many, emit->n, 1024, 0, st, *emit);
+        PGS_LAUNCH(k_emit_many, grid_e, emit_geo.emit_warps * 32, emit_geo.emit_dyn, st, *emit);
+        n = 3;
     }
     mark(1);
     return n;

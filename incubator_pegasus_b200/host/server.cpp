@@ -1326,6 +1326,84 @@ int32_t pgs_rrdb_split(pgs_server *parent, uint32_t src_count, uint32_t dst_coun
     if (decree_out) *decree_out = decree;
     return PGS_OK;
 }
+// pgs_rrdb_split of many replicas (every primary of an app splits at about the same moment; local_partition_split walks every
+// replica of the app on the node): the parents' memtables flushed together (flush_many), their snapshots split in one
+// partition_split_many
+int32_t pgs_rrdb_split_many(pgs_server *const *parents, uint32_t n, uint32_t src_count, uint32_t dst_count, pgs_server *const *children,
+                            int64_t *decrees_out)
+{
+    if (n == 0) return PGS_OK;
+    if (!parents || !children || src_count == 0) return PGS_INVALID_ARGUMENT;
+    const uint32_t S = dst_count / src_count; // a row of children: pgs_rrdb_split's n
+    if (S == 0 || S > 1024) return PGS_INVALID_ARGUMENT;
+    // every replica once, all on one engine; the children stay locked for the whole call
+    std::vector<Server *> kids, all;
+    for (uint32_t i = 0; i < n; i++) {
+        if (!parents[i]) return PGS_INVALID_ARGUMENT;
+        if (parents[i]->s.part->p.eng != parents[0]->s.part->p.eng) {
+            set_error("rrdb_split_many: parent %u is on another engine than parent 0", i);
+            return PGS_INVALID_ARGUMENT;
+        }
+        all.push_back(&parents[i]->s);
+        for (uint32_t c = 0; c < S; c++)
+            if (pgs_server *k = children[(size_t)i * S + c]) {
+                kids.push_back(&k->s);
+                all.push_back(&k->s);
+            }
+    }
+    std::sort(kids.begin(), kids.end());
+    std::sort(all.begin(), all.end());
+    if (std::adjacent_find(all.begin(), all.end()) != all.end()) { set_error("rrdb_split_many: a replica given twice"); return PGS_INVALID_ARGUMENT; }
+    std::vector<std::unique_lock<std::shared_mutex>> held_kids;
+    for (Server *k : kids) held_kids.emplace_back(k->mu);
+    for (uint32_t i = 0; i < n; i++)
+        for (uint32_t c = 0; c < S; c++) {
+            pgs_server *k = children[(size_t)i * S + c];
+            if (!k) continue;
+            const Server &ch = k->s, &p = parents[i]->s;
+            if (!ch.mem.empty() || !k->s.runs().empty() || ch.last_committed_decree != 0 || ch.last_flushed_decree != 0 ||
+                (int64_t)ch.pidx != (int64_t)p.pidx + (int64_t)c * src_count) {
+                set_error("rrdb_split_many: row %u: child %u is not an empty, new replica of index %lld", i, c, (long long)p.pidx + (long long)c * src_count);
+                return PGS_INVALID_ARGUMENT;
+            }
+        }
+    // each parent's state as pgs_rrdb_split fixes it, the memtables flushed together under the parents' writer locks
+    std::vector<std::vector<std::shared_ptr<Run>>> snaps(n);
+    std::vector<int64_t> decree(n);
+    std::vector<uint64_t> last_seq(n), mc_finish(n);
+    {
+        std::vector<std::unique_lock<std::shared_mutex>> held;
+        if (const int32_t st = lock_replicas(parents, n, "rrdb_split_many", held)) return st;
+        if (const int32_t st = flush_many(parents, n)) return st;
+        for (uint32_t i = 0; i < n; i++) {
+            Server &s = parents[i]->s;
+            snaps[i] = s.runs();
+            decree[i] = s.last_flushed_decree;
+            last_seq[i] = s.last_seq;
+            mc_finish[i] = s.manual_compact_last_finish_ms;
+        }
+    }
+    std::vector<pgs_partition *> dst((size_t)n * S, nullptr);
+    std::vector<pgs_split_job> jobs(n);
+    for (uint32_t i = 0; i < n; i++) {
+        for (uint32_t c = 0; c < S; c++)
+            if (pgs_server *k = children[(size_t)i * S + c]) dst[(size_t)i * S + c] = k->s.part;
+        jobs[i] = pgs_split_job{parents[i]->s.part, dst.data() + (size_t)i * S};
+    }
+    if (const int32_t st = partition_split_many(jobs.data(), n, src_count, dst_count, snaps.data(), nullptr)) return st;
+    for (uint32_t i = 0; i < n; i++) {
+        for (uint32_t c = 0; c < S; c++)
+            if (pgs_server *k = children[(size_t)i * S + c]) {
+                Server &ch = k->s;
+                ch.last_seq = last_seq[i]; // new writes on the child win over every copied version
+                ch.last_committed_decree = ch.last_flushed_decree = decree[i];
+                ch.last_durable_decree = 0;
+                ch.manual_compact_last_finish_ms = mc_finish[i];
+            }
+        if (decrees_out) decrees_out[i] = decree[i];
+    }
+    return PGS_OK;
+}
 int64_t pgs_rrdb_last_flushed_decree(pgs_server *h) { RLOCKED(h); return h->s.last_flushed_decree; }
 int64_t pgs_rrdb_last_committed_decree(pgs_server *h) { RLOCKED(h); return h->s.last_committed_decree; }
 

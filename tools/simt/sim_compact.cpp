@@ -164,6 +164,8 @@ struct Split { // the children of the last sim_split call
     uint32_t Q = 0;
 } g_split;
 
+std::vector<Split> g_split_many; // the children of the last sim_split_many call, one Split per parent run
+
 } // namespace
 
 extern "C" {
@@ -678,6 +680,115 @@ int32_t sim_split_child_bloom_check(uint32_t c, const uint8_t *key, uint32_t len
 {
     const HostRun &r = g_split.child[c];
     return bloom_may_contain(r.d_bloom, r.bloom_lines, bloom_hash_bytes(key, len)) ? 1 : 0;
+}
+
+// n parent runs split together into dst_count / src_count children each, through split_many_plan / split_many_buffers /
+// split_many_child / split_many_launch, as pgs_partition_split_many runs them.  Run i comes from the flat arrays; want[i] = its
+// built children (bit c).  seg_weight: the launch's one segment weight (0: the product's default budget).  Returns a status
+// (pgs_partition_split_many's for the child-run count and the joint plan); dropped[i] = run i's empty writes, *launches = the
+// launches made.  Every run's children stay until the next call: sim_split_many_select(i) makes run i's the ones
+// sim_split_child_* read.
+int32_t sim_split_many(uint32_t n, const uint8_t **data, const uint64_t *data_bytes, const uint64_t **blk_off, const uint32_t **blk_size,
+                       const uint32_t *n_blocks, const uint32_t *want, uint32_t block_size, uint32_t restart_interval, uint32_t src_count,
+                       uint32_t dst_count, uint64_t seg_weight, uint64_t *dropped, uint32_t *launches)
+{
+    g_split_many.clear();
+    *launches = 0;
+    if (n == 0 || src_count == 0 || dst_count % src_count) return PGS_INVALID_ARGUMENT;
+    const uint32_t NC = dst_count / src_count;
+    std::vector<HostRun> in(n);
+    for (uint32_t i = 0; i < n; i++)
+        if (const int32_t rc = load_run(in[i], data[i], data_bytes[i], blk_off[i], blk_size[i], n_blocks[i])) return rc;
+    crc64_make_table(crc_tab);
+    std::vector<SplitParams> SP(n);
+    std::vector<CompactTotals> T(n);
+    uint64_t child_runs = 0;
+    for (uint32_t i = 0; i < n; i++) {
+        SplitParams &s = SP[i];
+        s.M.runs[0] = in[i].dev();
+        s.M.block_size = block_size;
+        s.M.restart_interval = restart_interval;
+        s.M.data_version = 1;
+        s.M.crc_table = (const unsigned long long *)crc_tab;
+        s.S = NC; s.src_count = src_count; s.dst_count = dst_count; s.want = want[i];
+        T[i].add(in[i].info, in[i].n_bloom_entries);
+        child_runs += __builtin_popcount(want[i]);
+    }
+    if (child_runs > kMaxCompactJobs) return PGS_NOT_SUPPORTED;
+    const uint32_t smem = compact_smem_budget(kSimSmemOptin);
+    SplitJobs J{};
+    MergeJobs M{};
+    SplitGeometry geo{};
+    if (const int32_t rc = split_many_plan(SP.data(), T.data(), n, smem, J, M, geo, 0, seg_weight)) return rc;
+    HostMem scratch;
+    split_many_buffers(SP.data(), n, J, host_count_buffers(scratch));
+    for (uint64_t y = 0; y < (uint64_t)n * NC; y++) J.stats[y] = merge_stats_init();
+    std::vector<MergeParams> MP(n);
+    for (uint32_t i = 0; i < n; i++) MP[i] = SP[i].M;
+    std::vector<uint32_t> seg_base(n + 1), blk_base(n + 1);
+    compact_many_bases(MP.data(), n, seg_base.data(), blk_base.data());
+    M.job = MP.data();
+    M.seg_base = J.seg_base = seg_base.data();
+    M.blk_base = blk_base.data();
+    J.job = SP.data();
+    J.crc_table = (const unsigned long long *)crc_tab;
+    *launches += split_many_launch(J, M, geo, nullptr, CompactGeometry{}, 2, 0, nullptr, [](int) {});
+    g_split_many.resize(n);
+    for (uint32_t i = 0; i < n; i++) {
+        dropped[i] = J.dropped[i];
+        Split &R = g_split_many[i];
+        R.child.resize(NC);
+        R.built.assign(NC, 0);
+        R.st.assign(SP[i].stats, SP[i].stats + NC);
+        R.Q = SP[i].M.Q;
+        for (uint32_t c = 0; c < NC; c++)
+            if (R.st[c].error) { fprintf(stderr, "sim_split_many: run %u: counting pass status %u (child %u)\n", i, R.st[c].error, c); return (int32_t)R.st[c].error; }
+    }
+    std::vector<MergeParams> Pc;
+    std::vector<uint32_t> emit_base(1, 0);
+    CompactGeometry shape{};
+    for (uint32_t i = 0; i < n; i++)
+        for (uint32_t c = 0; c < NC; c++) {
+            Split &R = g_split_many[i];
+            if (!((want[i] >> c) & 1u) || R.st[c].cnt[EV_OUT] == 0) continue;
+            MergeParams P{};
+            CompactGeometry g{};
+            CompactTotals Tc{};
+            if (!split_many_child(SP[i], c, R.st[c], SP[i].prefixes[c], smem, P, g, Tc, Pc.empty() ? nullptr : &Pc[0], &shape)) return PGS_NOT_SUPPORTED;
+            HostRun &run = R.child[c];
+            compact_buffers(P, g, Tc, run, [&](auto *&p, uint64_t cnt, int fill, bool out) { if (out) host_count_buffers(run.mem)(p, cnt, fill); });
+            if (Pc.empty()) shape = g;
+            Pc.push_back(P);
+            emit_base.push_back(emit_base.back() + P.Q);
+            R.built[c] = 1;
+        }
+    if (!Pc.empty()) {
+        MergeJobs E{};
+        E.job = Pc.data();
+        E.seg_base = emit_base.data();
+        E.n = (uint32_t)Pc.size();
+        E.Q = emit_base.back();
+        E.ticket = J.ticket + 2;
+        *launches += split_many_launch(J, M, geo, &E, shape, 2, 2, nullptr, [](int) {});
+    }
+    for (uint32_t i = 0; i < n; i++) {
+        Split &R = g_split_many[i];
+        R.st.assign(SP[i].stats, SP[i].stats + NC);
+        for (uint32_t c = 0; c < NC; c++) {
+            if (R.st[c].error) { fprintf(stderr, "sim_split_many: run %u: status %u at segment %u (child %u)\n", i, R.st[c].error, R.st[c].error_seg, c); return (int32_t)R.st[c].error; }
+            if (!R.built[c]) continue;
+            pgs_compact_result cr{};
+            R.child[c].n_bloom_entries = compact_result_stats(R.st[c], 0, cr, R.child[c].info);
+        }
+    }
+    return PGS_OK;
+}
+// run i of the last sim_split_many becomes the one sim_split_child_* read
+int32_t sim_split_many_select(uint32_t i)
+{
+    if (i >= g_split_many.size()) return PGS_INVALID_ARGUMENT;
+    g_split = g_split_many[i];
+    return PGS_OK;
 }
 
 } // extern "C"
