@@ -33,6 +33,81 @@ int32_t compact_init_kernels(int max_smem)
 }
 } // namespace pgs
 
+namespace pgs {
+namespace {
+
+// PGS_WALK_G (diagnostics): the lanes per merge group of every compaction's walk, 1, 2, 4, 8 or 16 (0: the planner's choice)
+uint32_t walk_g_override()
+{
+    const char *ev = getenv("PGS_WALK_G");
+    const int v = ev ? atoi(ev) : 0;
+    return v == 1 || v == 2 || v == 4 || v == 8 || v == 16 ? (uint32_t)v : 0u;
+}
+
+// A compaction job's k input runs, looked up by id under part's lock, and the bottommost < 0 rule: true iff every run outside
+// the inputs is newer than every input.  Refuses an unknown run and a run given twice, with a message that starts with who.
+int32_t compact_inputs(Partition &part, const uint64_t *run_ids, uint32_t k, int32_t &bottommost, std::vector<std::shared_ptr<Run>> &in,
+                       const char *who)
+{
+    std::lock_guard<std::mutex> g(part.mu);
+    for (uint32_t i = 0; i < k; i++) {
+        auto r = part.find(run_ids[i]);
+        if (!r) { set_error("%s unknown run %llu", who, (unsigned long long)run_ids[i]); return PGS_NOT_FOUND; }
+        if (std::find(in.begin(), in.end(), r) != in.end()) { set_error("%s run %llu given twice", who, (unsigned long long)run_ids[i]); return PGS_INVALID_ARGUMENT; }
+        in.push_back(r);
+    }
+    if (bottommost < 0) {
+        size_t first_in = part.runs.size();
+        for (size_t i = 0; i < part.runs.size(); i++)
+            if (std::find(in.begin(), in.end(), part.runs[i]) != in.end()) { first_in = i; break; }
+        bottommost = 1;
+        for (size_t i = first_in; i < part.runs.size(); i++)
+            if (std::find(in.begin(), in.end(), part.runs[i]) == in.end()) bottommost = 0;
+    }
+    return PGS_OK;
+}
+
+// n finished merges installed, all or none (many: with pgs_compact_many's messages).  Every partition's lock is held from the
+// check that each job's inputs in[i] are still in parts[i] (PGS_ABORTED otherwise: pgs_run_drop took one during the merge) to
+// the last install.  Job i's inputs leave unless KEEP_INPUTS, its output outr[i] goes in unless it is empty or DISCARD_OUTPUT,
+// and out[i] (if out) = res's launches and times with job i's counters, segments and new run id.
+int32_t compact_install(uint32_t n, Partition *const *parts, const std::vector<std::shared_ptr<Run>> *in, const std::shared_ptr<Run> *outr,
+                        const MergeStats *hs, const MergeParams *P, const CompactTotals *T, const pgs_compact_result &res, uint32_t flags,
+                        bool many, pgs_compact_result *out)
+{
+    Engine *e = parts[0]->eng;
+    std::vector<pgs_compact_result> r(n, res);
+    for (uint32_t i = 0; i < n; i++) {
+        outr[i]->n_bloom_entries = compact_result_stats(hs[i], T[i].in_block_bytes, r[i], outr[i]->info);
+        outr[i]->info.level = outr[i]->level;
+        r[i].n_tiles = P[i].Q;
+    }
+    const auto held = lock_partitions(std::vector<Partition *>(parts, parts + n));
+    for (uint32_t i = 0; i < n; i++)
+        for (auto &x : in[i])
+            if (std::find(parts[i]->runs.begin(), parts[i]->runs.end(), x) == parts[i]->runs.end()) {
+                if (many) set_error("compact_many: job %u: run %llu left the partition during the merge", i, (unsigned long long)x->id);
+                else set_error("compact: run %llu left the partition during the merge", (unsigned long long)x->id);
+                return PGS_ABORTED;
+            }
+    for (uint32_t i = 0; i < n; i++) {
+        Partition &part = *parts[i];
+        if (!(flags & PGS_COMPACT_KEEP_INPUTS))
+            for (auto &x : in[i]) part.runs.erase(std::find(part.runs.begin(), part.runs.end(), x));
+        if (hs[i].tot_blocks > 0 && !(flags & PGS_COMPACT_DISCARD_OUTPUT)) {
+            outr[i]->id = e->next_run_id++;
+            outr[i]->info.run_id = outr[i]->id;
+            part.insert(outr[i]);
+            r[i].new_run_id = outr[i]->id;
+        }
+    }
+    if (out) memcpy(out, r.data(), sizeof(pgs_compact_result) * (size_t)n);
+    return PGS_OK;
+}
+
+} // namespace
+} // namespace pgs
+
 using namespace pgs;
 
 extern "C" int32_t pgs_compact(pgs_partition *ph, const uint64_t *run_ids, uint32_t k, int32_t out_level,
@@ -47,59 +122,25 @@ extern "C" int32_t pgs_compact_ex(pgs_partition *ph, const uint64_t *run_ids, ui
                                   pgs_compact_result *out)
 {
     if (!ph || !run_ids || k == 0 || out_level < 0) return PGS_INVALID_ARGUMENT;
-    Partition &part = ph->p;
+    Partition &part = ph->p, *parts = &part;
     Engine *e = part.eng;
-    pgs_compact_result res{};
     std::vector<std::shared_ptr<Run>> in;
-    {
-        std::lock_guard<std::mutex> g(part.mu);
-        for (uint32_t i = 0; i < k; i++) {
-            auto r = part.find(run_ids[i]);
-            if (!r) { set_error("compact: unknown run %llu", (unsigned long long)run_ids[i]); return PGS_NOT_FOUND; }
-            for (auto &x : in) if (x == r) return PGS_INVALID_ARGUMENT;
-            in.push_back(r);
-        }
-        if (bottommost < 0) { // true iff every run outside the input set is newer than every input
-            size_t first_in = part.runs.size();
-            for (size_t i = 0; i < part.runs.size(); i++)
-                if (std::find(in.begin(), in.end(), part.runs[i]) != in.end()) { first_in = i; break; }
-            bottommost = 1;
-            for (size_t i = first_in; i < part.runs.size(); i++)
-                if (std::find(in.begin(), in.end(), part.runs[i]) == in.end()) bottommost = 0;
-        }
-    }
-    if (k > kMaxRuns) { set_error("compact: %u runs > %u per merge", k, kMaxRuns); return PGS_NOT_SUPPORTED; }
+    if (const int32_t rc = compact_inputs(part, run_ids, k, bottommost, in, "compact:")) return rc;
+    MergeParams P{};
+    CompactTotals T{};
+    uint32_t ops_len = 0;
+    if (const int32_t rc = compact_job_params(P, T, k, [&](uint32_t i) -> const Run & { return *in[i]; }, e->cfg.block_size, e->cfg.restart_interval,
+                                              bottommost, now, part.data_version, fp, (const unsigned long long *)e->d_crc, ops_len, "compact:"))
+        return rc;
     PGS_CUDA(cudaSetDevice(e->device));
     cudaStream_t st = e->stream;
-
-    MergeParams P{};
-    P.k = k;
-    CompactTotals T{};
-    for (uint32_t i = 0; i < k; i++) {
-        P.runs[i] = in[i]->dev();
-        const pgs_run_info &fi = in[i]->info;
-        T.add(fi, in[i]->n_bloom_entries);
-        if (fi.n_blocks >= (1u << 28) || fi.data_bytes >= (1ull << 40)) return PGS_NOT_SUPPORTED;
-    }
-    if (T.max_ukey > kMaxUkeyLen) { set_error("compact: user key of %u bytes > %u", T.max_ukey, kMaxUkeyLen); return PGS_NOT_SUPPORTED; }
-    P.block_size = e->cfg.block_size;
-    P.restart_interval = e->cfg.restart_interval;
-    P.bottommost = bottommost ? 1 : 0;
-    P.now = now;
-    P.data_version = part.data_version;
-    uint32_t ops_len = 0;
-    if (!compact_filter(P, fp, ops_len)) { set_error("compact: malformed ops table of %u bytes", fp->ops_len); return PGS_INVALID_ARGUMENT; }
-    if (P.validate_hash) P.crc_table = (const unsigned long long *)e->d_crc;
     CompactGeometry geo{};
-    uint32_t force_G = 0; // diagnostics: PGS_WALK_G = lanes per merge group (1, 2, 4, 8, 16)
-    if (const char *ev = getenv("PGS_WALK_G")) { const int v = atoi(ev); if (v == 1 || v == 2 || v == 4 || v == 8 || v == 16) force_G = (uint32_t)v; }
     const uint32_t smem = compact_smem_budget((uint32_t)e->max_smem_optin);
-    bool geo_ok = compact_geometry(P, T, smem, geo, force_G);
+    Resident walk{};
+    bool geo_ok = compact_geometry(P, T, smem, geo, walk_g_override());
     if (geo_ok) { // second pass: the segment budget follows from how many groups the device runs at once
-        int occ = 0;
-        PGS_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, walk_kernel(geo.G), (int)kWalkThreads, (size_t)geo.walk_dyn));
-        const uint64_t groups = (uint64_t)std::max(1, occ) * e->sm_count * (kWalkThreads / geo.G);
-        geo_ok = compact_geometry(P, T, smem, geo, geo.G, 0, groups);
+        PGS_CUDA(resident(*e, walk_kernel(geo.G), kWalkThreads, geo.G, geo.walk_dyn, walk));
+        geo_ok = compact_geometry(P, T, smem, geo, geo.G, 0, walk.groups);
     }
     if (!geo_ok) {
         set_error("compact: input too large for one merge launch (keys of %u bytes, %llu records)", T.max_ukey, (unsigned long long)T.n_rec);
@@ -110,13 +151,9 @@ extern "C" int32_t pgs_compact_ex(pgs_partition *ph, const uint64_t *run_ids, ui
     auto outr = std::make_shared<Run>(e);
     outr->level = out_level;
     cudaError_t ce = cudaSuccess;
-    compact_buffers(P, geo, T, *outr, [&](auto *&p, uint64_t n, int fill, bool out) {
-        const size_t bytes = sizeof(*p) * n;
-        if (ce != cudaSuccess) return;
-        if ((void *)&p == (void *)&outr->d_data) ce = e->alloc_data(*outr, bytes); // from the spare list when one fits
-        else ce = out ? cudaMallocAsync((void **)&p, bytes, st) : S.alloc(p, bytes); // ~Run frees the run's buffers
-        if (ce == cudaSuccess && fill != kNoFill) ce = cudaMemsetAsync(p, fill, bytes, st);
-    });
+    auto keep = run_buffers(e, *outr, ce);
+    auto scratch = scratch_buffers(S, ce);
+    compact_buffers(P, geo, T, *outr, [&](auto *&p, uint64_t n, int fill, bool is_out) { if (is_out) keep(p, n, fill); else scratch(p, n, fill); });
     PGS_CUDA(ce);
     MergeStats hs = merge_stats_init();
     PGS_CUDA(S.upload(P.stats, &hs, 1));
@@ -124,43 +161,25 @@ extern "C" int32_t pgs_compact_ex(pgs_partition *ph, const uint64_t *run_ids, ui
 
     cudaEvent_t ev[4];
     for (auto &x : ev) PGS_CUDA(S.event(x));
-    int occ_w = 0, occ_e = 0;
-    PGS_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_w, walk_kernel(geo.G), (int)kWalkThreads, (size_t)geo.walk_dyn));
-    PGS_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_e, k_emit, (int)(geo.emit_warps * 32), (size_t)geo.emit_dyn));
-    const uint32_t launches = compact_launch(P, geo, (uint64_t)std::max(1, occ_w) * e->sm_count, (uint64_t)std::max(1, occ_e) * e->sm_count,
-                                             st, [&](int i) { if (ce == cudaSuccess) ce = cudaEventRecord(ev[i], st); });
+    Resident emit{};
+    PGS_CUDA(resident(*e, k_emit, geo.emit_warps * 32, 32, geo.emit_dyn, emit));
+    const uint32_t launches = compact_launch(P, geo, walk.ctas, emit.ctas, st, [&](int i) { if (ce == cudaSuccess) ce = cudaEventRecord(ev[i], st); });
     e->launches += launches;
     PGS_CUDA(ce);
     PGS_CUDA(cudaMemcpyAsync(&hs, P.stats, sizeof hs, cudaMemcpyDeviceToHost, st));
     cudaError_t se = cudaStreamSynchronize(st);
     if (se != cudaSuccess) return cuda_fail(se, "compaction kernels");
-    float ms_total = 0, ms_merge = 0, ms_walk = 0, ms_emit = 0;
-    cudaEventElapsedTime(&ms_total, ev[0], ev[3]);
-    cudaEventElapsedTime(&ms_merge, ev[1], ev[3]);
-    cudaEventElapsedTime(&ms_walk, ev[1], ev[2]);
-    cudaEventElapsedTime(&ms_emit, ev[2], ev[3]);
+    pgs_compact_result res{};
+    res.n_launches = launches;
+    cudaEventElapsedTime(&res.device_ms, ev[0], ev[3]);
+    cudaEventElapsedTime(&res.merge_kernel_ms, ev[1], ev[3]);
+    cudaEventElapsedTime(&res.walk_ms, ev[1], ev[2]);
+    cudaEventElapsedTime(&res.emit_ms, ev[2], ev[3]);
     if (hs.error) {
         set_error("compaction kernel failed with status %u at segment %u of %u", hs.error, hs.error_seg, P.Q);
         return (int32_t)hs.error;
     }
-    outr->n_bloom_entries = compact_result_stats(hs, T.in_block_bytes, res, outr->info);
-    outr->info.level = out_level;
-    res.n_tiles = P.Q; res.n_launches = launches;
-    res.device_ms = ms_total; res.merge_kernel_ms = ms_merge;
-    res.walk_ms = ms_walk; res.emit_ms = ms_emit;
-    {
-        std::lock_guard<std::mutex> g(part.mu);
-        if (!(flags & PGS_COMPACT_KEEP_INPUTS))
-            for (auto &r : in) part.runs.erase(std::find(part.runs.begin(), part.runs.end(), r));
-        if (hs.tot_blocks > 0 && !(flags & PGS_COMPACT_DISCARD_OUTPUT)) {
-            outr->id = e->next_run_id++;
-            outr->info.run_id = outr->id;
-            part.insert(outr);
-            res.new_run_id = outr->id;
-        }
-    }
-    if (out) *out = res;
-    return PGS_OK;
+    return compact_install(1, &parts, &in, &outr, &hs, &P, &T, res, flags, false, out);
 }
 
 // ---- pgs_compact_many --------------------------------------------------------------------------------------------------------
@@ -171,7 +190,7 @@ extern "C" int32_t pgs_compact_many(const pgs_compact_job *jobs, uint32_t n, uin
     if (n == 0) return PGS_OK;
     if (!jobs) { set_error("compact_many: %u jobs and no job array", n); return PGS_INVALID_ARGUMENT; }
     if (n > kMaxCompactJobs) { set_error("compact_many: %u jobs > %u per call", n, kMaxCompactJobs); return PGS_NOT_SUPPORTED; }
-    Engine *e = nullptr;
+    JobPartitions set;
     std::vector<Partition *> parts(n);
     for (uint32_t i = 0; i < n; i++) {
         const pgs_compact_job &J = jobs[i];
@@ -180,80 +199,41 @@ extern "C" int32_t pgs_compact_many(const pgs_compact_job *jobs, uint32_t n, uin
             return PGS_INVALID_ARGUMENT;
         }
         parts[i] = &J.part->p;
-        if (!e) e = parts[i]->eng;
-        if (parts[i]->eng != e) { set_error("compact_many: job %u: its partition is on another engine than job 0's", i); return PGS_INVALID_ARGUMENT; }
+        if (!set.add(*parts[i], i)) { set_error("compact_many: job %u: its partition is on another engine than job 0's", i); return PGS_INVALID_ARGUMENT; }
     }
-    std::vector<Partition *> order = parts; // the install locks them in this order
-    std::sort(order.begin(), order.end());
-    for (uint32_t i = 1; i < n; i++)
-        if (order[i] == order[i - 1]) {
-            const uint32_t j = (uint32_t)(std::find(parts.begin(), parts.end(), order[i]) - parts.begin());
-            set_error("compact_many: job %u: its partition is in another job too", j);
-            return PGS_INVALID_ARGUMENT;
-        }
+    uint32_t a = 0, b = 0;
+    if (set.twice(a, b)) { set_error("compact_many: job %u: its partition is in another job too", a); return PGS_INVALID_ARGUMENT; }
+    Engine *e = set.e;
+    char who_buf[40];
+    auto who = [&](uint32_t i) { snprintf(who_buf, sizeof who_buf, "compact_many: job %u:", i); return who_buf; };
 
-    // the inputs and the bottommost rule of every job, as pgs_compact_ex finds them
+    // the inputs and the bottommost rule of every job, then every job's limits and filter, as pgs_compact_ex checks them
     std::vector<std::vector<std::shared_ptr<Run>>> in(n);
     std::vector<int32_t> bottom(n);
     for (uint32_t i = 0; i < n; i++) {
-        const pgs_compact_job &J = jobs[i];
-        Partition &part = *parts[i];
-        std::lock_guard<std::mutex> g(part.mu);
-        for (uint32_t x = 0; x < J.k; x++) {
-            auto r = part.find(J.run_ids[x]);
-            if (!r) { set_error("compact_many: job %u: unknown run %llu", i, (unsigned long long)J.run_ids[x]); return PGS_NOT_FOUND; }
-            for (auto &y : in[i])
-                if (y == r) { set_error("compact_many: job %u: run %llu given twice", i, (unsigned long long)J.run_ids[x]); return PGS_INVALID_ARGUMENT; }
-            in[i].push_back(r);
-        }
-        bottom[i] = J.bottommost;
-        if (bottom[i] < 0) {
-            size_t first_in = part.runs.size();
-            for (size_t x = 0; x < part.runs.size(); x++)
-                if (std::find(in[i].begin(), in[i].end(), part.runs[x]) != in[i].end()) { first_in = x; break; }
-            bottom[i] = 1;
-            for (size_t x = first_in; x < part.runs.size(); x++)
-                if (std::find(in[i].begin(), in[i].end(), part.runs[x]) == in[i].end()) bottom[i] = 0;
-        }
+        bottom[i] = jobs[i].bottommost;
+        if (const int32_t rc = compact_inputs(*parts[i], jobs[i].run_ids, jobs[i].k, bottom[i], in[i], who(i))) return rc;
     }
     std::vector<MergeParams> P(n);
     std::vector<CompactTotals> T(n);
     std::vector<uint32_t> ops_len(n);
-    uint64_t ops_total = 0;
     uint32_t any_hash = 0;
     for (uint32_t i = 0; i < n; i++) {
-        const pgs_compact_job &J = jobs[i];
-        if (J.k > kMaxRuns) { set_error("compact_many: job %u: %u runs > %u per merge", i, J.k, kMaxRuns); return PGS_NOT_SUPPORTED; }
-        MergeParams &p = P[i];
-        p.k = J.k;
-        for (uint32_t x = 0; x < J.k; x++) {
-            p.runs[x] = in[i][x]->dev();
-            const pgs_run_info &fi = in[i][x]->info;
-            T[i].add(fi, in[i][x]->n_bloom_entries);
-            if (fi.n_blocks >= (1u << 28) || fi.data_bytes >= (1ull << 40)) { set_error("compact_many: job %u: a run too large for a merge", i); return PGS_NOT_SUPPORTED; }
-        }
-        if (T[i].max_ukey > kMaxUkeyLen) { set_error("compact_many: job %u: user key of %u bytes > %u", i, T[i].max_ukey, kMaxUkeyLen); return PGS_NOT_SUPPORTED; }
-        p.block_size = e->cfg.block_size;
-        p.restart_interval = e->cfg.restart_interval;
-        p.bottommost = bottom[i] ? 1 : 0;
-        p.now = now;
-        p.data_version = parts[i]->data_version;
-        if (!compact_filter(p, J.fp, ops_len[i])) { set_error("compact_many: job %u: malformed ops table of %u bytes", i, J.fp->ops_len); return PGS_INVALID_ARGUMENT; }
-        if (p.validate_hash) { p.crc_table = (const unsigned long long *)e->d_crc; any_hash = 1; }
-        ops_total += (ops_len[i] + 15) & ~15u;
+        if (const int32_t rc = compact_job_params(P[i], T[i], jobs[i].k, [&](uint32_t x) -> const Run & { return *in[i][x]; }, e->cfg.block_size,
+                                                  e->cfg.restart_interval, bottom[i], now, parts[i]->data_version, jobs[i].fp,
+                                                  (const unsigned long long *)e->d_crc, ops_len[i], who(i)))
+            return rc;
+        if (P[i].validate_hash) any_hash = 1;
     }
     MergeJobs M{};
     CompactGeometry shared{};
     std::vector<CompactGeometry> geo(n);
-    uint32_t force_G = 0; // diagnostics: PGS_WALK_G, as pgs_compact_ex
-    if (const char *ev = getenv("PGS_WALK_G")) { const int v = atoi(ev); if (v == 1 || v == 2 || v == 4 || v == 8 || v == 16) force_G = (uint32_t)v; }
     const uint32_t smem = compact_smem_budget((uint32_t)e->max_smem_optin);
-    bool geo_ok = compact_many_geometry(P.data(), T.data(), geo.data(), n, smem, M, shared, force_G);
+    Resident walk{};
+    bool geo_ok = compact_many_geometry(P.data(), T.data(), geo.data(), n, smem, M, shared, walk_g_override());
     if (geo_ok) { // second pass: the segment weight follows from how many groups the device runs at once
-        int occ = 0;
-        PGS_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, walk_many_kernel(shared.G), (int)kWalkThreads, (size_t)shared.walk_dyn));
-        const uint64_t groups = (uint64_t)std::max(1, occ) * e->sm_count * (kWalkThreads / shared.G);
-        geo_ok = compact_many_geometry(P.data(), T.data(), geo.data(), n, smem, M, shared, shared.G, 0, groups);
+        PGS_CUDA(resident(*e, walk_many_kernel(shared.G), kWalkThreads, shared.G, shared.walk_dyn, walk));
+        geo_ok = compact_many_geometry(P.data(), T.data(), geo.data(), n, smem, M, shared, shared.G, 0, walk.groups);
     }
     if (!geo_ok) {
         uint32_t widest = 0;
@@ -265,82 +245,54 @@ extern "C" int32_t pgs_compact_many(const pgs_compact_job *jobs, uint32_t n, uin
     PGS_CUDA(cudaSetDevice(e->device));
     cudaStream_t st = e->stream;
     LaunchScratch S(st);
-    // the merged runs' buffers, one set per job; the scratch of every job is laid out in one allocation, grouped by fill byte
-    struct Slice { void **p; uint64_t bytes; int fill; };
-    std::vector<Slice> slices;
+    // the merged runs' buffers, one set per job; the scratch of every job in one allocation
+    ScratchArena arena;
     std::vector<std::shared_ptr<Run>> outr(n);
     cudaError_t ce = cudaSuccess;
     for (uint32_t i = 0; i < n; i++) {
         outr[i] = std::make_shared<Run>(e);
         outr[i]->level = jobs[i].out_level;
-        Run &r = *outr[i];
-        compact_buffers(P[i], geo[i], T[i], r, [&](auto *&p, uint64_t cnt, int fill, bool is_out) {
-            const size_t bytes = sizeof(*p) * cnt;
-            if (!is_out) { slices.push_back(Slice{(void **)&p, bytes, fill}); return; }
-            if (ce != cudaSuccess) return;
-            if ((void *)&p == (void *)&r.d_data) ce = e->alloc_data(r, bytes);
-            else ce = cudaMallocAsync((void **)&p, bytes, st); // ~Run frees the run's buffers
-            if (ce == cudaSuccess && fill != kNoFill) ce = cudaMemsetAsync(p, fill, bytes, st);
-        });
+        auto keep = run_buffers(e, *outr[i], ce);
+        compact_buffers(P[i], geo[i], T[i], *outr[i], [&](auto *&p, uint64_t cnt, int fill, bool is_out) { if (is_out) keep(p, cnt, fill); else arena(p, cnt, fill); });
     }
     PGS_CUDA(ce);
-    slices.push_back(Slice{(void **)&M.ticket, 2 * sizeof(uint32_t), 0});
-    std::vector<int> fills;
-    for (auto &s : slices)
-        if (std::find(fills.begin(), fills.end(), s.fill) == fills.end()) fills.push_back(s.fill);
-    std::vector<uint64_t> offs(slices.size());
-    std::vector<std::pair<uint64_t, uint64_t>> fill_range(fills.size());
-    uint64_t arena_bytes = 0;
-    for (size_t f = 0; f < fills.size(); f++) {
-        fill_range[f].first = arena_bytes;
-        for (size_t x = 0; x < slices.size(); x++)
-            if (slices[x].fill == fills[f]) { offs[x] = arena_bytes; arena_bytes += (std::max<uint64_t>(slices[x].bytes, 16) + 255) & ~255ull; }
-        fill_range[f].second = arena_bytes;
-    }
-    uint8_t *arena = nullptr;
-    PGS_CUDA(S.alloc(arena, arena_bytes));
-    for (size_t f = 0; f < fills.size(); f++)
-        if (fills[f] != kNoFill) PGS_CUDA(cudaMemsetAsync(arena + fill_range[f].first, fills[f], fill_range[f].second - fill_range[f].first, st));
-    for (size_t x = 0; x < slices.size(); x++) *slices[x].p = arena + offs[x];
+    arena(M.ticket, 2, 0);
+    PGS_CUDA(arena.place(S));
 
-    // the job table: MergeParams[n] | MergeStats[n] | seg_base[n + 1] | blk_base[n + 1] | the ops tables, in one upload
-    const uint64_t o_stats = sizeof(MergeParams) * (uint64_t)n, o_seg = (o_stats + sizeof(MergeStats) * (uint64_t)n + 15) & ~15ull;
-    const uint64_t o_blk = (o_seg + 4ull * (n + 1) + 15) & ~15ull, o_ops = (o_blk + 4ull * (n + 1) + 15) & ~15ull;
-    const uint64_t tab_bytes = o_ops + ops_total;
-    uint8_t *tab = nullptr;
-    PGS_CUDA(S.alloc(tab, tab_bytes));
-    std::vector<uint8_t> h(tab_bytes, 0);
-    uint64_t ops_at = o_ops;
+    // the job table: MergeParams[n] | MergeStats[n] | seg_base[n + 1] | blk_base[n + 1] | the ops tables
+    JobTable tab;
+    const uint64_t o_job = tab.add<MergeParams>(n), o_stats = tab.add<MergeStats>(n);
+    const uint64_t o_seg = tab.add<uint32_t>(n + 1), o_blk = tab.add<uint32_t>(n + 1);
+    std::vector<uint64_t> o_ops(n);
+    for (uint32_t i = 0; i < n; i++)
+        if (ops_len[i]) o_ops[i] = tab.add<uint8_t>(ops_len[i]);
+    PGS_CUDA(tab.alloc(S));
     for (uint32_t i = 0; i < n; i++) {
-        P[i].stats = (MergeStats *)(tab + o_stats) + i;
+        P[i].stats = tab.dev<MergeStats>(o_stats) + i;
+        tab.host<MergeStats>(o_stats)[i] = merge_stats_init();
         if (ops_len[i]) {
-            memcpy(h.data() + ops_at, jobs[i].fp->ops, ops_len[i]);
-            P[i].ops = tab + ops_at;
-            ops_at += (ops_len[i] + 15) & ~15u;
+            memcpy(tab.host<uint8_t>(o_ops[i]), jobs[i].fp->ops, ops_len[i]);
+            P[i].ops = tab.dev<uint8_t>(o_ops[i]);
         }
-        const MergeStats s0 = merge_stats_init();
-        memcpy(h.data() + o_stats + sizeof(MergeStats) * i, &s0, sizeof s0);
     }
-    memcpy(h.data(), P.data(), sizeof(MergeParams) * (size_t)n);
-    compact_many_bases(P.data(), n, (uint32_t *)(h.data() + o_seg), (uint32_t *)(h.data() + o_blk));
-    PGS_CUDA(cudaMemcpyAsync(tab, h.data(), tab_bytes, cudaMemcpyHostToDevice, st));
-    M.job = (const MergeParams *)tab;
-    M.seg_base = (const uint32_t *)(tab + o_seg);
-    M.blk_base = (const uint32_t *)(tab + o_blk);
+    memcpy(tab.host<MergeParams>(o_job), P.data(), sizeof(MergeParams) * (size_t)n);
+    compact_many_bases(P.data(), n, tab.host<uint32_t>(o_seg), tab.host<uint32_t>(o_blk));
+    PGS_CUDA(tab.upload(st));
+    M.job = tab.dev<MergeParams>(o_job);
+    M.seg_base = tab.dev<uint32_t>(o_seg);
+    M.blk_base = tab.dev<uint32_t>(o_blk);
     M.validate_hash = any_hash;
     M.crc_table = (const unsigned long long *)e->d_crc;
 
     cudaEvent_t ev[4];
     for (auto &x : ev) PGS_CUDA(S.event(x));
-    int occ_w = 0, occ_e = 0;
-    PGS_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_w, walk_many_kernel(shared.G), (int)kWalkThreads, (size_t)shared.walk_dyn));
-    PGS_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_e, k_emit_many, (int)(shared.emit_warps * 32), (size_t)shared.emit_dyn));
-    const uint32_t launches = compact_launch_many(M, shared, (uint64_t)std::max(1, occ_w) * e->sm_count, (uint64_t)std::max(1, occ_e) * e->sm_count,
-                                                  st, [&](int i) { if (ce == cudaSuccess) ce = cudaEventRecord(ev[i], st); });
+    Resident emit{};
+    PGS_CUDA(resident(*e, k_emit_many, shared.emit_warps * 32, 32, shared.emit_dyn, emit));
+    const uint32_t launches = compact_launch_many(M, shared, walk.ctas, emit.ctas, st, [&](int i) { if (ce == cudaSuccess) ce = cudaEventRecord(ev[i], st); });
     e->launches += launches;
     PGS_CUDA(ce);
     std::vector<MergeStats> hs(n);
-    PGS_CUDA(cudaMemcpyAsync(hs.data(), tab + o_stats, sizeof(MergeStats) * (size_t)n, cudaMemcpyDeviceToHost, st));
+    PGS_CUDA(cudaMemcpyAsync(hs.data(), tab.dev<MergeStats>(o_stats), sizeof(MergeStats) * (size_t)n, cudaMemcpyDeviceToHost, st));
     cudaError_t se = cudaStreamSynchronize(st);
     if (se != cudaSuccess) return cuda_fail(se, "multi-job compaction kernels");
     for (uint32_t i = 0; i < n; i++)
@@ -348,41 +300,13 @@ extern "C" int32_t pgs_compact_many(const pgs_compact_job *jobs, uint32_t n, uin
             set_error("compact_many: job %u: compaction kernel failed with status %u at segment %u of %u", i, hs[i].error, hs[i].error_seg, P[i].Q);
             return (int32_t)hs[i].error;
         }
-    float ms_total = 0, ms_merge = 0, ms_walk = 0, ms_emit = 0;
-    cudaEventElapsedTime(&ms_total, ev[0], ev[3]);
-    cudaEventElapsedTime(&ms_merge, ev[1], ev[3]);
-    cudaEventElapsedTime(&ms_walk, ev[1], ev[2]);
-    cudaEventElapsedTime(&ms_emit, ev[2], ev[3]);
-    std::vector<pgs_compact_result> res(n);
-    for (uint32_t i = 0; i < n; i++) {
-        outr[i]->n_bloom_entries = compact_result_stats(hs[i], T[i].in_block_bytes, res[i], outr[i]->info);
-        outr[i]->info.level = jobs[i].out_level;
-        res[i].n_tiles = P[i].Q; res[i].n_launches = launches;
-        res[i].device_ms = ms_total; res[i].merge_kernel_ms = ms_merge;
-        res[i].walk_ms = ms_walk; res[i].emit_ms = ms_emit;
-    }
-    // all partitions or none: every lock is held (in address order) from the check that the inputs are still there to the install
-    std::vector<std::unique_lock<std::mutex>> held;
-    for (Partition *p : order) held.emplace_back(p->mu);
-    for (uint32_t i = 0; i < n; i++)
-        for (auto &r : in[i])
-            if (std::find(parts[i]->runs.begin(), parts[i]->runs.end(), r) == parts[i]->runs.end()) {
-                set_error("compact_many: job %u: run %llu left the partition during the merge", i, (unsigned long long)r->id);
-                return PGS_ABORTED;
-            }
-    for (uint32_t i = 0; i < n; i++) {
-        Partition &part = *parts[i];
-        if (!(flags & PGS_COMPACT_KEEP_INPUTS))
-            for (auto &r : in[i]) part.runs.erase(std::find(part.runs.begin(), part.runs.end(), r));
-        if (hs[i].tot_blocks > 0 && !(flags & PGS_COMPACT_DISCARD_OUTPUT)) {
-            outr[i]->id = e->next_run_id++;
-            outr[i]->info.run_id = outr[i]->id;
-            part.insert(outr[i]);
-            res[i].new_run_id = outr[i]->id;
-        }
-    }
-    if (out) memcpy(out, res.data(), sizeof(pgs_compact_result) * (size_t)n);
-    return PGS_OK;
+    pgs_compact_result res{};
+    res.n_launches = launches;
+    cudaEventElapsedTime(&res.device_ms, ev[0], ev[3]);
+    cudaEventElapsedTime(&res.merge_kernel_ms, ev[1], ev[3]);
+    cudaEventElapsedTime(&res.walk_ms, ev[1], ev[2]);
+    cudaEventElapsedTime(&res.emit_ms, ev[2], ev[3]);
+    return compact_install(n, parts.data(), in.data(), outr.data(), hs.data(), P.data(), T.data(), res, flags, true, out);
 }
 
 // ---- pgs_partition_split ------------------------------------------------------------------------------------------------------
@@ -419,18 +343,16 @@ int32_t split_run(Engine *e, const Run &in, const SplitParams &proto, std::vecto
     if (in.info.n_blocks >= (1u << 28) || in.info.data_bytes >= (1ull << 40)) return PGS_NOT_SUPPORTED;
     const uint32_t smem = compact_smem_budget((uint32_t)e->max_smem_optin);
     SplitGeometry geo{};
+    Resident walk{};
     int32_t rc = split_plan(SP, T, smem, geo);
-    int occ_w = 0;
     if (rc == PGS_OK) { // second pass: segments sized by the groups the device runs at once
-        PGS_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_w, split_kernel(geo.G, false), (int)kSplitThreads, (size_t)geo.walk_dyn));
-        const uint64_t groups = (uint64_t)std::max(1, occ_w) * e->sm_count * (kSplitThreads / geo.G);
-        rc = split_plan(SP, T, smem, geo, groups);
+        PGS_CUDA(resident(*e, split_kernel(geo.G, false), kSplitThreads, geo.G, geo.walk_dyn, walk));
+        rc = split_plan(SP, T, smem, geo, walk.groups);
     }
     if (rc != PGS_OK) {
         set_error("partition_split: a run with user keys of %u bytes into %u children is not supported", T.max_ukey, NC);
         return rc;
     }
-    const uint64_t walk_ctas = (uint64_t)std::max(1, occ_w) * e->sm_count;
 
     LaunchScratch S(st);
     cudaError_t ce = cudaSuccess;
@@ -440,7 +362,7 @@ int32_t split_run(Engine *e, const Run &in, const SplitParams &proto, std::vecto
     PGS_CUDA(cudaMemcpyAsync(SP.stats, hs.data(), sizeof(MergeStats) * NC, cudaMemcpyHostToDevice, st));
     cudaEvent_t ev[5];
     for (auto &x : ev) PGS_CUDA(S.event(x));
-    res.n_launches += split_launch(SP, geo, nullptr, nullptr, 0, walk_ctas, 0, st, [&](int i) { if (ce == cudaSuccess) ce = cudaEventRecord(ev[i], st); });
+    res.n_launches += split_launch(SP, geo, nullptr, nullptr, 0, walk.ctas, 0, st, [&](int i) { if (ce == cudaSuccess) ce = cudaEventRecord(ev[i], st); });
     PGS_CUDA(ce);
     std::vector<unsigned long long> prefixes(NC);
     unsigned long long dropped = 0;
@@ -465,13 +387,8 @@ int32_t split_run(Engine *e, const Run &in, const SplitParams &proto, std::vecto
         if (!split_child(SP, hs[c], prefixes[c], smem, P, g, Tc)) { set_error("partition_split: child %u's run is too large", c); return PGS_NOT_SUPPORTED; }
         auto r = std::make_shared<Run>(e);
         r->level = in.level;
-        compact_buffers(P, g, Tc, *r, [&](auto *&p, uint64_t n, int fill, bool is_out) {
-            const size_t bytes = sizeof(*p) * n;
-            if (!is_out || ce != cudaSuccess) return; // the scratch is the split's
-            if ((void *)&p == (void *)&r->d_data) ce = e->alloc_data(*r, bytes);
-            else ce = cudaMallocAsync((void **)&p, bytes, st); // ~Run frees the run's buffers
-            if (ce == cudaSuccess && fill != kNoFill) ce = cudaMemsetAsync(p, fill, bytes, st);
-        });
+        auto keep = run_buffers(e, *r, ce);
+        compact_buffers(P, g, Tc, *r, [&](auto *&p, uint64_t n, int fill, bool is_out) { if (is_out) keep(p, n, fill); }); // the scratch is the split's
         PGS_CUDA(ce);
         split_child_scratch(SP, c, P);
         Pc.push_back(P);
@@ -479,10 +396,9 @@ int32_t split_run(Engine *e, const Run &in, const SplitParams &proto, std::vecto
         which.push_back(c);
         out[c] = r;
     }
-    int occ_e = 1;
-    if (!gc.empty())
-        PGS_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_e, k_emit, (int)(gc[0].emit_warps * 32), (size_t)gc[0].emit_dyn));
-    res.n_launches += split_launch(SP, geo, Pc.data(), gc.data(), (uint32_t)Pc.size(), walk_ctas, (uint64_t)std::max(1, occ_e) * e->sm_count, st,
+    Resident emit{};
+    if (!gc.empty()) PGS_CUDA(resident(*e, k_emit, gc[0].emit_warps * 32, 32, gc[0].emit_dyn, emit));
+    res.n_launches += split_launch(SP, geo, Pc.data(), gc.data(), (uint32_t)Pc.size(), walk.ctas, emit.ctas, st,
                                    [&](int i) { if (ce == cudaSuccess) ce = cudaEventRecord(ev[2 + i], st); });
     PGS_CUDA(ce);
     PGS_CUDA(cudaMemcpyAsync(hs.data(), SP.stats, sizeof(MergeStats) * NC, cudaMemcpyDeviceToHost, st));
@@ -550,6 +466,43 @@ int32_t split_dests(pgs_partition *src, uint32_t src_count, uint32_t dst_count, 
     if (NC > kSplitMaxChildren) { set_error("partition_split: %u children > %u", NC, kSplitMaxChildren); return PGS_NOT_SUPPORTED; }
     return PGS_OK;
 }
+
+// The children of n split jobs installed, all or none (many: with pgs_partition_split_many's messages).  rows[i][c] = job i's
+// child c (null: not built), built[i * NC + c] = its runs in the parent's order.  Every child's lock is held from the check that
+// none took runs during the split (PGS_ABORTED otherwise) to the last install; each run gets its id and res[i].child[c] counts it.
+int32_t split_install(Engine *e, pgs_partition *const *const *rows, uint32_t n, uint32_t NC, const std::vector<std::vector<std::shared_ptr<Run>>> &built,
+                      pgs_split_result *res, bool many)
+{
+    std::vector<Partition *> kids;
+    for (uint32_t i = 0; i < n; i++)
+        for (uint32_t c = 0; c < NC; c++)
+            if (rows[i][c]) kids.push_back(&rows[i][c]->p);
+    const auto held = lock_partitions(kids);
+    for (uint32_t i = 0; i < n; i++)
+        for (uint32_t c = 0; c < NC; c++)
+            if (rows[i][c] && !rows[i][c]->p.runs.empty()) {
+                if (many) set_error("partition_split_many: job %u: destination %u took runs during the split", i, c);
+                else set_error("partition_split: destination %d took runs during the split", rows[i][c]->p.pidx);
+                return PGS_ABORTED;
+            }
+    for (uint32_t i = 0; i < n; i++)
+        for (uint32_t c = 0; c < NC; c++) {
+            if (!rows[i][c]) continue;
+            pgs_split_child_result &cr = res[i].child[c];
+            const auto &b = built[(size_t)i * NC + c];
+            for (auto &r : b) {
+                r->id = e->next_run_id++;
+                r->info.run_id = r->id;
+                cr.records += r->info.n_records;
+                cr.tombstones += r->info.n_tombstones;
+                cr.raw_bytes += r->info.raw_key_bytes + r->info.raw_value_bytes;
+                cr.block_bytes += r->info.data_bytes;
+                cr.runs++;
+            }
+            rows[i][c]->p.runs = b;
+        }
+    return PGS_OK;
+}
 } // namespace
 
 // pgs_partition_split over the runs `snap` of src (nullptr: its current runs); pgs_rrdb_split passes the snapshot it took
@@ -598,29 +551,7 @@ int32_t partition_split(pgs_partition *src, const std::vector<std::shared_ptr<Ru
     PGS_CUDA(cudaEventSynchronize(t1));
     cudaEventElapsedTime(&res.device_ms, t0, t1);
     res.kernel_ms = res.count_ms + res.walk_ms + res.emit_ms;
-    // all children, or none: every child's lock is held (in address order) from the check to the install
-    std::vector<Partition *> kids;
-    for (uint32_t c = 0; c < NC; c++)
-        if (dst[c]) kids.push_back(&dst[c]->p);
-    std::sort(kids.begin(), kids.end());
-    std::vector<std::unique_lock<std::mutex>> held;
-    for (Partition *k : kids) held.emplace_back(k->mu);
-    for (Partition *k : kids)
-        if (!k->runs.empty()) { set_error("partition_split: destination %d took runs during the split", k->pidx); return PGS_ABORTED; }
-    for (uint32_t c = 0; c < NC; c++) {
-        if (!dst[c]) continue;
-        pgs_split_child_result &cr = res.child[c];
-        for (auto &r : built[c]) {
-            r->id = e->next_run_id++;
-            r->info.run_id = r->id;
-            cr.records += r->info.n_records;
-            cr.tombstones += r->info.n_tombstones;
-            cr.raw_bytes += r->info.raw_key_bytes + r->info.raw_value_bytes;
-            cr.block_bytes += r->info.data_bytes;
-            cr.runs++;
-        }
-        dst[c]->p.runs = built[c];
-    }
+    if (const int32_t rc = split_install(e, &dst, 1, NC, built, &res, false)) return rc;
     e->launches += res.n_launches;
     if (out) *out = res;
     return PGS_OK;
@@ -635,33 +566,23 @@ int32_t partition_split_many(const pgs_split_job *jobs, uint32_t n, uint32_t src
     if (n == 0) return PGS_OK;
     if (!jobs) { set_error("partition_split_many: %u jobs and no job array", n); return PGS_INVALID_ARGUMENT; }
     if (n > PGS_SPLIT_MANY_MAX_JOBS) { set_error("partition_split_many: %u jobs > %u per call", n, PGS_SPLIT_MANY_MAX_JOBS); return PGS_NOT_SUPPORTED; }
-    const uint32_t n_dst = src_count ? dst_count / src_count : 0;
+    const uint32_t NC = src_count ? dst_count / src_count : 0;
     std::vector<uint32_t> want(n);
-    Engine *e = nullptr;
+    // every partition in one job only: a parent is no other job's parent or child, a child no other job's child
+    JobPartitions set;
     for (uint32_t i = 0; i < n; i++) {
-        if (const int32_t rc = split_dests(jobs[i].src, src_count, dst_count, jobs[i].dst, n_dst, want[i])) {
+        if (const int32_t rc = split_dests(jobs[i].src, src_count, dst_count, jobs[i].dst, NC, want[i])) {
             const std::string why = pgs_last_error();
             set_error("partition_split_many: job %u: %s", i, why.c_str());
             return rc;
         }
-        if (!e) e = jobs[i].src->p.eng;
-        if (jobs[i].src->p.eng != e) { set_error("partition_split_many: job %u: its parent is on another engine than job 0's", i); return PGS_INVALID_ARGUMENT; }
-    }
-    const uint32_t NC = n_dst;
-    // every partition in one job only: a parent is no other job's parent or child, a child no other job's child
-    std::vector<std::pair<Partition *, uint32_t>> seen;
-    for (uint32_t i = 0; i < n; i++) {
-        seen.emplace_back(&jobs[i].src->p, i);
+        if (!set.add(jobs[i].src->p, i)) { set_error("partition_split_many: job %u: its parent is on another engine than job 0's", i); return PGS_INVALID_ARGUMENT; }
         for (uint32_t c = 0; c < NC; c++)
-            if (jobs[i].dst[c]) seen.emplace_back(&jobs[i].dst[c]->p, i);
+            if (jobs[i].dst[c]) set.add(jobs[i].dst[c]->p, i); // on the parent's engine (split_dests)
     }
-    std::sort(seen.begin(), seen.end());
-    for (size_t x = 1; x < seen.size(); x++)
-        if (seen[x].first == seen[x - 1].first) {
-            set_error("partition_split_many: job %u: a partition of job %u is in job %u too", std::max(seen[x].second, seen[x - 1].second),
-                      std::min(seen[x].second, seen[x - 1].second), std::max(seen[x].second, seen[x - 1].second));
-            return PGS_INVALID_ARGUMENT;
-        }
+    uint32_t a = 0, b = 0;
+    if (set.twice(a, b)) { set_error("partition_split_many: job %u: a partition of job %u is in job %u too", b, a, b); return PGS_INVALID_ARGUMENT; }
+    Engine *e = set.e;
 
     // the parent runs, job by job in each parent's order; run x belongs to job run_job[x]
     std::vector<std::shared_ptr<Run>> in;
@@ -711,13 +632,12 @@ int32_t partition_split_many(const pgs_split_job *jobs, uint32_t n, uint32_t src
     SplitJobs J{};
     MergeJobs M{};
     SplitGeometry geo{};
-    int occ_w = 0;
+    Resident walk{};
     if (nr) {
         int32_t rc = split_many_plan(SP.data(), T.data(), nr, smem, J, M, geo);
         if (rc == PGS_OK) { // second pass: segments sized by the groups the device runs at once
-            PGS_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_w, split_many_kernel(geo.G, false), (int)kSplitThreads, (size_t)geo.walk_dyn));
-            const uint64_t groups = (uint64_t)std::max(1, occ_w) * e->sm_count * (kSplitThreads / geo.G);
-            rc = split_many_plan(SP.data(), T.data(), nr, smem, J, M, geo, groups);
+            PGS_CUDA(resident(*e, split_many_kernel(geo.G, false), kSplitThreads, geo.G, geo.walk_dyn, walk));
+            rc = split_many_plan(SP.data(), T.data(), nr, smem, J, M, geo, walk.groups);
         }
         for (uint32_t x = 0; x < nr && rc == PGS_OK; x++) emit_segments += (uint64_t)SP[x].M.Q * __builtin_popcount(SP[x].want);
         if (rc == PGS_OK && emit_segments > 0x7FFFFFF0ull) rc = PGS_NOT_SUPPORTED;
@@ -741,50 +661,27 @@ int32_t partition_split_many(const pgs_split_job *jobs, uint32_t n, uint32_t src
     std::vector<std::vector<std::shared_ptr<Run>>> outs(nr, std::vector<std::shared_ptr<Run>>(NC));
     cudaError_t ce = cudaSuccess;
     if (nr) {
-        // the scratch in one allocation grouped by fill byte: one pass of split_many_buffers sizes it, a second hands it out
-        std::vector<std::pair<uint64_t, int>> sl;
-        split_many_buffers(SP.data(), nr, J, [&](auto *&p, uint64_t cnt, int fill, bool) { sl.emplace_back(sizeof(*p) * cnt, fill); p = nullptr; });
-        std::vector<int> fills;
-        for (auto &s : sl)
-            if (std::find(fills.begin(), fills.end(), s.second) == fills.end()) fills.push_back(s.second);
-        std::vector<uint64_t> offs(sl.size());
-        std::vector<std::pair<uint64_t, uint64_t>> fill_range(fills.size());
-        uint64_t arena_bytes = 0;
-        for (size_t f = 0; f < fills.size(); f++) {
-            fill_range[f].first = arena_bytes;
-            for (size_t x = 0; x < sl.size(); x++)
-                if (sl[x].second == fills[f]) { offs[x] = arena_bytes; arena_bytes += (std::max<uint64_t>(sl[x].first, 16) + 255) & ~255ull; }
-            fill_range[f].second = arena_bytes;
-        }
-        uint8_t *arena = nullptr;
-        PGS_CUDA(S.alloc(arena, arena_bytes));
-        for (size_t f = 0; f < fills.size(); f++)
-            if (fills[f] != kNoFill) PGS_CUDA(cudaMemsetAsync(arena + fill_range[f].first, fills[f], fill_range[f].second - fill_range[f].first, st));
-        size_t at = 0;
-        split_many_buffers(SP.data(), nr, J, [&](auto *&p, uint64_t, int, bool) { *(void **)&p = arena + offs[at++]; });
+        ScratchArena arena; // the scratch in one allocation
+        split_many_buffers(SP.data(), nr, J, arena);
+        PGS_CUDA(arena.place(S));
         PGS_CUDA(cudaMemcpyAsync(J.stats, hs.data(), sizeof(MergeStats) * hs.size(), cudaMemcpyHostToDevice, st));
 
-        // the job tables: MergeParams[nr] (the planner's) | SplitParams[nr] | seg_base[nr + 1] | blk_base[nr + 1], in one upload
-        std::vector<MergeParams> MP(nr);
-        for (uint32_t x = 0; x < nr; x++) MP[x] = SP[x].M;
-        const uint64_t o_split = (sizeof(MergeParams) * (uint64_t)nr + 15) & ~15ull;
-        const uint64_t o_seg = (o_split + sizeof(SplitParams) * (uint64_t)nr + 15) & ~15ull, o_blk = (o_seg + 4ull * (nr + 1) + 15) & ~15ull;
-        const uint64_t tab_bytes = o_blk + 4ull * (nr + 1);
-        std::vector<uint8_t> h(tab_bytes, 0);
-        memcpy(h.data(), MP.data(), sizeof(MergeParams) * (size_t)nr);
-        memcpy(h.data() + o_split, SP.data(), sizeof(SplitParams) * (size_t)nr);
-        compact_many_bases(MP.data(), nr, (uint32_t *)(h.data() + o_seg), (uint32_t *)(h.data() + o_blk));
-        uint8_t *tab = nullptr;
-        PGS_CUDA(S.upload(tab, h.data(), tab_bytes));
-        M.job = (const MergeParams *)tab;
-        M.seg_base = J.seg_base = (const uint32_t *)(tab + o_seg);
-        M.blk_base = (const uint32_t *)(tab + o_blk);
-        J.job = (const SplitParams *)(tab + o_split);
+        // the job tables: MergeParams[nr] (the planner's) | SplitParams[nr] | seg_base[nr + 1] | blk_base[nr + 1]
+        JobTable tab;
+        const uint64_t o_job = tab.add<MergeParams>(nr), o_split = tab.add<SplitParams>(nr);
+        const uint64_t o_seg = tab.add<uint32_t>(nr + 1), o_blk = tab.add<uint32_t>(nr + 1);
+        split_many_tables(SP.data(), nr, J, tab.host<MergeParams>(o_job), tab.host<uint32_t>(o_seg), tab.host<uint32_t>(o_blk));
+        memcpy(tab.host<SplitParams>(o_split), SP.data(), sizeof(SplitParams) * (size_t)nr);
+        PGS_CUDA(tab.alloc(S));
+        PGS_CUDA(tab.upload(st));
+        M.job = tab.dev<MergeParams>(o_job);
+        M.seg_base = J.seg_base = tab.dev<uint32_t>(o_seg);
+        M.blk_base = tab.dev<uint32_t>(o_blk);
+        J.job = tab.dev<SplitParams>(o_split);
         J.crc_table = (const unsigned long long *)e->d_crc;
 
         // counting phase, then one read-back of every (job, child) counter, prefix count and dropped count
-        const uint64_t walk_ctas = (uint64_t)std::max(1, occ_w) * e->sm_count;
-        all.n_launches += split_many_launch(J, M, geo, nullptr, CompactGeometry{}, walk_ctas, 0, st,
+        all.n_launches += split_many_launch(J, M, geo, nullptr, CompactGeometry{}, walk.ctas, 0, st,
                                             [&](int i) { if (ce == cudaSuccess) ce = cudaEventRecord(ev[i], st); });
         PGS_CUDA(ce);
         PGS_CUDA(cudaMemcpyAsync(hs.data(), J.stats, sizeof(MergeStats) * hs.size(), cudaMemcpyDeviceToHost, st));
@@ -800,51 +697,40 @@ int32_t partition_split_many(const pgs_split_job *jobs, uint32_t n, uint32_t src
 
         // the children's outputs, sized by what the counting pass found; every (parent run, built child) is a job of k_emit_many
         std::vector<MergeParams> Pc;
-        std::vector<uint32_t> emit_base(1, 0);
+        std::vector<uint32_t> emit_base;
         CompactGeometry shape{};
-        for (uint32_t x = 0; x < nr; x++)
-            for (uint32_t c = 0; c < NC; c++) {
-                const size_t y = (size_t)x * NC + c;
-                if (!((SP[x].want >> c) & 1u) || hs[y].cnt[EV_OUT] == 0) continue;
-                MergeParams P{};
-                CompactGeometry g{};
-                CompactTotals Tc{};
-                if (!split_many_child(SP[x], c, hs[y], prefixes[y], smem, P, g, Tc, Pc.empty() ? nullptr : &Pc[0], &shape)) {
-                    set_error("partition_split_many: job %u: child %u's run is too large, or not of the launch's shape", run_job[x], c);
-                    return PGS_NOT_SUPPORTED;
-                }
-                auto r = std::make_shared<Run>(e);
-                r->level = in[x]->level;
-                compact_buffers(P, g, Tc, *r, [&](auto *&p, uint64_t cnt, int fill, bool is_out) {
-                    const size_t bytes = sizeof(*p) * cnt;
-                    if (!is_out || ce != cudaSuccess) return; // the scratch is the split's
-                    if ((void *)&p == (void *)&r->d_data) ce = e->alloc_data(*r, bytes);
-                    else ce = cudaMallocAsync((void **)&p, bytes, st); // ~Run frees the run's buffers
-                    if (ce == cudaSuccess && fill != kNoFill) ce = cudaMemsetAsync(p, fill, bytes, st);
-                });
-                PGS_CUDA(ce);
-                if (Pc.empty()) shape = g;
-                Pc.push_back(P);
-                emit_base.push_back(emit_base.back() + P.Q);
-                outs[x][c] = r;
-            }
+        uint64_t at = 0;
+        const bool sized = split_many_children(SP.data(), nr, hs.data(), prefixes.data(), smem, Pc, emit_base, shape, at,
+                                               [&](uint32_t x, uint32_t c, MergeParams &P, const CompactGeometry &g, const CompactTotals &Tc) {
+                                                   auto r = std::make_shared<Run>(e);
+                                                   r->level = in[x]->level;
+                                                   auto keep = run_buffers(e, *r, ce);
+                                                   compact_buffers(P, g, Tc, *r, [&](auto *&p, uint64_t cnt, int fill, bool is_out) { if (is_out) keep(p, cnt, fill); });
+                                                   outs[x][c] = r;
+                                                   return ce == cudaSuccess;
+                                               });
+        PGS_CUDA(ce);
+        if (!sized) {
+            set_error("partition_split_many: job %u: child %u's run is too large, or not of the launch's shape", run_job[at / NC], (uint32_t)(at % NC));
+            return PGS_NOT_SUPPORTED;
+        }
         if (!Pc.empty()) { // writing phase
             const uint32_t nc = (uint32_t)Pc.size();
-            const uint64_t o_base = (sizeof(MergeParams) * (uint64_t)nc + 15) & ~15ull;
-            std::vector<uint8_t> hc(o_base + 4ull * (nc + 1), 0);
-            memcpy(hc.data(), Pc.data(), sizeof(MergeParams) * (size_t)nc);
-            memcpy(hc.data() + o_base, emit_base.data(), 4ull * (nc + 1));
-            uint8_t *ctab = nullptr;
-            PGS_CUDA(S.upload(ctab, hc.data(), hc.size()));
+            JobTable ctab;
+            const uint64_t o_pc = ctab.add<MergeParams>(nc), o_base = ctab.add<uint32_t>(nc + 1);
+            memcpy(ctab.host<MergeParams>(o_pc), Pc.data(), sizeof(MergeParams) * (size_t)nc);
+            memcpy(ctab.host<uint32_t>(o_base), emit_base.data(), 4ull * (nc + 1));
+            PGS_CUDA(ctab.alloc(S));
+            PGS_CUDA(ctab.upload(st));
             MergeJobs E{};
-            E.job = (const MergeParams *)ctab;
-            E.seg_base = (const uint32_t *)(ctab + o_base);
+            E.job = ctab.dev<MergeParams>(o_pc);
+            E.seg_base = ctab.dev<uint32_t>(o_base);
             E.n = nc;
             E.Q = emit_base.back();
             E.ticket = J.ticket + 2;
-            int occ_e = 0;
-            PGS_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_e, k_emit_many, (int)(shape.emit_warps * 32), (size_t)shape.emit_dyn));
-            all.n_launches += split_many_launch(J, M, geo, &E, shape, walk_ctas, (uint64_t)std::max(1, occ_e) * e->sm_count, st,
+            Resident emit{};
+            PGS_CUDA(resident(*e, k_emit_many, shape.emit_warps * 32, 32, shape.emit_dyn, emit));
+            all.n_launches += split_many_launch(J, M, geo, &E, shape, walk.ctas, emit.ctas, st,
                                                 [&](int i) { if (ce == cudaSuccess) ce = cudaEventRecord(ev[2 + i], st); });
             PGS_CUDA(ce);
             PGS_CUDA(cudaMemcpyAsync(hs.data(), J.stats, sizeof(MergeStats) * hs.size(), cudaMemcpyDeviceToHost, st));
@@ -856,11 +742,8 @@ int32_t partition_split_many(const pgs_split_job *jobs, uint32_t n, uint32_t src
                               hs[y].error_seg, (uint32_t)(y % NC));
                     return (int32_t)hs[y].error;
                 }
-            float ms_walk = 0, ms_emit = 0;
-            cudaEventElapsedTime(&ms_walk, ev[2], ev[4]);
-            cudaEventElapsedTime(&ms_emit, ev[4], ev[3]);
-            all.walk_ms = ms_walk;
-            all.emit_ms = ms_emit;
+            cudaEventElapsedTime(&all.walk_ms, ev[2], ev[4]);
+            cudaEventElapsedTime(&all.emit_ms, ev[4], ev[3]);
         }
         cudaEventElapsedTime(&all.count_ms, ev[0], ev[1]);
     }
@@ -883,40 +766,13 @@ int32_t partition_split_many(const pgs_split_job *jobs, uint32_t n, uint32_t src
                 o.info.level = in[x]->level;
             }
     }
-    // all children of all jobs, or none: every child's lock is held (in address order) from the check to the last install
-    std::vector<Partition *> kids;
-    for (uint32_t i = 0; i < n; i++)
-        for (uint32_t c = 0; c < NC; c++)
-            if (jobs[i].dst[c]) kids.push_back(&jobs[i].dst[c]->p);
-    std::sort(kids.begin(), kids.end());
-    std::vector<std::unique_lock<std::mutex>> held;
-    for (Partition *k : kids) held.emplace_back(k->mu);
-    for (uint32_t i = 0; i < n; i++)
-        for (uint32_t c = 0; c < NC; c++)
-            if (jobs[i].dst[c] && !jobs[i].dst[c]->p.runs.empty()) {
-                set_error("partition_split_many: job %u: destination %u took runs during the split", i, c);
-                return PGS_ABORTED;
-            }
     std::vector<std::vector<std::shared_ptr<Run>>> built((size_t)n * NC); // job i's child c at i * NC + c, in the parent's run order
     for (uint32_t x = 0; x < nr; x++)
         for (uint32_t c = 0; c < NC; c++)
             if (outs[x][c]) built[(size_t)run_job[x] * NC + c].push_back(outs[x][c]);
-    for (uint32_t i = 0; i < n; i++)
-        for (uint32_t c = 0; c < NC; c++) {
-            if (!jobs[i].dst[c]) continue;
-            pgs_split_child_result &cr = res[i].child[c];
-            auto &b = built[(size_t)i * NC + c];
-            for (auto &r : b) {
-                r->id = e->next_run_id++;
-                r->info.run_id = r->id;
-                cr.records += r->info.n_records;
-                cr.tombstones += r->info.n_tombstones;
-                cr.raw_bytes += r->info.raw_key_bytes + r->info.raw_value_bytes;
-                cr.block_bytes += r->info.data_bytes;
-                cr.runs++;
-            }
-            jobs[i].dst[c]->p.runs = b;
-        }
+    std::vector<pgs_partition *const *> rows(n);
+    for (uint32_t i = 0; i < n; i++) rows[i] = jobs[i].dst;
+    if (const int32_t rc = split_install(e, rows.data(), n, NC, built, res.data(), true)) return rc;
     e->launches += all.n_launches;
     if (out) memcpy(out, res.data(), sizeof(pgs_split_result) * (size_t)n);
     return PGS_OK;

@@ -360,6 +360,35 @@ inline bool compact_filter(MergeParams &P, const pgs_filter_params *fp, uint32_t
     return true;
 }
 
+// One compaction job's MergeParams and CompactTotals from its k input runs (run(i): the i-th, with dev(), info and
+// n_bloom_entries), the engine's block shape, the merge's policy and the filter fp (nullptr: none; the crc table is set when it
+// validates hashes).  Refuses more than kMaxRuns runs, a run of 2^28 blocks or 2^40 bytes and a user key over kMaxUkeyLen
+// (PGS_NOT_SUPPORTED), then a malformed ops table (PGS_INVALID_ARGUMENT), with a message that starts with who.  ops_len as
+// compact_filter.
+template <class RunAt>
+inline int32_t compact_job_params(MergeParams &P, CompactTotals &T, uint32_t k, RunAt &&run, uint32_t block_size, uint32_t restart_interval,
+                                  int32_t bottommost, uint32_t now, uint32_t data_version, const pgs_filter_params *fp,
+                                  const unsigned long long *crc_table, uint32_t &ops_len, const char *who)
+{
+    if (k > kMaxRuns) { set_error("%s %u runs > %u per merge", who, k, kMaxRuns); return PGS_NOT_SUPPORTED; }
+    P.k = k;
+    for (uint32_t i = 0; i < k; i++) {
+        const auto &r = run(i);
+        P.runs[i] = r.dev();
+        T.add(r.info, r.n_bloom_entries);
+        if (r.info.n_blocks >= (1u << 28) || r.info.data_bytes >= (1ull << 40)) { set_error("%s a run too large for a merge", who); return PGS_NOT_SUPPORTED; }
+    }
+    if (T.max_ukey > kMaxUkeyLen) { set_error("%s user key of %u bytes > %u", who, T.max_ukey, kMaxUkeyLen); return PGS_NOT_SUPPORTED; }
+    P.block_size = block_size;
+    P.restart_interval = restart_interval;
+    P.bottommost = bottommost ? 1 : 0;
+    P.now = now;
+    P.data_version = data_version;
+    if (!compact_filter(P, fp, ops_len)) { set_error("%s malformed ops table of %u bytes", who, fp->ops_len); return PGS_INVALID_ARGUMENT; }
+    if (P.validate_hash) P.crc_table = crc_table;
+    return PGS_OK;
+}
+
 // Every buffer of one launch: buf(pointer, elements, fill, out) allocates the elements and, unless fill is kNoFill, sets each
 // byte to fill before the first kernel.  The scratch (out = false) lives as long as the launch; the merged run's buffers
 // (out = true) are fields of `run` (the library's Run, or the simulator's host copy), which outlives it.  P points at all of them.

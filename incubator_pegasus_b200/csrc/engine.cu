@@ -307,11 +307,7 @@ static int32_t upload_stage_b(Engine *e, UploadJob &j)
     cudaStream_t st = e->stream;
     PGS_CUDA(cudaEventSynchronize(j.pass1));
     cudaError_t ce = cudaSuccess;
-    const int32_t rc = index_buffers(j.X, *j.r, j.nrec, j.lastlen, *j.hs_out, j.rec_cum, j.key_cum, [&](auto *&p, uint64_t n, int fill) {
-        const size_t bytes = sizeof(*p) * n;
-        if (ce == cudaSuccess) ce = cudaMallocAsync((void **)&p, bytes, st); // ~Run frees the run's buffers
-        if (ce == cudaSuccess && fill != kNoFill) ce = cudaMemsetAsync(p, fill, bytes, st);
-    });
+    const int32_t rc = index_buffers(j.X, *j.r, j.nrec, j.lastlen, *j.hs_out, j.rec_cum, j.key_cum, run_buffers(e, *j.r, ce));
     if (rc) return rc;
     PGS_CUDA(ce);
     PGS_CUDA(cudaMemcpyAsync(j.X.blk_rec, j.rec_cum, sizeof(uint32_t) * (nb + 1), cudaMemcpyHostToDevice, st));
@@ -663,8 +659,7 @@ int32_t pgs_run_build_many(const pgs_run_build_job *jobs, uint32_t n, uint64_t *
     if (n == 0) return PGS_OK;
     if (!jobs) { set_error("run build many: %u jobs and no job array", n); return PGS_INVALID_ARGUMENT; }
     if (n > PGS_RUN_BUILD_MANY_MAX_JOBS) { set_error("run build many: %u jobs > %u per call", n, PGS_RUN_BUILD_MANY_MAX_JOBS); return PGS_NOT_SUPPORTED; }
-    Engine *e = nullptr;
-    std::vector<Partition *> parts(n);
+    JobPartitions set;
     for (uint32_t i = 0; i < n; i++) {
         const pgs_run_build_job &x = jobs[i];
         if (!x.part || x.level < 0 || (x.n && (!x.key_off || !x.val_off || !x.seq || !x.type)) ||
@@ -672,20 +667,11 @@ int32_t pgs_run_build_many(const pgs_run_build_job *jobs, uint32_t n, uint64_t *
             set_error("run build many: job %u: no partition, a negative level or a missing array", i);
             return PGS_INVALID_ARGUMENT;
         }
-        parts[i] = &x.part->p;
-        if (!e) e = parts[i]->eng;
-        if (parts[i]->eng != e) { set_error("run build many: job %u: its partition is on another engine than job 0's", i); return PGS_INVALID_ARGUMENT; }
+        if (!set.add(x.part->p, i)) { set_error("run build many: job %u: its partition is on another engine than job 0's", i); return PGS_INVALID_ARGUMENT; }
     }
-    {
-        std::vector<Partition *> order = parts;
-        std::sort(order.begin(), order.end());
-        for (uint32_t i = 1; i < n; i++)
-            if (order[i] == order[i - 1]) {
-                const uint32_t j = (uint32_t)(std::find(parts.begin(), parts.end(), order[i]) - parts.begin());
-                set_error("run build many: job %u: its partition is in another job too", j);
-                return PGS_INVALID_ARGUMENT;
-            }
-    }
+    uint32_t twice_a = 0, twice_b = 0;
+    if (set.twice(twice_a, twice_b)) { set_error("run build many: job %u: its partition is in another job too", twice_a); return PGS_INVALID_ARGUMENT; }
+    Engine *e = set.e;
     std::vector<const pgs_run_build_job *> J; // the nonempty jobs, and which job each one is
     std::vector<uint32_t> which;
     uint64_t total = 0;
@@ -803,11 +789,7 @@ int32_t pgs_run_build_many(const pgs_run_build_job *jobs, uint32_t n, uint64_t *
     for (uint32_t d = 0; d < jn; d++) {
         const uint32_t b0 = job_out[d];
         const int32_t rc = index_buffers(X[d], *runs[d], h_nrec + b0, h_lastlen + b0, hs[d], rec_cum + b0 + d, key_cum + b0 + d,
-                                         [&](auto *&p, uint64_t cnt, int fill) {
-                                             const size_t sz = sizeof(*p) * cnt;
-                                             if (ce == cudaSuccess) ce = cudaMallocAsync((void **)&p, sz, st); // ~Run frees them
-                                             if (ce == cudaSuccess && fill != kNoFill) ce = cudaMemsetAsync(p, fill, sz, st);
-                                         });
+                                         run_buffers(e, *runs[d], ce));
         if (rc) {
             const std::string m = g_last_error;
             set_error("run build many: job %u: %s", which[d], m.c_str());
@@ -822,12 +804,10 @@ int32_t pgs_run_build_many(const pgs_run_build_job *jobs, uint32_t n, uint64_t *
     PGS_CUDA(cudaEventRecord(ev[4], st));
     PGS_CUDA(cudaEventSynchronize(ev[4]));
     {
-        // all partitions or none: every lock is held, in address order, while the runs go in
-        std::vector<Partition *> order;
-        for (auto *x : J) order.push_back(&x->part->p);
-        std::sort(order.begin(), order.end());
-        std::vector<std::unique_lock<std::mutex>> held;
-        for (Partition *p : order) held.emplace_back(p->mu);
+        // all partitions or none: every lock is held while the runs go in
+        std::vector<Partition *> parts;
+        for (auto *x : J) parts.push_back(&x->part->p);
+        const auto held = lock_partitions(parts);
         for (uint32_t d = 0; d < jn; d++) {
             Run &r = *runs[d];
             run_info_from_index(hs[d], nb[d], bytes[d], job_out[jn + d], r.info);

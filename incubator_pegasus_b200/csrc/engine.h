@@ -2,6 +2,7 @@
 #pragma once
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <atomic>
 #include <cstdint>
 #include <memory>
@@ -199,6 +200,103 @@ inline auto device_buffers(LaunchScratch &S, cudaError_t &ce)
         if (ce == cudaSuccess && in.src) ce = cudaMemcpyAsync((void *)p, in.src, in.src_bytes, cudaMemcpyHostToDevice, S.st);
         if (ce == cudaSuccess && in.fill != kNoFill) ce = cudaMemsetAsync((void *)p, in.fill, bytes, S.st);
     };
+}
+// The (pointer, count, fill) buffers run r keeps (compact_buffers' `out` ones, index_buffers'): d_data from the engine's spare
+// list when one fits, every other one from the stream-ordered pool, each set to fill unless it is kNoFill; ~Run frees them.
+// ce keeps the first failure; after it nothing is allocated.
+inline auto run_buffers(Engine *e, Run &r, cudaError_t &ce)
+{
+    return [e, &r, &ce](auto *&p, uint64_t count, int fill) {
+        const size_t bytes = sizeof(*p) * count;
+        if (ce != cudaSuccess) return;
+        if ((void *)&p == (void *)&r.d_data) ce = e->alloc_data(r, bytes);
+        else ce = cudaMallocAsync((void **)&p, bytes, e->stream);
+        if (ce == cudaSuccess && fill != kNoFill) ce = cudaMemsetAsync((void *)p, fill, bytes, e->stream);
+    };
+}
+// The scratch of a multi-job launch in one allocation: the plan's buffers are collected as (pointer, count, fill[, out]) and
+// place() lays them out grouped by fill byte, 256-aligned, so that every fill is one memset, then points each one into it.
+struct ScratchArena {
+    struct Slice { void **p; uint64_t bytes; int fill; };
+    std::vector<Slice> slices;
+    template <class T> void operator()(T *&p, uint64_t count, int fill, bool = false) { slices.push_back(Slice{(void **)&p, sizeof(T) * count, fill}); }
+    cudaError_t place(LaunchScratch &S)
+    {
+        std::vector<int> fills;
+        for (auto &s : slices)
+            if (std::find(fills.begin(), fills.end(), s.fill) == fills.end()) fills.push_back(s.fill);
+        std::vector<uint64_t> off(slices.size()), end(fills.size() + 1, 0); // fill f's slices are [end[f], end[f + 1])
+        for (size_t f = 0; f < fills.size(); f++) {
+            end[f + 1] = end[f];
+            for (size_t x = 0; x < slices.size(); x++)
+                if (slices[x].fill == fills[f]) { off[x] = end[f + 1]; end[f + 1] += (std::max<uint64_t>(slices[x].bytes, 16) + 255) & ~255ull; }
+        }
+        uint8_t *base = nullptr;
+        cudaError_t ce = S.alloc(base, end.back());
+        for (size_t f = 0; f < fills.size() && ce == cudaSuccess; f++)
+            if (fills[f] != kNoFill) ce = cudaMemsetAsync(base + end[f], fills[f], end[f + 1] - end[f], S.st);
+        if (ce == cudaSuccess)
+            for (size_t x = 0; x < slices.size(); x++) *slices[x].p = base + off[x];
+        return ce;
+    }
+};
+// The job tables of a multi-job launch, read by the kernels from device memory: sections of 16-aligned offsets in one host
+// image, allocated in S (so that the tables can hold each other's device addresses) and uploaded with one copy.
+struct JobTable {
+    std::vector<uint8_t> h;
+    uint8_t *d = nullptr;
+    template <class T> uint64_t add(uint64_t count) // a section of count elements, zero until written; returns its offset
+    {
+        const uint64_t at = (h.size() + 15) & ~15ull;
+        h.resize(at + sizeof(T) * count, 0);
+        return at;
+    }
+    template <class T> T *host(uint64_t at) { return (T *)(h.data() + at); }
+    template <class T> T *dev(uint64_t at) const { return (T *)(d + at); }
+    cudaError_t alloc(LaunchScratch &S) { return S.alloc(d, h.size()); }
+    cudaError_t upload(cudaStream_t st) const { return cudaMemcpyAsync(d, h.data(), h.size(), cudaMemcpyHostToDevice, st); }
+};
+
+// The partitions a call of several jobs works on, and the job of each (a job may have several).  add() refuses a partition on
+// another engine than the first one's (e); twice() finds a partition that two jobs share.
+struct JobPartitions {
+    Engine *e = nullptr;
+    std::vector<std::pair<Partition *, uint32_t>> seen;
+    bool add(Partition &p, uint32_t job)
+    {
+        if (!e) e = p.eng;
+        seen.emplace_back(&p, job);
+        return p.eng == e;
+    }
+    // true when a partition is in two jobs: a < b are the jobs of the first such partition by address
+    bool twice(uint32_t &a, uint32_t &b)
+    {
+        std::sort(seen.begin(), seen.end());
+        for (size_t x = 1; x < seen.size(); x++)
+            if (seen[x].first == seen[x - 1].first) { a = seen[x - 1].second; b = seen[x].second; return true; }
+        return false;
+    }
+};
+// Every partition of ps locked, in address order: calls that lock several partitions take them in this one order, so that two
+// of them never wait for each other.  Held until the result goes out of scope.
+inline std::vector<std::unique_lock<std::mutex>> lock_partitions(std::vector<Partition *> ps)
+{
+    std::sort(ps.begin(), ps.end());
+    std::vector<std::unique_lock<std::mutex>> held;
+    for (Partition *p : ps) held.emplace_back(p->mu);
+    return held;
+}
+
+// How many CTAs of kernel (threads per CTA, dyn bytes of dynamic shared memory) the device runs at once, at least one per SM,
+// and how many lane groups of G threads they hold: the walkers size their segments by the groups, and loop over them with the CTAs.
+struct Resident { uint64_t ctas, groups; };
+template <class K> inline cudaError_t resident(const Engine &e, K kernel, uint32_t threads, uint32_t G, size_t dyn, Resident &r)
+{
+    int occ = 0;
+    const cudaError_t ce = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, (int)threads, dyn);
+    r.ctas = (uint64_t)std::max(1, occ) * e.sm_count;
+    r.groups = r.ctas * (threads / G);
+    return ce;
 }
 
 } // namespace pgs

@@ -587,8 +587,8 @@ inline int32_t split_many_plan(SplitParams *S, const CompactTotals *T, uint32_t 
     return PGS_OK;
 }
 
-// The scratch of a joint split, every buffer through buf(pointer, elements, fill, out = false) as split_buffers hands them out,
-// in an order that depends only on the plan (the library sizes an arena with one pass and hands it out with a second).
+// The scratch of a joint split, every buffer through buf(pointer, elements, fill, out = false) as split_buffers hands them out.
+// buf may place them later (the library's one allocation): nothing here reads a pointer it was given.
 template <class F>
 inline void split_many_buffers(SplitParams *S, uint32_t n, SplitJobs &J, F &&buf)
 {
@@ -597,14 +597,23 @@ inline void split_many_buffers(SplitParams *S, uint32_t n, SplitJobs &J, F &&buf
     buf(J.stats, n * C, kNoFill, false); // the caller sets every one to merge_stats_init()
     buf(J.prefixes, n * C, 0, false);
     buf(J.dropped, n, 0, false);
+    for (uint32_t i = 0; i < n; i++) split_scratch(S[i], buf);
+}
+
+// The counting phase's tables of a joint split, once split_many_buffers' buffers are placed: every job gets its slice of the
+// launch's counters, job[i] = S[i].M (the planner kernels' jobs), and seg_base / blk_base their prefixes (compact_many_bases).
+inline void split_many_tables(SplitParams *S, uint32_t n, const SplitJobs &J, MergeParams *job, uint32_t *seg_base, uint32_t *blk_base)
+{
+    const uint64_t C = J.S;
     for (uint32_t i = 0; i < n; i++) {
-        split_scratch(S[i], buf);
         S[i].stats = J.stats + i * C;
         S[i].prefixes = J.prefixes + i * C;
         S[i].dropped = J.dropped + i;
         S[i].M.stats = S[i].stats;
         S[i].M.ticket = nullptr; // the launch's tickets are J's
+        job[i] = S[i].M;
     }
+    compact_many_bases(job, n, seg_base, blk_base);
 }
 
 // Child c of job S's k_seg_scan_many / k_emit_many parameters: split_child and split_child_scratch, and the emit shape every
@@ -618,6 +627,32 @@ inline bool split_many_child(const SplitParams &S, uint32_t c, const MergeStats 
     return !shape || (Pc.KS == shape->KS && Pc.blk_buf == shape->blk_buf && Pc.emit_warp_smem == shape->emit_warp_smem &&
                       Pc.emit_obuf == shape->emit_obuf && Pc.ks_stage == shape->ks_stage && geo.emit_warps == shape_geo->emit_warps &&
                       geo.emit_dyn == shape_geo->emit_dyn);
+}
+
+// The children of a joint split after its counting pass (st, prefixes: [n * S] as read back): every (job x, child c) that is
+// built and got records, in that order, becomes one job of k_emit_many -- Pc its parameters, emit_base [Pc.size() + 1] the
+// prefixes of their segments, shape the emit shape they share.  out(x, c, P, geo, T) gives the child's run its buffers
+// (compact_buffers' `out` ones) and returns false to stop.  Returns false when a child is refused (at = x * S + c) or out stopped.
+template <class Out>
+inline bool split_many_children(const SplitParams *S, uint32_t n, const MergeStats *st, const unsigned long long *prefixes, uint32_t max_smem,
+                                std::vector<MergeParams> &Pc, std::vector<uint32_t> &emit_base, CompactGeometry &shape, uint64_t &at, Out &&out)
+{
+    const uint32_t NC = n ? S[0].S : 0;
+    emit_base.assign(1, 0);
+    for (uint32_t x = 0; x < n; x++)
+        for (uint32_t c = 0; c < NC; c++) {
+            at = (uint64_t)x * NC + c;
+            if (!((S[x].want >> c) & 1u) || st[at].cnt[EV_OUT] == 0) continue;
+            MergeParams P{};
+            CompactGeometry g{};
+            CompactTotals T{};
+            if (!split_many_child(S[x], c, st[at], prefixes[at], max_smem, P, g, T, Pc.empty() ? nullptr : &Pc[0], &shape)) return false;
+            if (!out(x, c, P, g, T)) return false;
+            if (Pc.empty()) shape = g;
+            Pc.push_back(P);
+            emit_base.push_back(emit_base.back() + P.Q);
+        }
+    return true;
 }
 
 // The launches of a joint split on stream st.  emit == nullptr: the counting phase (k_plan_many, k_seg_bounds_many,

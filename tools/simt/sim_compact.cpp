@@ -140,6 +140,15 @@ int32_t load_run(HostRun &r, const uint8_t *data, uint64_t data_bytes, const uin
     return build_index(r, nb, max_blk);
 }
 
+int32_t load_runs(uint32_t k, const uint8_t **data, const uint64_t *data_bytes, const uint64_t **blk_off, const uint32_t **blk_size,
+                  const uint32_t *n_blocks, std::vector<HostRun> &runs)
+{
+    runs.resize(k);
+    for (uint32_t i = 0; i < k; i++)
+        if (const int32_t rc = load_run(runs[i], data[i], data_bytes[i], blk_off[i], blk_size[i], n_blocks[i])) return rc;
+    return PGS_OK;
+}
+
 uint64_t crc_tab[256];
 
 struct Merged { // the output of the last sim_compact call
@@ -175,31 +184,20 @@ int32_t sim_compact(uint32_t k, const uint8_t **data, const uint64_t *data_bytes
                     const uint32_t *n_blocks, uint32_t block_size, uint32_t restart_interval, int32_t bottommost,
                     const pgs_filter_params *fp, uint32_t now, uint32_t group_lanes, uint64_t seg_weight, const uint64_t *crc_table)
 {
-    std::vector<HostRun> runs(k);
+    std::vector<HostRun> runs;
+    if (const int32_t rc = load_runs(k, data, data_bytes, blk_off, blk_size, n_blocks, runs)) return rc;
+    if (crc_table) memcpy(crc_tab, crc_table, sizeof crc_tab); else crc64_make_table(crc_tab);
     MergeParams P{};
-    P.k = k;
     CompactTotals T{};
-    for (uint32_t i = 0; i < k; i++) {
-        if (const int32_t rc = load_run(runs[i], data[i], data_bytes[i], blk_off[i], blk_size[i], n_blocks[i])) return rc;
-        P.runs[i] = runs[i].dev();
-        T.add(runs[i].info, runs[i].n_bloom_entries);
-    }
-    P.block_size = block_size;
-    P.restart_interval = restart_interval;
-    P.bottommost = bottommost ? 1 : 0;
-    P.now = now;
-    P.data_version = fp ? fp->data_version : 1;
-    HostMem scratch;
     uint32_t n = 0;
-    if (!compact_filter(P, fp, n)) return PGS_INVALID_ARGUMENT;
+    if (const int32_t rc = compact_job_params(P, T, k, [&](uint32_t i) -> const HostRun & { return runs[i]; }, block_size, restart_interval, bottommost,
+                                              now, fp ? fp->data_version : 1, fp, (const unsigned long long *)crc_tab, n, "sim_compact:"))
+        return rc;
+    HostMem scratch;
     if (n) {
         uint8_t *ops;
         memcpy(host_alloc(scratch, ops, n, 0), fp->ops, n);
         P.ops = ops;
-    }
-    if (P.validate_hash) {
-        if (crc_table) memcpy(crc_tab, crc_table, sizeof crc_tab); else crc64_make_table(crc_tab);
-        P.crc_table = (const unsigned long long *)crc_tab;
     }
     CompactGeometry geo{};
     if (group_lanes && group_lanes != 1 && group_lanes != 2 && group_lanes != 4 && group_lanes != 8 && group_lanes != 16) return PGS_INVALID_ARGUMENT;
@@ -232,9 +230,8 @@ int32_t sim_compact_many(uint32_t n, const uint32_t *k, const uint8_t **data, co
     *launches = 0;
     uint32_t total = 0;
     for (uint32_t i = 0; i < n; i++) total += k[i];
-    std::vector<HostRun> runs(total);
-    for (uint32_t i = 0; i < total; i++)
-        if (const int32_t rc = load_run(runs[i], data[i], data_bytes[i], blk_off[i], blk_size[i], n_blocks[i])) return rc;
+    std::vector<HostRun> runs;
+    if (const int32_t rc = load_runs(total, data, data_bytes, blk_off, blk_size, n_blocks, runs)) return rc;
     if (group_lanes && group_lanes != 1 && group_lanes != 2 && group_lanes != 4 && group_lanes != 8 && group_lanes != 16) return PGS_INVALID_ARGUMENT;
     crc64_make_table(crc_tab);
     HostMem scratch;
@@ -243,25 +240,17 @@ int32_t sim_compact_many(uint32_t n, const uint32_t *k, const uint8_t **data, co
     uint32_t any_hash = 0;
     for (uint32_t i = 0, r = 0; i < n; r += k[i], i++) {
         if (k[i] == 0) return PGS_INVALID_ARGUMENT;
-        if (k[i] > kMaxRuns) return PGS_NOT_SUPPORTED;
-        P[i].k = k[i];
-        for (uint32_t x = 0; x < k[i]; x++) {
-            P[i].runs[x] = runs[r + x].dev();
-            T[i].add(runs[r + x].info, runs[r + x].n_bloom_entries);
-        }
-        P[i].block_size = block_size;
-        P[i].restart_interval = restart_interval;
-        P[i].bottommost = bottommost[i] ? 1 : 0;
-        P[i].now = now;
-        P[i].data_version = fp[i].data_version;
         uint32_t len = 0;
-        if (!compact_filter(P[i], &fp[i], len)) return PGS_INVALID_ARGUMENT;
+        if (const int32_t rc = compact_job_params(P[i], T[i], k[i], [&](uint32_t x) -> const HostRun & { return runs[r + x]; }, block_size,
+                                                  restart_interval, bottommost[i], now, fp[i].data_version, &fp[i],
+                                                  (const unsigned long long *)crc_tab, len, "sim_compact_many:"))
+            return rc;
         if (len) {
             uint8_t *ops;
             memcpy(host_alloc(scratch, ops, len, 0), fp[i].ops, len);
             P[i].ops = ops;
         }
-        if (P[i].validate_hash) { P[i].crc_table = (const unsigned long long *)crc_tab; any_hash = 1; }
+        if (P[i].validate_hash) any_hash = 1;
     }
     MergeJobs M{};
     CompactGeometry shared{};
@@ -378,15 +367,6 @@ int32_t sim_run_index(const uint8_t *data, uint64_t data_bytes, const uint64_t *
     if (ikeys) memcpy(ikeys, r.d_ikeys, std::min<uint64_t>(ikeys_cap, r.d_ikey_off[n_blocks]));
     if (rec_off) memcpy(rec_off, r.d_rec_off, 4 * std::min<uint64_t>(rec_cap, r.d_blk_rec[n_blocks]));
     if (bloom) copy_bloom(r, bloom, bloom_cap);
-    return PGS_OK;
-}
-
-static int32_t load_runs(uint32_t k, const uint8_t **data, const uint64_t *data_bytes, const uint64_t **blk_off, const uint32_t **blk_size,
-                      const uint32_t *n_blocks, std::vector<HostRun> &runs)
-{
-    runs.resize(k);
-    for (uint32_t i = 0; i < k; i++)
-        if (const int32_t rc = load_run(runs[i], data[i], data_bytes[i], blk_off[i], blk_size[i], n_blocks[i])) return rc;
     return PGS_OK;
 }
 
@@ -724,9 +704,8 @@ int32_t sim_split_many(uint32_t n, const uint8_t **data, const uint64_t *data_by
     split_many_buffers(SP.data(), n, J, host_count_buffers(scratch));
     for (uint64_t y = 0; y < (uint64_t)n * NC; y++) J.stats[y] = merge_stats_init();
     std::vector<MergeParams> MP(n);
-    for (uint32_t i = 0; i < n; i++) MP[i] = SP[i].M;
     std::vector<uint32_t> seg_base(n + 1), blk_base(n + 1);
-    compact_many_bases(MP.data(), n, seg_base.data(), blk_base.data());
+    split_many_tables(SP.data(), n, J, MP.data(), seg_base.data(), blk_base.data());
     M.job = MP.data();
     M.seg_base = J.seg_base = seg_base.data();
     M.blk_base = blk_base.data();
@@ -745,23 +724,17 @@ int32_t sim_split_many(uint32_t n, const uint8_t **data, const uint64_t *data_by
             if (R.st[c].error) { fprintf(stderr, "sim_split_many: run %u: counting pass status %u (child %u)\n", i, R.st[c].error, c); return (int32_t)R.st[c].error; }
     }
     std::vector<MergeParams> Pc;
-    std::vector<uint32_t> emit_base(1, 0);
+    std::vector<uint32_t> emit_base;
     CompactGeometry shape{};
-    for (uint32_t i = 0; i < n; i++)
-        for (uint32_t c = 0; c < NC; c++) {
-            Split &R = g_split_many[i];
-            if (!((want[i] >> c) & 1u) || R.st[c].cnt[EV_OUT] == 0) continue;
-            MergeParams P{};
-            CompactGeometry g{};
-            CompactTotals Tc{};
-            if (!split_many_child(SP[i], c, R.st[c], SP[i].prefixes[c], smem, P, g, Tc, Pc.empty() ? nullptr : &Pc[0], &shape)) return PGS_NOT_SUPPORTED;
-            HostRun &run = R.child[c];
-            compact_buffers(P, g, Tc, run, [&](auto *&p, uint64_t cnt, int fill, bool out) { if (out) host_count_buffers(run.mem)(p, cnt, fill); });
-            if (Pc.empty()) shape = g;
-            Pc.push_back(P);
-            emit_base.push_back(emit_base.back() + P.Q);
-            R.built[c] = 1;
-        }
+    uint64_t at = 0;
+    if (!split_many_children(SP.data(), n, J.stats, J.prefixes, smem, Pc, emit_base, shape, at,
+                             [&](uint32_t x, uint32_t c, MergeParams &P, const CompactGeometry &g, const CompactTotals &Tc) {
+                                 HostRun &run = g_split_many[x].child[c];
+                                 compact_buffers(P, g, Tc, run, [&](auto *&p, uint64_t cnt, int fill, bool out) { if (out) host_count_buffers(run.mem)(p, cnt, fill); });
+                                 g_split_many[x].built[c] = 1;
+                                 return true;
+                             }))
+        return PGS_NOT_SUPPORTED;
     if (!Pc.empty()) {
         MergeJobs E{};
         E.job = Pc.data();
